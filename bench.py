@@ -51,6 +51,13 @@ def workload_config(n_gpus):
             'l2': 'GPU arm: L2 flushed between timed steps (256 MiB memset outside the timed spans); CPU arm: not applicable'}
 
 
+def dump_outputs(path, arrays):
+    """One float32 .npy per array (the gradient and the parameters are 6.6 MB each)."""
+    os.makedirs(path, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(path, name + '.npy'), t.detach().float().cpu().numpy())
+
+
 def percentile_stats(ms):
     a = np.sort(np.asarray(ms, dtype=np.float64))
     return {'median': float(np.median(a)), 'p90': float(a[min(len(a) - 1, int(math.ceil(0.9 * len(a))) - 1)]),
@@ -63,7 +70,8 @@ def measured_peaks():
         p = json.load(open(path))
         return {'hbm_gbs': p['hbm_gbs'], 'bf16_tflops': p['bf16_tflops'],
                 'bf16_tflops_sustained': p.get('bf16_tflops_sustained', p['bf16_tflops']), 'source': 'measured'}
-    return {'hbm_gbs': 6650.0, 'bf16_tflops': 1590.0, 'bf16_tflops_sustained': 1400.0, 'source': 'fallback'}
+    # H100 SXM data sheet (dense, 700 W); a card at a lower power limit reaches less
+    return {'hbm_gbs': 3350.0, 'bf16_tflops': 989.0, 'bf16_tflops_sustained': 989.0, 'source': 'H100 SXM data sheet'}
 
 
 class ClockSampler:
@@ -232,9 +240,14 @@ def main():
     ap.add_argument('--no-extra', action='store_true')
     ap.add_argument('--no-graph', action='store_true')
     ap.add_argument('--cpu-budget', type=float, default=15.0, help='seconds of CPU work for the cpu_baseline sample')
+    ap.add_argument('--dump-outputs', metavar='DIR',
+                    help='after the timed steps, write what the last timed step computed (loss, gradient, updated '
+                         'parameters) as DIR/<name>.npy (float32)')
     ap.add_argument('--nccl-allreduce', action='store_true',
                     help='N>1: NCCL all-reduce + local Adam instead of the fused peer-memory optimiser step')
     args = ap.parse_args()
+    if args.impl == 'reference' and args.dump_outputs:
+        ap.error('--dump-outputs writes the outputs of the GPU path; it is not available with --impl reference')
     world = int(os.environ.get('WORLD_SIZE', '1'))
     rank = int(os.environ.get('RANK', '0'))
     local_rank = int(os.environ.get('LOCAL_RANK', '0'))
@@ -290,7 +303,7 @@ def main():
     net._arena.grad = grad
     batches = [synthetic.gum_batch(rng, BATCH) for _ in range(4)]
     encs = [b.encode(net) for b in batches]
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 50 MB L2
     stream = torch.cuda.current_stream()
 
     def barrier():
@@ -373,6 +386,10 @@ def main():
         run_step(i)
         ev[i][1].record(stream)
     barrier()
+    if args.dump_outputs and rank == 0:
+        # the step's graph zeroes the gradient, runs forward + backward and applies Adam: after the last timed step the
+        # buffers hold its loss, its gradient and the parameters it produced
+        dump_outputs(args.dump_outputs, {'loss': loss.view(1), 'grad': grad[:nparams], 'params': net._arena.data[:nparams]})
     # graph replays bypass the library's host-side launch counter: count the launches of one eager step
     l0 = _lib.call('ppb_launch_count')
     device_step(0)
@@ -521,7 +538,7 @@ def main():
 
 def scoring_rooflines(dev, peaks):
     """HBM roofline of the scoring / sampling / normalisation kernels at a saturating size (2^24 particles,
-    per-particle parameters: every operand array is 64 MiB, the working set is far beyond the 126 MB L2).
+    per-particle parameters: every operand array is 64 MiB, the working set is far beyond the 50 MB L2).
     achieved = algorithmic bytes per particle (SURVEY 8d) x N / CUDA-event time."""
     from pyprob_b200 import ops
     n, K, C = 1 << 24, 10, 8
@@ -572,7 +589,7 @@ def scoring_rooflines(dev, peaks):
 
 def gate_gemm_saturating(dev, peaks):
     """The LSTM gate GEMM shape at a saturating batch (one recurrent step of 4096 traces: [4096,512] x [512,2048]^T)
-    through the production tcgen05 kernel: achieved tensor throughput vs the tf32 roofline."""
+    through the production wgmma kernel: achieved tensor throughput vs the tf32 roofline."""
     from pyprob_b200 import _lib
     from pyprob_b200._lib import call, ptr, stream
     M, N, K = 4096, 2048, 512
@@ -611,7 +628,7 @@ def gate_gemm_saturating(dev, peaks):
 
 def committed_traffic(key):
     """DRAM bytes per launch (dram__bytes_read.sum + dram__bytes_write.sum) of a kernel class from the committed
-    `ncu --set full` capture (profiles/ncu_traffic.json, written by scripts/summarise_ncu.py), or None."""
+    `ncu --set full` capture (profiles/ncu_traffic.json, written by scripts/summarise_ncu.py), or None when there is none."""
     path = os.path.join(ROOT, 'profiles', 'ncu_traffic.json')
     if not os.path.exists(path):
         return None

@@ -1,5 +1,5 @@
 /*
- * pyprob_b200 — C-ABI of the B200-native inference-compilation hot path.
+ * pyprob_b200 — C-ABI of the H100-native inference-compilation hot path.
  *
  * This header is the drop-in boundary (SURVEY.md §8b).  pyprob has no FFI of its own: the
  * reference reaches its arithmetic through Python calls into torch.  Every entry point below
@@ -36,8 +36,7 @@ extern "C" {
 
 const char* ppb_last_error(void);
 int ppb_version(void);
-/* Compute capability major*10+minor of the current device; the library refuses (PPB_ENOTSUP) to run
- * tensor-core paths on anything but sm_100. */
+/* Compute capability major*10+minor of the current device (90 on an H100; the kernels are built for sm_90a only). */
 int ppb_device_arch(void);
 /* Number of kernels this library has launched in the calling process (bench.py's gpu_launches). */
 int64_t ppb_launch_count(void);
@@ -380,16 +379,16 @@ int ppb_ic_train_step_host(ppb_net* net, float* arena, float* grad_arena, float*
                            int32_t* status_host, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * 6. Tensor-core building blocks exposed for tests (tcgen05 / TMEM / bulk-TMA; sm_100a only)
- *    pack : row-major fp32 X[rows, K] (leading dim ldx) -> UMMA-ready K-major SWIZZLE_128B tile
+ * 6. Tensor-core building blocks exposed for tests (wgmma / bulk-TMA; sm_90a only)
+ *    pack : row-major fp32 X[rows, K] (leading dim ldx) -> wgmma-ready K-major SWIZZLE_128B tile
  *           images (tf32 hi and lo parts), see DESIGN.md §4.
  *    gemm : C[M,N] (ldc) = A[M,K] * B[N,K]^T (+ bias[N]) (relu) from packed images, 3xTF32 or TF32.
  * ---------------------------------------------------------------------------------------------- */
 int64_t ppb_packed_floats(int64_t rows, int64_t K);
 int ppb_pack_tf32(const float* X, int64_t rows, int64_t K, int64_t ldx, float* hi_out, float* lo_out,
                   void* stream);
-/* Same geometry, MN-major swizzle pattern (SWIZZLE_128B_BASE32B): the operand form whose reduction runs along
- * the image rows (weight-gradient and input-gradient GEMMs).  See DESIGN.md section 4. */
+/* Same geometry, MN-major swizzle pattern (32-byte chunks permuted by (c ^ (row & 3))): the operand form whose reduction
+ * runs along the image rows (weight-gradient and input-gradient GEMMs; the GEMM kernels rewrite it K-major in shared memory).  See DESIGN.md section 4. */
 int ppb_pack_tf32_mn(const float* X, int64_t rows, int64_t K, int64_t ldx, float* hi_out, float* lo_out,
                      void* stream);
 int ppb_gemm_packed(const float* A_hi, const float* A_lo, const float* B_hi, const float* B_lo,

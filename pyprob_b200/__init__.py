@@ -1,4 +1,4 @@
-"""pyprob_b200 — B200-native inference-compilation hot path of pyprob (see DESIGN.md).
+"""pyprob_b200 — H100-native inference-compilation hot path of pyprob (see DESIGN.md).
 
 ``import pyprob_b200 as pyprob`` gives the reference's public names for the importance-sampling path:
 Model, sample/observe/tag/factor, the enums, and ``pyprob_b200.distributions``.

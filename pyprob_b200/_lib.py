@@ -1,6 +1,6 @@
 """ctypes binding of the C-ABI in include/pyprob_b200.h.
 
-The shared library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_100a).  There is no CPU
+The shared library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_90a).  There is no CPU
 fallback: if the library is missing, or an entry point fails, the call raises.
 """
 import ctypes as C
@@ -101,7 +101,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise RuntimeError('pyprob_b200: native library not found at {} — run `python -c "import __graft_entry__ as g; '
-                           'g.build()"` (nvcc, sm_100a). There is no CPU fallback.'.format(LIB_PATH))
+                           'g.build()"` (nvcc, sm_90a). There is no CPU fallback.'.format(LIB_PATH))
     lib = C.CDLL(LIB_PATH)
     for name, argtypes in _SIGNATURES.items():
         try:
@@ -147,4 +147,4 @@ def stream():
 
 def require_cuda():
     if not torch.cuda.is_available():
-        raise RuntimeError('pyprob_b200 needs a CUDA device (sm_100a); there is no CPU fallback')
+        raise RuntimeError('pyprob_b200 needs a CUDA device (sm_90a: H100); there is no CPU fallback')

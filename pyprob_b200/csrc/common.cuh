@@ -1,4 +1,4 @@
-// Shared helpers for the pyprob_b200 CUDA sources (sm_100a only).
+// Shared helpers for the pyprob_b200 CUDA sources (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -7,7 +7,7 @@
 
 #include "../../include/pyprob_b200.h"
 
-#define PPB_NUM_SMS 148  // B200: 2 dies x 74 SMs; grids are sized in multiples of this
+#define PPB_NUM_SMS 132  // H100 SXM; grids are sized in multiples of this
 
 void ppb_set_error(const char* fmt, ...);
 
@@ -43,9 +43,8 @@ extern unsigned long long g_ppb_launches;  // kernels launched by this library (
 // ---- programmatic dependent launch (PDL) -----------------------------------------------------------------------------------
 // A kernel launched with the programmatic-stream-serialisation attribute may START (block scheduling, shared-memory carve-out,
 // its own prologue) while its predecessor in the stream is still running; ppb_pdl_wait() then blocks until the predecessor
-// grid has completed and its writes are visible.  Between two dependent graph nodes the B200 leaves about 2 us idle
-// (profiles/r02d_phase_stamps_*: "start +2016 ns after previous end"), and the tensor-core kernels spend another ~1 us on
-// barrier init / TMEM allocation / descriptor fetch: both are hidden behind the predecessor's tail this way.
+// grid has completed and its writes are visible.  The launch gap between two dependent kernels and the tensor-core
+// kernels' prologue (barrier init, descriptor fetch) are hidden behind the predecessor's tail this way.
 // Rules kept by every converted kernel: before ppb_pdl_wait() it reads nothing but its host-uploaded descriptor table and
 // writes nothing to global memory; ppb_pdl_trigger() comes first so that the successor can be scheduled as early as possible
 // (the hardware launches it only after EVERY block of this grid has started, so it cannot starve this grid of SMs).

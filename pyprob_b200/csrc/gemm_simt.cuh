@@ -2,7 +2,7 @@
 //   C[gm(m), n] (op)= act( sum_k A(gm(m), ka(k)) * B(n, kb(k)) + bias[n] )
 // with arbitrary strides (so NT / NN / TN forms share one kernel), optional row gather on M and
 // independent gathers on K for A and B.  Exact-fp32 cross-check path and the workhorse for the small
-// / ragged GEMMs of the proposal network; the large GEMMs run on tcgen05 (tc_*.cu).
+// / ragged GEMMs of the proposal network; the large GEMMs run on wgmma (tc_*.cuh).
 #pragma once
 #include "common.cuh"
 

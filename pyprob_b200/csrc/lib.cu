@@ -17,8 +17,7 @@ void ppb_set_error(const char* fmt, ...) {
 
 // read at every launch (a getenv per eager launch; graph replays do not come here) so that tests can flip it in-process.
 // PPB_PDL = 0: off; 1 (default): tensor-core kernels and the element-wise kernels between them (cell, pack, NLL); 2: also the
-// observe-MLP backward kernels; 3: also Adam (2 + 3 together measured 10 us SLOWER on the configs[1] step: their early-resident
-// blocks take SMs from the side-stream branches; profiles/r02f_ab_pdl.txt)
+// observe-MLP backward kernels; 3: also Adam (early-resident blocks of levels 2 and 3 take SMs from the side-stream branches)
 int ppb_pdl_level() {
   const char* e = getenv("PPB_PDL");
   return (e && e[0] >= '0' && e[0] <= '9') ? e[0] - '0' : 1;

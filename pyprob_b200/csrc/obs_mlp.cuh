@@ -197,8 +197,7 @@ inline size_t smem_bytes_bwd() { return (size_t)(4 * TB * LD) * sizeof(float); }
 
 // =====================================================================================================================
 // Warp-per-trace variant (default for narrow layers).  The kernels above synchronise the whole CTA twice per layer and
-// pay one global atomic per weight per 4-trace CTA in the backward pass (measured on B200 at B = 256: 12.5 us forward,
-// 30 us backward for ~5 MFLOP).  Here every weight matrix is staged ONCE per CTA in shared memory, each warp walks the
+// pay one global atomic per weight per 4-trace CTA in the backward pass.  Here every weight matrix is staged ONCE per CTA in shared memory, each warp walks the
 // whole layer chain of its traces with warp-level synchronisation only, and the weight gradients are a separate,
 // atomic-free reduction over traces (k_dw): dW[n][k] = sum_b dy[b][n] x[b][k].
 // =====================================================================================================================

@@ -67,7 +67,7 @@ struct Sink {
 
 // ---- two-parameter families ---------------------------------------------------------------------
 // MUFU approximations (<= 2 ulp): the scoring kernels are bound by instruction issue, not HBM, as soon as they carry an IEEE
-// division or a libm logf/expf (ncu: profiles/r02c_ncu_scoring.md); results stay within 1e-6 relative of the libm forms.
+// division or a libm logf/expf; results stay within 1e-6 relative of the libm forms.
 __device__ __forceinline__ float fast_rcp(float x) { float r; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
 __device__ __forceinline__ float fast_ex2(float x) { float r; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
 __device__ __forceinline__ float fast_lg2(float x) { float r; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
@@ -184,15 +184,15 @@ __global__ void __launch_bounds__(kThreads) k_categorical(const float* __restric
 //   logsumexp_k(log w_k + log N(v; mu_k, sigma_k)) = max_k(-z_k^2 / 2) + log sum_k (w_k / sigma_k) exp(-z_k^2 / 2 - max) - log sqrt(2 pi)
 // (truncated components: sigma_k -> sigma_k Z_k, and -inf outside [low, high]): one exp and one reciprocal per component and
 // ONE log per particle instead of two logs, an exp and two divisions per component — these kernels are bound by the
-// transcendental/ALU rate, not by HBM (ncu: profiles/).  Same value as the reference's formula up to fp32 rounding.
+// transcendental/ALU rate, not by HBM.  Same value as the reference's formula up to fp32 rounding.
 // EXACT: K == KMAX is known at compile time (the component loops carry no k < K predicates)
 template <int KMAX, bool TRUNC, bool EXACT = false>
 __device__ __forceinline__ float mixture_row(float v, const float* __restrict__ m, const float* __restrict__ s,
                                              const float* __restrict__ p, int K_rt, float lo, float hi) {
   const int K = EXACT ? KMAX : K_rt;
   // Reciprocals, the exponentials and the final log use the hardware approximations (MUFU.RCP / EX2 / LG2: <= 2 ulp on the
-  // terms that matter — exp arguments are <= 0 and the largest term is exp(0) = 1 exactly): with IEEE divisions and expf the
-  // kernel issued 660 instructions per particle at K = 10 and was issue-bound at 0.72 of HBM (profiles/r02c_ncu_scoring.md).
+  // terms that matter — exp arguments are <= 0 and the largest term is exp(0) = 1 exactly): IEEE divisions and expf make the
+  // kernel issue-bound well below HBM bandwidth.
   float pk[KMAX], a[KMAX], scale[KMAX];
   float psum = 0.0f;
 #pragma unroll

@@ -1,6 +1,5 @@
-// tcgen05 / TMEM / mbarrier / bulk-TMA primitives for sm_100a (inline PTX; no CUTLASS dependency).
-// Bit layouts follow the PTX ISA "tcgen05" matrix / instruction descriptors (cross-checked against the
-// field comments of CUTLASS cute/arch/mma_sm100_desc.hpp shipped in this image).
+// wgmma / mbarrier / bulk-TMA primitives for sm_90a (inline PTX; no CUTLASS dependency).
+// Bit layouts follow the PTX ISA "wgmma" shared-memory matrix descriptor.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -11,7 +10,7 @@ namespace tc {
 // A matrix X[rows, K] is stored as tiles of 128 rows x 32 fp32 (one 128-byte swizzle span along K):
 //   tile(rt, kb) at float offset (rt * KB + kb) * 4096, KB = ceil(K/32)
 //   inside a tile: 16 atoms of 8 rows x 128 B; row rr of an atom holds its eight 16-byte chunks at
-//   chunk position (c ^ rr)  -> exactly the shared-memory image tcgen05.mma expects, so a tile moves
+//   chunk position (c ^ rr)  -> exactly the shared-memory image wgmma expects, so a tile moves
 //   HBM -> SMEM with one linear cp.async.bulk (no tensor map needed).
 constexpr int kTileRows = 128;
 constexpr int kTileK = 32;                       // fp32 elements per 128-byte swizzle span
@@ -24,10 +23,10 @@ __host__ __device__ __forceinline__ int64_t packed_offset(int64_t row, int64_t k
   return (rt * KB + kb) * kTileFloats + atom * 256 + rr * 32 + ((c ^ rr) << 2) + j;
 }
 
-// MN-major flavour of the same tile (tf32 operands whose reduction runs along the image ROWS must use the
-// SWIZZLE_128B_BASE32B pattern — "for mn-major tf32 operands, SW128_32B is the only available smem layout"):
-// same geometry (row r at byte r*128 of the tile), but the four 32-byte chunks of a row are permuted by
-// (c32 ^ (r & 3)) instead of the eight 16-byte chunks by (c16 ^ (r & 7)).
+// MN-major flavour of the same tile (for tensors whose reduction runs along the image ROWS): same geometry (row r at
+// byte r*128 of the tile), but the four 32-byte chunks of a row are permuted by (c32 ^ (r & 3)) instead of the eight
+// 16-byte chunks by (c16 ^ (r & 7)).  tf32 wgmma reads K-major operands only, so the GEMM kernels rewrite an MN-major
+// stage into the K-major image in shared memory before the MMAs (tcg::stage_to_kmajor).
 __host__ __device__ __forceinline__ int64_t packed_offset_mn(int64_t row, int64_t k, int64_t KB) {
   int64_t rt = row >> 7, r = row & 127, kb = k >> 5, kk = k & 31;
   int64_t c32 = kk >> 3, j = kk & 7;
@@ -71,87 +70,36 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
                : "memory");
 }
 
-// ---- TMEM ------------------------------------------------------------------------------------------
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "n"(NCOLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {  // whole warp (the allocating one)
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-__device__ __forceinline__ void fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// 32 lanes x 32 columns of fp32: thread l of the warp gets TMEM lane (lane_base + l), columns [col, col+32)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,"
-      "%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// ---- descriptors -----------------------------------------------------------------------------------
-// Shared-memory matrix descriptor, K-major, SWIZZLE_128B, dense 8-row atoms (SBO = 1024 B, LBO = 16 B).
+// ---- wgmma (sm_90a warpgroup MMA) --------------------------------------------------------------------
+// Shared-memory matrix descriptor, K-major, SWIZZLE_128B, dense 8-row atoms (SBO = 1024 B; LBO unused for SW128 K-major).
+// The swizzle is applied to absolute address bits, so a descriptor may start 32/64/96 B into a 1024-aligned atom row:
+// that is how the four k8 steps of a 32-element chunk are addressed (+2 in the 16-byte start-address field per step).
 __device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);  // start address   bits [0,14)
   d |= (uint64_t)1 << 16;                        // leading byte offset (16 B >> 4), unused for SW128 K-major
   d |= (uint64_t)(1024 >> 4) << 32;              // stride byte offset: next 8-row atom
-  d |= (uint64_t)1 << 46;                        // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                        // layout type SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                        // layout type SWIZZLE_128B
   return d;
-}
-// MN-major operand over the same tile image: the 128-byte swizzle span runs along M/N (32 fp32) and the
-// 8 rows of an atom are 8 consecutive K indices.  LBO = byte distance between consecutive 32-element
-// M/N blocks, SBO = distance between 8-row K groups (one tf32 MMA consumes exactly one group).
-__device__ __forceinline__ uint64_t smem_desc_sw128_mn(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;   // between 32-element M/N blocks
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;   // between 4-row K groups (512 B in the tile image)
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)1 << 61;                             // layout type SWIZZLE_128B_BASE32B
-  return d;
-}
-// Instruction descriptor for kind::tf32, fp32 accumulate; a_mn / b_mn select MN-major operands.
-__host__ __device__ constexpr uint32_t idesc_tf32(int M, int N, int a_mn = 0, int b_mn = 0) {
-  return (1u << 4)                      // D format F32
-         | (2u << 7)                    // A format TF32
-         | (2u << 10)                   // B format TF32
-         | ((uint32_t)a_mn << 15)       // A major: 0 = K, 1 = MN
-         | ((uint32_t)b_mn << 16)       // B major
-         | ((uint32_t)(N >> 3) << 17)   // N / 8
-         | ((uint32_t)(M >> 4) << 24);  // M / 16
 }
 
-__device__ __forceinline__ void mma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                         uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// D[64 x 64] += A[64 x 8] B[64 x 8]^T, tf32 operands K-major in shared memory, fp32 accumulators in registers.
+// Fragment: thread (warp w of the warpgroup, lane l) holds d[4 i + j] = D(16 w + l / 4 + 8 (j >> 1), 8 i + 2 (l % 4) + (j & 1)).
+__device__ __forceinline__ void wgmma_tf32_m64n64k8(float (&d)[32], uint64_t a_desc, uint64_t b_desc) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
+      "setp.ne.b32 p, 1, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a_desc), "l"(b_desc)
       : "memory");
-}
-// Arrive on an mbarrier once all previously issued MMAs of this thread have completed.
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
 }
 
 __device__ __forceinline__ bool elect_one() {

@@ -1,11 +1,11 @@
-// Cluster split-K tcgen05 GEMM: small-M problems spread over the SMs without atomics.
+// Cluster split-K wgmma GEMM: small-M problems spread over the SMs without atomics.
 //
 // The proposal network's per-time-step GEMMs have few rows (one minibatch: M = 256 .. 512) and a deep reduction
 // (K = 512 forward, K = 2048 in BPTT).  One 128 x 128 tile per CTA leaves most SMs idle and makes one CTA walk the whole
 // reduction at the per-SM operand-ingest rate (measured ~100 GB/s: 0.64 us per 32-element chunk in 3xTF32); global
 // split-K (tc_grouped.cuh) fixes the parallelism but pays one fp32 red.add per element per split (measured 33 us for the
 // 512 x 512 x 2048 BPTT GEMM, 9.4 MB of atomics).  Here the CS splits of one output tile form a thread-block CLUSTER:
-// every CTA accumulates its K-slice in TMEM, parks the fp32 partial tile in its own shared memory (the operand stages
+// every CTA accumulates its K-slice in registers, parks the fp32 partial tile in its own shared memory (the operand stages
 // are idle by then), and after a cluster barrier each CTA reduces 128 / CS rows of the tile over all partials through
 // distributed shared memory (ld.shared::cluster) and runs the epilogue for those rows only.  No atomics, no zero-fill,
 // fixed summation order, and the epilogue work is spread over the cluster too.
@@ -15,7 +15,7 @@
 //   k_cluster<X3, CS, 2>   tile images (+fp32, ReLU-mask from an image)          head hidden layer and its gradient
 //   k_lstm_cluster<X3, CS> LSTM cell: with gate-interleaved W_hh the four columns of a thread are the gates i, f, g, o
 //                          of ONE hidden unit, so the cell update is thread-local (tc_lstm.cuh has the layout)
-// Mainloop, descriptors, the three-accumulator 3xTF32 scheme: tc_grouped.cuh.
+// Mainloop, descriptors, the 3xTF32 scheme: tc_grouped.cuh.
 #pragma once
 #include "tc_grouped.cuh"
 #include "tc_lstm.cuh"
@@ -25,10 +25,8 @@ namespace tcc {
 using namespace tc;
 
 // Parked partial tile: 128 rows x 128 floats, row r at byte 512 r, the eight 16-byte chunks of every 128-byte segment permuted
-// by (chunk ^ (r & 7)).  The park phase (thread = row) writes 16-byte vectors — four lanes share a bank group, the minimum for a
-// 512-byte warp store — and a reduce-phase warp reads one whole, 128-byte ALIGNED segment of one row per request: with the
-// former odd pitch (129 floats) every remote read straddled two segments and distributed shared memory delivered 8-9 B/clk
-// per SM instead of the ~17 it is good for (profiles/r02d_phase_stamps_gum.txt).
+// by (chunk ^ (r & 7)), so that a reduce-phase warp reads one whole, 128-byte ALIGNED segment of one row per request (an odd
+// pitch would make every remote read straddle two segments of distributed shared memory).
 constexpr int kPitch = 128;
 constexpr int kPartFloats = 128 * kPitch;    // 64 KB, aliases the operand stages
 static_assert(kPartFloats * 4 <= 2 * tcg::kStages * kTileBytes, "partial tile must fit in the A stages");
@@ -84,8 +82,6 @@ struct __align__(1024) Smem {
   float b_lo[tcg::kStages][kTileFloats];
   uint64_t full[tcg::kStages];
   uint64_t empty[tcg::kStages];
-  uint64_t tmem_full;
-  uint32_t tmem_base;
   union { tcg::Problem prob; tcl::Step step; BStep bstep; };
 };
 inline size_t smem_bytes() { return sizeof(Smem) + 1024; }
@@ -105,9 +101,10 @@ inline size_t smem_bytes() { return sizeof(Smem) + 1024; }
 // Called by all threads; returns after the first cluster barrier (every partial of the cluster is readable).
 template <bool X3>
 __device__ __forceinline__ void mainloop_and_park(Smem& sm, const tcg::Operand& A, const tcg::Operand& B, int mt, int nt,
-                                                  int c0, int c1, uint32_t tmem, int warp, int lane,
+                                                  int c0, int c1, int warp, int lane,
                                                   unsigned long long* trace = nullptr, int b_prefetched = 0) {
-  if (warp == 0) {
+  const tcg::Ring R{sm.a_hi[0], sm.a_lo[0], sm.b_hi[0], sm.b_lo[0], kTileFloats, tcg::kStages, sm.full, sm.empty};
+  if (warp == tcg::kProducerWarp) {
     if (lane == 0) {
       const uint32_t bytes = (tcg::stage_bytes(A, mt) + tcg::stage_bytes(B, nt)) * (X3 ? 2u : 1u);
       for (int c = c0; c < c1; ++c) {
@@ -120,71 +117,18 @@ __device__ __forceinline__ void mainloop_and_park(Smem& sm, const tcg::Operand& 
         if (!b_there) tcg::load_operand(B, nt, c, sm.b_hi[s], sm.b_lo[s], X3, &sm.full[s]);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = idesc_tf32(128, tcg::kBN, A.mn, B.mn);
-      const bool amn = A.mn != 0, bmn = B.mn != 0;
-      for (int c = c0; c < c1; ++c) {
-        int s = (c - c0) % tcg::kStages;
-        uint32_t ph = ((c - c0) / tcg::kStages) & 1;
-        mbar_wait(&sm.full[s], ph);
-        if (c == c0) TCC_TRACE(2);
-        fence_after_sync();
-        uint32_t sa_hi = smem_u32(sm.a_hi[s]), sa_lo = smem_u32(sm.a_lo[s]);
-        uint32_t sb_hi = smem_u32(sm.b_hi[s]), sb_lo = smem_u32(sm.b_lo[s]);
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) {
-          uint64_t ah = tcg::operand_desc(amn, sa_hi, ks), bh = tcg::operand_desc(bmn, sb_hi, ks);
-          if (X3) {
-            uint64_t al = tcg::operand_desc(amn, sa_lo, ks), bl = tcg::operand_desc(bmn, sb_lo, ks);
-            mma_tf32(tmem + 2 * tcg::kBN, al, bh, idesc, (c == c0 && ks == 0) ? 0u : 1u);
-            mma_tf32(tmem + 2 * tcg::kBN, ah, bl, idesc, 1u);
-            mma_tf32(tmem + (c & 1) * tcg::kBN, ah, bh, idesc, (c - c0 < 2 && ks == 0) ? 0u : 1u);
-          } else {
-            mma_tf32(tmem, ah, bh, idesc, (c == c0 && ks == 0) ? 0u : 1u);
-          }
-        }
-        mma_commit(&sm.empty[s]);
-      }
-      mma_commit(&sm.tmem_full);
-      TCC_TRACE(3);
-    }
   } else {
-    // thread = TMEM lane = row of the tile; 32 consecutive columns per load
-    const int q = warp & 3, cb = (warp - 2) >> 2;
+    float acc[32];
+    tcg::mma_mainloop<X3>(R, 0, c1 - c0, A.mn != 0, B.mn != 0, warp, lane, acc);
+    if (threadIdx.x == 0) TCC_TRACE(3);
     float* part = reinterpret_cast<float*>(sm.a_hi);
-    mbar_wait(&sm.tmem_full, 0);
+    tcg::consumer_sync();   // every warpgroup is done reading the A stages
     if (threadIdx.x == 64) TCC_TRACE(4);
-    fence_after_sync();
-    float v[32];
-    if (c1 > c0) {
-      tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + (X3 ? (c0 & 1) * tcg::kBN : 0) + cb * 32, v);
-      if (X3) {
-        float u[32];
-        if (c1 - c0 > 1) {
-          tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + ((c0 & 1) ^ 1) * tcg::kBN + cb * 32, u);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] += u[j];
-        }
-        tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + 2 * tcg::kBN + cb * 32, u);
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] += u[j];
-      }
-    } else {
-#pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] = 0.0f;
-    }
-    const int prow = q * 32 + lane;
-    const uint32_t dst = smem_u32(part + prow * kPitch + cb * 32);
-#pragma unroll
-    for (int j4 = 0; j4 < 8; ++j4)
-      asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(dst + 16 * (j4 ^ (prow & 7))), "f"(v[4 * j4]),
-                   "f"(v[4 * j4 + 1]), "f"(v[4 * j4 + 2]), "f"(v[4 * j4 + 3])
-                   : "memory");
+    tcg::store_acc(acc, warp, lane, [&](int r, int c) {
+      return part + r * kPitch + (c & ~31) + ((((c >> 2) & 7) ^ (r & 7)) << 2) + (c & 3);
+    });
   }
-  fence_before_sync();
   cluster_sync_all();
-  fence_after_sync();
   if (threadIdx.x == 64) TCC_TRACE(7);
 }
 
@@ -204,16 +148,12 @@ __device__ __forceinline__ void reduce_row(const Smem& sm, int row, int lane, fl
 }
 
 __device__ __forceinline__ void common_setup(Smem& sm, int warp, int lane, bool pdl_wait = true) {
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < tcg::kStages; ++s) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], 1); }
-    mbar_init(&sm.tmem_full, 1);
+  if (warp == tcg::kProducerWarp && lane == 0) {
+    for (int s = 0; s < tcg::kStages; ++s) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], tcg::kEpiWarps); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<tcg::kTmemCols>(&sm.tmem_base);
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  // PDL (common.cuh): up to here only the host-uploaded descriptor table, shared memory and TMEM were touched
+  // PDL (common.cuh): up to here only the host-uploaded descriptor table and shared memory were touched
   ppb_pdl_trigger();
   if (pdl_wait) ppb_pdl_wait();
 }
@@ -243,13 +183,12 @@ __global__ void __launch_bounds__(tcg::kThreads, 1) k_cluster(const tcg::Problem
   const int KC = (P.K + 31) / 32;
   const int c0 = (int)((int64_t)KC * split / CS), c1 = (int)((int64_t)KC * (split + 1) / CS);
   common_setup(sm, warp, lane);
-  const uint32_t tmem = sm.tmem_base;
   if (threadIdx.x == 0) TCC_TRACE(1);
-  mainloop_and_park<X3>(sm, P.a, P.b, mt, nt, c0, c1, tmem, warp, lane, trace);
+  mainloop_and_park<X3>(sm, P.a, P.b, mt, nt, c0, c1, warp, lane, trace);
 
-  if (warp >= 2) {
+  if (warp < tcg::kEpiWarps) {
     constexpr int kRowsPerCta = 128 / CS, kRowsPerWarp = kRowsPerCta / tcg::kEpiWarps;
-    const int ew = warp - 2;
+    const int ew = warp;
     const bool do_relu = (P.flags & tcg::kRelu) != 0, do_mask = (P.flags & tcg::kMaskImg) != 0;
     const int m_valid = (P.flags & tcg::kZeroInvalid) ? P.m_valid : P.M;
     float bias[4];
@@ -321,13 +260,8 @@ __global__ void __launch_bounds__(tcg::kThreads, 1) k_cluster(const tcg::Problem
     }
   }
   if (threadIdx.x == 64) TCC_TRACE(5);
-  fence_before_sync();
   cluster_sync_all();
   if (threadIdx.x == 0) TCC_TRACE(6);
-  if (warp == 1) {
-    fence_after_sync();
-    tmem_dealloc<tcg::kTmemCols>(tmem);
-  }
   if (threadIdx.x == 0 && trace && blockIdx.x == 0) {
     const int dm[3] = {P.M, P.N, P.K};
     trace[13] = 1ull + CS * 16;
@@ -363,13 +297,12 @@ __global__ void __launch_bounds__(tcg::kThreads, 1) k_lstm_cluster(const tcl::St
   const int KC = (io.H + 31) / 32;
   const int c0 = (int)((int64_t)KC * split / CS), c1 = (int)((int64_t)KC * (split + 1) / CS);
   common_setup(sm, warp, lane, false);
-  const uint32_t tmem = sm.tmem_base;
   if (threadIdx.x == 0) TCC_TRACE(1);
   // The W_hh tiles of the first stages do not depend on the previous time step (the images are packed once per training step,
   // before the chain of step kernels starts): the producer requests them BEFORE the PDL wait, so that only the h_{t-1} tiles
   // remain to be fetched once the previous step's kernel has finished.
   int b_pre = 0;
-  if (warp == 0 && lane == 0) {
+  if (warp == tcg::kProducerWarp && lane == 0) {
     const uint32_t bytes = (tcg::stage_bytes(P.a, mt) + tcg::stage_bytes(P.b, nt)) * (X3 ? 2u : 1u);
     b_pre = (c1 - c0) < tcg::kStages ? (c1 - c0) : tcg::kStages;
     if (P.io.no_b_prefetch) b_pre = 0;
@@ -383,19 +316,19 @@ __global__ void __launch_bounds__(tcg::kThreads, 1) k_lstm_cluster(const tcl::St
   // epilogue warps fetch it while the mainloop runs instead of after the cluster barrier.
   constexpr int kRowsPerCta = 128 / CS, kRowsPerWarp = kRowsPerCta / tcg::kEpiWarps;
   int m_tr[kRowsPerWarp], m_st[kRowsPerWarp], m_rp[kRowsPerWarp];
-  if (warp >= 2) {
+  if (warp < tcg::kEpiWarps) {
 #pragma unroll
     for (int rr = 0; rr < kRowsPerWarp; ++rr) {
-      const int64_t row = (int64_t)P.row0 + mt * 128 + split * kRowsPerCta + (warp - 2) * kRowsPerWarp + rr;
+      const int64_t row = (int64_t)P.row0 + mt * 128 + split * kRowsPerCta + warp * kRowsPerWarp + rr;
       m_tr[rr] = __ldg(io.row_trace + row);
       m_st[rr] = __ldg(io.row_step + row);
       m_rp[rr] = (int)__ldg(io.row_prev + row);
     }
   }
-  mainloop_and_park<X3>(sm, P.a, P.b, mt, nt, c0, c1, tmem, warp, lane, trace, b_pre);
+  mainloop_and_park<X3>(sm, P.a, P.b, mt, nt, c0, c1, warp, lane, trace, b_pre);
 
-  if (warp >= 2) {
-    const int ew = warp - 2;
+  if (warp < tcg::kEpiWarps) {
+    const int ew = warp;
     const int H = io.H, H4 = 4 * io.H, S = io.S;
     const int u = nt * 32 + lane;     // hidden unit of this lane
     float wsmp[4][SMAX];
@@ -473,13 +406,8 @@ __global__ void __launch_bounds__(tcg::kThreads, 1) k_lstm_cluster(const tcl::St
     }
   }
   if (threadIdx.x == 64) TCC_TRACE(5);
-  fence_before_sync();
   cluster_sync_all();
   if (threadIdx.x == 0) TCC_TRACE(6);
-  if (warp == 1) {
-    fence_after_sync();
-    tmem_dealloc<tcg::kTmemCols>(tmem);
-  }
   if (threadIdx.x == 0 && trace && blockIdx.x == 0) {
     const int dm[3] = {P.M, 4 * io.H, io.H};
     trace[13] = 2ull + CS * 16;
@@ -514,23 +442,22 @@ __global__ void __launch_bounds__(tcg::kThreads, 1) k_lstm_bwd_cluster(const BSt
   const int KC = H4 / 32;
   const int c0 = (int)((int64_t)KC * split / CS), c1 = (int)((int64_t)KC * (split + 1) / CS);
   common_setup(sm, warp, lane);
-  const uint32_t tmem = sm.tmem_base;
   // row metadata while the mainloop runs (it heads the dependency chain of the reduce phase)
   constexpr int kRowsPerCta = 128 / CS, kRowsPerWarp = kRowsPerCta / tcg::kEpiWarps;
   int m_tr[kRowsPerWarp], m_nx[kRowsPerWarp], m_rp[kRowsPerWarp];
-  if (warp >= 2) {
+  if (warp < tcg::kEpiWarps) {
 #pragma unroll
     for (int rr = 0; rr < kRowsPerWarp; ++rr) {
-      const int64_t row = (int64_t)P.row0 + mt * 128 + split * kRowsPerCta + (warp - 2) * kRowsPerWarp + rr;
+      const int64_t row = (int64_t)P.row0 + mt * 128 + split * kRowsPerCta + warp * kRowsPerWarp + rr;
       m_tr[rr] = __ldg(io.row_trace + row);
       m_nx[rr] = __ldg(io.row_next + row);
       m_rp[rr] = (P.t > 0) ? __ldg(io.row_prev + row) : 0;
     }
   }
-  mainloop_and_park<X3>(sm, P.a, P.b, mt, nt, c0, c1, tmem, warp, lane);
+  mainloop_and_park<X3>(sm, P.a, P.b, mt, nt, c0, c1, warp, lane);
 
-  if (warp >= 2) {
-    const int ew = warp - 2;
+  if (warp < tcg::kEpiWarps) {
+    const int ew = warp;
     // descriptor fields in registers (P sits in shared memory behind a generic pointer, every io.x would be a dependent load)
     const float* const g_gates = io.gates; const float* const g_c = io.c; const float* const g_dh = io.dh;
     float* const g_dc = io.dc; float* const g_dp = io.d_pobs; float* const g_dg = io.dgates;
@@ -604,12 +531,7 @@ __global__ void __launch_bounds__(tcg::kThreads, 1) k_lstm_bwd_cluster(const BSt
       }
     }
   }
-  fence_before_sync();
   cluster_sync_all();
-  if (warp == 1) {
-    fence_after_sync();
-    tmem_dealloc<tcg::kTmemCols>(tmem);
-  }
 }
 
 // host-side launch with a (CS, 1, 1) cluster (and the PDL attribute, common.cuh)

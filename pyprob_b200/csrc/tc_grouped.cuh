@@ -1,4 +1,4 @@
-// Grouped tcgen05 GEMM over packed tile images (the tensor-core workhorse of the proposal network).
+// Grouped wgmma GEMM over packed tile images (the tensor-core workhorse of the proposal network).
 //
 //   C[m, n] (op)= epi( sum_k A(m, k) * B(n, k) )      fp32-faithful 3xTF32 or single-pass TF32
 //
@@ -7,10 +7,10 @@
 //   * MN-major when the reduction runs along the image ROWS    (image columns = M or N index)      [fmt MN]
 // so forward GEMMs, input-gradient GEMMs and weight-gradient GEMMs all read the same row-major tensors
 // without transposed copies (a tensor that is read both ways keeps one image per format).
-// One pipeline stage = 32 reduction elements: a 16 KB tile (K-major) or 4 x 4 KB row pieces (MN-major).
-// Warp roles (576 threads): warp 0 bulk-TMA producer, warp 1 TMEM owner + MMA issuer, warps 2-17 epilogue
-// (a lone warp per scheduler issues ~0.2 instr/clk on dependent code; 16 warps hide that latency).
-// One 128 x 128 output tile per CTA.
+// One pipeline stage = 32 reduction elements: a 16 KB tile (K-major) or 4 x 4 KB row pieces (MN-major, rewritten into
+// the K-major image in shared memory before the MMAs).
+// Warp roles (544 threads): warps 0-15 = four warpgroups, each issuing the wgmma of one 64 x 64 quadrant and then running
+// the epilogue of a 32 x 32 block; warp 16 bulk-TMA producer.  One 128 x 128 output tile per CTA.
 #pragma once
 #include "common.cuh"
 #include "tc.cuh"
@@ -61,11 +61,14 @@ struct Problem {
 };
 
 constexpr int kStages = 3;
-constexpr int kEpiWarps = 16;                     // 4 TMEM lane quadrants x 4 column chunks: one 32 x 32 block per warp
-constexpr int kThreads = 64 + 32 * kEpiWarps;     // + bulk-TMA producer warp + MMA/TMEM warp
+constexpr int kEpiWarps = 16;                     // = the MMA warps: four warpgroups, one 64 x 64 quadrant of the tile each
+constexpr int kProducerWarp = kEpiWarps;          // bulk-TMA producer
+constexpr int kThreads = 32 * (kEpiWarps + 1);
+constexpr int kConsumerThreads = 32 * kEpiWarps;
 constexpr int kBN = 128;
-constexpr int kTmemCols = 512;
 constexpr int kPiece = 32 * 128;  // bytes: 32 rows x 128 B
+constexpr int kCPitch = 129;      // fp32 result tile in shared memory: row r at float r * 129 (row and column reads conflict-free)
+constexpr int kCFloats = 128 * kCPitch;
 
 struct __align__(1024) Smem {
   float a_hi[kStages][kTileFloats];
@@ -74,13 +77,10 @@ struct __align__(1024) Smem {
   float b_lo[kStages][kTileFloats];
   uint64_t full[kStages];
   uint64_t empty[kStages];
-  uint64_t tmem_full;
-  uint32_t tmem_base;
   Problem prob;  // on-chip copy of the descriptor
 };
-// The epilogue warps transpose their blocks through the operand stages, which are idle once the last MMA has
-// completed (16 warps x 32 x 33 floats = 66 KB <= the 96 KB of a_hi + a_lo).
-static_assert(kEpiWarps * 32 * 33 * 4 <= 2 * kStages * kTileBytes, "transpose buffers must fit in the A stages");
+// The result tile is parked in the B stages, which are idle once the last MMA has completed.
+static_assert(kCFloats * 4 <= 2 * kStages * kTileBytes, "result tile must fit in the B stages");
 
 __device__ __forceinline__ uint32_t stage_bytes(const Operand& o, int tile_idx) {
   if (!o.mn) return kTileBytes;
@@ -110,8 +110,120 @@ __device__ __forceinline__ void load_operand(const Operand& o, int tile_idx, int
   }
 }
 
-__device__ __forceinline__ uint64_t operand_desc(bool mn, uint32_t smem_addr, int ks) {
-  return mn ? smem_desc_sw128_mn(smem_addr + ks * 1024, kPiece, 512) : smem_desc_sw128(smem_addr) + (uint64_t)(ks * 2);
+// named barrier of the 16 MMA / epilogue warps (ids 1-4 are the LSTM epilogue's quadrant barriers)
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 5, %0;" ::"n"(kConsumerThreads) : "memory"); }
+
+// An MN-major stage (four pieces of 32 reduction rows x 32 M/N columns, chunks permuted by (c32 ^ (k & 3))) is rewritten in
+// place into the K-major SWIZZLE_128B image of its 128 M/N rows, which is what tf32 wgmma reads.  Consecutive threads walk
+// along M/N, so the reads are conflict-free and the writes 4-way.
+__device__ __forceinline__ void stage_to_kmajor(float* const (&t)[4], int n, int tid) {
+  float v[4][8];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+    if (i < n)
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const int idx = tid + kConsumerThreads * e, r = idx & 127, k = idx >> 7;
+        v[i][e] = t[i][(r >> 5) * 1024 + k * 32 + ((((r & 31) >> 3) ^ (k & 3)) << 3) + (r & 7)];
+      }
+  consumer_sync();
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+    if (i < n)
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const int idx = tid + kConsumerThreads * e, r = idx & 127, k = idx >> 7;
+        t[i][r * 32 + (((k >> 2) ^ (r & 7)) << 2) + (k & 3)] = v[i][e];
+      }
+  fence_proxy_async();   // generic-proxy writes, read next by wgmma (async proxy)
+  consumer_sync();
+}
+
+// Operand stage ring: stage s of operand X at X + s * stride.
+struct Ring {
+  float* a_hi; float* a_lo; float* b_hi; float* b_lo;
+  int stride, stages;
+  uint64_t* full; uint64_t* empty;
+};
+
+// Mainloop of the 16 consumer warps over n chunks (ring positions kc0 .. kc0 + n - 1) of one 128 x 128 output tile.
+// Warpgroup g computes the quadrant rows 64 (g & 1), columns 64 (g >> 1) into acc (fragment layout of
+// wgmma_tf32_m64n64k8).  Each 32-element chunk is accumulated by the tensor core into a zeroed register tile and then added
+// to acc in fp32 with round-to-nearest, so the tensor core's truncating accumulation only ever spans 4 (TF32) or 12
+// (3xTF32: cross terms first, then hi * hi) products of one chunk.  The empty barrier of a stage expects one arrival per
+// consumer warp.
+template <bool X3>
+__device__ __forceinline__ void mma_mainloop(const Ring& R, uint32_t kc0, int n, bool amn, bool bmn, int warp, int lane,
+                                             float (&acc)[32]) {
+  const int tid = warp * 32 + lane;
+  const uint32_t a_off = (uint32_t)((warp >> 2) & 1) * 8192u, b_off = (uint32_t)(warp >> 3) * 8192u;
+#pragma unroll
+  for (int j = 0; j < 32; ++j) acc[j] = 0.0f;
+  for (int i = 0; i < n; ++i) {
+    const uint32_t kc = kc0 + (uint32_t)i;
+    const int s = (int)(kc % (uint32_t)R.stages);
+    const uint32_t ph = (kc / (uint32_t)R.stages) & 1;
+    float* const ah_p = R.a_hi + s * R.stride; float* const al_p = R.a_lo + s * R.stride;
+    float* const bh_p = R.b_hi + s * R.stride; float* const bl_p = R.b_lo + s * R.stride;
+    mbar_wait(&R.full[s], ph);
+    if (amn || bmn) {
+      float* t[4] = {nullptr, nullptr, nullptr, nullptr};
+      int nt = 0;
+      if (amn) { t[nt++] = ah_p; if (X3) t[nt++] = al_p; }
+      if (bmn) { t[nt++] = bh_p; if (X3) t[nt++] = bl_p; }
+      stage_to_kmajor(t, nt, tid);
+    }
+    float d[32];
+#pragma unroll
+    for (int j = 0; j < 32; ++j) d[j] = 0.0f;
+    const uint64_t ah = smem_desc_sw128(smem_u32(ah_p) + a_off), bh = smem_desc_sw128(smem_u32(bh_p) + b_off);
+    const uint64_t al = smem_desc_sw128(smem_u32(al_p) + a_off), bl = smem_desc_sw128(smem_u32(bl_p) + b_off);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) {
+      if (X3) {
+        wgmma_tf32_m64n64k8(d, al + 2 * ks, bh + 2 * ks);
+        wgmma_tf32_m64n64k8(d, ah + 2 * ks, bl + 2 * ks);
+      }
+      wgmma_tf32_m64n64k8(d, ah + 2 * ks, bh + 2 * ks);
+    }
+    wgmma_commit();
+    wgmma_wait0();
+#pragma unroll
+    for (int j = 0; j < 32; ++j) acc[j] += d[j];
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&R.empty[s]);
+  }
+}
+
+// Write the accumulator fragment of this thread to at(row, col) of the 128 x 128 tile.
+template <class At>
+__device__ __forceinline__ void store_acc(const float (&acc)[32], int warp, int lane, At at) {
+  const int r0 = ((warp >> 2) & 1) * 64 + (warp & 3) * 16 + (lane >> 2), c0 = (warp >> 3) * 64 + 2 * (lane & 3);
+#pragma unroll
+  for (int i = 0; i < 8; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) *at(r0 + 8 * (j >> 1), c0 + 8 * i + (j & 1)) = acc[4 * i + j];
+}
+
+// Bulk-TMA producer: streams n chunks (c0 .. c0 + n - 1, ring positions kc0 ..) of tile (mt, nt) into the ring.
+template <bool X3>
+__device__ __forceinline__ void produce(const Ring& R, const Operand& A, const Operand& B, int mt, int nt, int c0, int n,
+                                        uint32_t kc0) {
+  const uint32_t bytes = (stage_bytes(A, mt) + stage_bytes(B, nt)) * (X3 ? 2u : 1u);
+  for (int i = 0; i < n; ++i) {
+    const uint32_t kc = kc0 + (uint32_t)i;
+    const int s = (int)(kc % (uint32_t)R.stages);
+    const uint32_t ph = (kc / (uint32_t)R.stages) & 1;
+    mbar_wait(&R.empty[s], ph ^ 1);
+    mbar_expect_tx(&R.full[s], bytes);
+    load_operand(A, mt, c0 + i, R.a_hi + s * R.stride, R.a_lo + s * R.stride, X3, &R.full[s]);
+    load_operand(B, nt, c0 + i, R.b_hi + s * R.stride, R.b_lo + s * R.stride, X3, &R.full[s]);
+  }
+}
+
+__device__ __forceinline__ Ring ring_of(Smem& sm) {
+  return Ring{sm.a_hi[0], sm.a_lo[0], sm.b_hi[0], sm.b_lo[0], kTileFloats, kStages, sm.full, sm.empty};
 }
 
 // EPI selects the (compile-time) epilogue flavour so that the row loop is straight-line code:
@@ -149,73 +261,33 @@ __global__ void __launch_bounds__(kThreads, 1) k_grouped(const Problem* __restri
   const int nsplit = P.k_splits > 1 ? P.k_splits : 1;
   const int c0 = (int)((int64_t)KC * split / nsplit), c1 = (int)((int64_t)KC * (split + 1) / nsplit);
 
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < kStages; ++s) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], 1); }
-    mbar_init(&sm.tmem_full, 1);
+  if (warp == kProducerWarp && lane == 0) {
+    for (int s = 0; s < kStages; ++s) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], kEpiWarps); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<kTmemCols>(&sm.tmem_base);
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem = sm.tmem_base;
   if (threadIdx.x == 0) TCG_TRACE(1);
-  // PDL (common.cuh): everything above touched only the host-uploaded descriptor table, shared memory and TMEM
+  // PDL (common.cuh): everything above touched only the host-uploaded descriptor table and shared memory
   ppb_pdl_trigger();
   ppb_pdl_wait();
+  const Ring R = ring_of(sm);
 
-  if (warp == 0) {
-    if (lane == 0) {
-      const uint32_t bytes = (stage_bytes(P.a, mt) + stage_bytes(P.b, nt)) * (X3 ? 2u : 1u);
-      for (int c = c0; c < c1; ++c) {
-        int s = (c - c0) % kStages;
-        uint32_t ph = ((c - c0) / kStages) & 1;
-        mbar_wait(&sm.empty[s], ph ^ 1);
-        mbar_expect_tx(&sm.full[s], bytes);
-        load_operand(P.a, mt, c, sm.a_hi[s], sm.a_lo[s], X3, &sm.full[s]);
-        load_operand(P.b, nt, c, sm.b_hi[s], sm.b_lo[s], X3, &sm.full[s]);
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = idesc_tf32(128, kBN, P.a.mn, P.b.mn);
-      const bool amn = P.a.mn != 0, bmn = P.b.mn != 0;
-      for (int c = c0; c < c1; ++c) {
-        int s = (c - c0) % kStages;
-        uint32_t ph = ((c - c0) / kStages) & 1;
-        mbar_wait(&sm.full[s], ph);
-        if (c == c0) TCG_TRACE(2);
-        fence_after_sync();
-        uint32_t sa_hi = smem_u32(sm.a_hi[s]), sa_lo = smem_u32(sm.a_lo[s]);
-        uint32_t sb_hi = smem_u32(sm.b_hi[s]), sb_lo = smem_u32(sm.b_lo[s]);
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) {
-          uint64_t ah = operand_desc(amn, sa_hi, ks), bh = operand_desc(bmn, sb_hi, ks);
-          if (X3) {
-            uint64_t al = operand_desc(amn, sa_lo, ks), bl = operand_desc(bmn, sb_lo, ks);
-            // three accumulators (see tc_gemm.cu): cross terms, hi*hi of even chunks, hi*hi of odd chunks
-            mma_tf32(tmem + 2 * kBN, al, bh, idesc, (c == c0 && ks == 0) ? 0u : 1u);
-            mma_tf32(tmem + 2 * kBN, ah, bl, idesc, 1u);
-            mma_tf32(tmem + (c & 1) * kBN, ah, bh, idesc, (c - c0 < 2 && ks == 0) ? 0u : 1u);
-          } else {
-            mma_tf32(tmem, ah, bh, idesc, (c == c0 && ks == 0) ? 0u : 1u);
-          }
-        }
-        mma_commit(&sm.empty[s]);
-      }
-      mma_commit(&sm.tmem_full);
-      TCG_TRACE(3);
-    }
+  if (warp == kProducerWarp) {
+    if (lane == 0) produce<X3>(R, P.a, P.b, mt, nt, c0, c1 - c0, 0);
   } else {
-    // Epilogue.  TMEM hands each thread one ROW (32 consecutive columns per load); writing rows straight out would
-    // scatter every store instruction over 32 cache lines (measured: 8.7 us per tile).  Each warp therefore
-    // transposes its 32 x 32 block through shared memory and emits whole 128-byte row spans: lane = column.
-    const int q = warp & 3;                 // TMEM lane quadrant this warp may read
-    const int cb = (warp - 2) >> 2;         // its 32-column chunk of the 128-column tile
-    float (*stg)[33] = reinterpret_cast<float (*)[33]>(reinterpret_cast<float*>(sm.a_hi) + (warp - 2) * 32 * 33);
-    mbar_wait(&sm.tmem_full, 0);
-    if (threadIdx.x == 64) TCG_TRACE(4);
-    fence_after_sync();
+    float acc[32];
+    mma_mainloop<X3>(R, 0, c1 - c0, P.a.mn != 0, P.b.mn != 0, warp, lane, acc);
+    if (threadIdx.x == 0) TCG_TRACE(3);
+    float* const ctile = sm.b_hi[0];
+    consumer_sync();   // every warpgroup is done reading the B stages
+    store_acc(acc, warp, lane, [&](int r, int c) { return ctile + r * kCPitch + c; });
+    consumer_sync();
+    if (threadIdx.x == 0) TCG_TRACE(4);
+    // Epilogue: warp (q, cb) owns rows 32q..32q+31, columns 32cb..32cb+31 of the tile and emits whole 128-byte row spans
+    // (lane = column).
+    const int q = warp & 3;
+    const int cb = warp >> 2;
+    const float* stg = ctile + (q * 32) * kCPitch + cb * 32;
     const int m_base = mt * 128 + q * 32;  // first row of C handled by this warp
     // hoist everything that does not depend on the row out of the (fully unrolled) row loop
     const bool do_relu = (P.flags & kRelu) != 0, do_mask = (P.flags & kMaskImg) != 0;
@@ -229,23 +301,6 @@ __global__ void __launch_bounds__(kThreads, 1) k_grouped(const Problem* __restri
     {
       const int n0 = nt * kBN + cb * 32;
       if (n0 < ((P.N + 31) & ~31) && m_base < P.M) {  // warp-uniform
-      float v[32];
-      tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + (X3 ? (c0 & 1) * kBN : 0) + cb * 32, v);
-      if (X3) {
-        float u[32];
-        if (c1 - c0 > 1) {
-          tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + ((c0 & 1) ^ 1) * kBN + cb * 32, u);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] += u[j];
-        }
-        tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + 2 * kBN + cb * 32, u);
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] += u[j];
-      }
-      __syncwarp();
-#pragma unroll
-      for (int j = 0; j < 32; ++j) stg[lane][j] = v[j];
-      __syncwarp();
       const int n = n0 + lane;
       const bool col_ok = n < P.N;
       const float bias = (bias_p && col_ok) ? __ldg(bias_p + n) : 0.0f;
@@ -255,7 +310,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_grouped(const Problem* __restri
       float* cp = c_p ? c_p + (int64_t)m_base * ldc + n : nullptr;
       const bool c_ok = cp != nullptr && col_ok;
       // rows in batches of eight: the ReLU-mask loads of a batch are issued together (one L2 round trip per batch instead of
-      // one per row — the mask read used to serialise the whole epilogue: 10 us for a one-chunk GEMM)
+      // one per row)
 #pragma unroll
       for (int rb = 0; rb < 32; rb += 8) {
         float mk[8];
@@ -273,7 +328,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_grouped(const Problem* __restri
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           const int r = rb + j;
-          float x = stg[r][lane] + bias;
+          float x = stg[r * kCPitch + lane] + bias;
           x = do_relu ? fmaxf(x, 0.0f) : x;
           const bool live = r < rows;                        // row exists in C
           x = (col_ok && r < valid_rows) ? x : 0.0f;
@@ -299,14 +354,9 @@ __global__ void __launch_bounds__(kThreads, 1) k_grouped(const Problem* __restri
       }
     }
   }
-  if (threadIdx.x == 64) TCG_TRACE(5);
-  fence_before_sync();
+  if (threadIdx.x == 0) TCG_TRACE(5);
   __syncthreads();
   if (threadIdx.x == 0) TCG_TRACE(6);
-  if (warp == 1) {
-    fence_after_sync();
-    tmem_dealloc<kTmemCols>(tmem);
-  }
   if (threadIdx.x == 0 && trace && blockIdx.x == 0) { trace[8] = (unsigned long long)P.M; trace[9] = (unsigned long long)P.N; trace[10] = (unsigned long long)P.K; trace[11] = (unsigned long long)gridDim.x; trace[12] = (unsigned long long)(c1 - c0); }
 }
 

@@ -1,6 +1,6 @@
 // LSTM time step with the cell update fused into the recurrent GEMM's epilogue (DESIGN.md 9, item 1).
 //
-//   pre[:, g*H + u] = h_{t-1} W_hh^T  (tcgen05, 3xTF32 or TF32)  + P_obs[trace] + P_step[segment] + smp_emb W_smp
+//   pre[:, g*H + u] = h_{t-1} W_hh^T  (wgmma, 3xTF32 or TF32)  + P_obs[trace] + P_step[segment] + smp_emb W_smp
 //   i,f,o = sigmoid, g = tanh;  c_t = f c_{t-1} + i g;  h_t = o tanh(c_t)          (torch.nn.LSTM, gate order i,f,g,o)
 //
 // replaces, for t >= 1, the pair (tcg::k_grouped<X3,0> writing fp32 gate pre-activations, k_cell_fwd re-reading
@@ -12,10 +12,10 @@
 // each complete 8 rows of the cell: c, h, and the K-/MN-format tile images of h that the next step, the heads and
 // the weight-gradient GEMMs read.
 //
-// Mainloop, pipeline, descriptors and the three-accumulator 3xTF32 scheme are those of tc_grouped.cuh.
+// Mainloop, pipeline, descriptors and the 3xTF32 scheme are those of tc_grouped.cuh.
 //
-// STATUS: written after the round-1 GPU budget was spent — compiles, never run.  Opt-in: PPB_FUSED_CELL=1 launches
-// k_lstm_step once per time step, PPB_FUSED_CELL=2 runs all steps in one persistent launch (k_lstm_seq).
+// Opt-in: PPB_FUSED_CELL=1 launches k_lstm_step once per time step, PPB_FUSED_CELL=2 runs all steps in one persistent
+// launch (k_lstm_seq).
 #pragma once
 #include "tc_grouped.cuh"
 
@@ -70,45 +70,28 @@ struct __align__(1024) Smem {
   float b_lo[tcg::kStages][kTileFloats];
   uint64_t full[tcg::kStages];
   uint64_t empty[tcg::kStages];
-  uint64_t tmem_full;
-  uint32_t tmem_base;
   union { Step step; Seq seq; };
 };
 static_assert(tcg::kEpiWarps * 32 * 33 * 4 <= 2 * tcg::kStages * kTileBytes, "staging blocks must fit in the A stages");
 
-__device__ __forceinline__ void quad_barrier(int q) {  // the four epilogue warps that share TMEM lane quadrant q
+__device__ __forceinline__ void quad_barrier(int q) {  // the four epilogue warps of 32-row block q
   asm volatile("bar.sync %0, %1;" ::"r"(1 + q), "r"(128) : "memory");
 }
 
 // Epilogue of one 128-row x 32-unit tile: gate activations (phase 1), then the cell update (phase 2).
-// `staging` = base of the idle operand stages; `tile_row0` = global row of the tile's first row.  Called by the 16
-// epilogue warps only, after the accumulators of the step are complete.
-template <bool X3>
-__device__ __forceinline__ void cell_epilogue(float* staging, const CellIO& io, uint32_t tmem, int warp, int lane,
-                                              int KC, int nt, int64_t tile_row0) {
-  const int q = warp & 3;              // TMEM lane quadrant = 32-row block of the tile
-  const int g = (warp - 2) >> 2;       // 32-column chunk of the tile = gate (i, f, g, o)
-  const int qi = (warp - 2) & 3;       // position of this quadrant's warp inside every group of four staging blocks
-  float (*stg)[33] = reinterpret_cast<float (*)[33]>(staging + (warp - 2) * 32 * 33);
+// `staging` = base of the idle A stages, `ctile` = the step's result tile (tcg::kCPitch, in the B stages);
+// `tile_row0` = global row of the tile's first row.  Called by the 16 consumer warps only, after the result tile is complete.
+__device__ __forceinline__ void cell_epilogue(float* staging, const float* ctile, const CellIO& io, int warp, int lane, int nt,
+                                              int64_t tile_row0) {
+  const int q = warp & 3;              // 32-row block of the tile
+  const int g = warp >> 2;             // 32-column chunk of the tile = gate (i, f, g, o)
+  const int qi = q;                    // position of this quadrant's warp inside every group of four staging blocks
+  float (*stg)[33] = reinterpret_cast<float (*)[33]>(staging + warp * 32 * 33);
   const int H = io.H, H4 = 4 * io.H, S = io.S;
   const int u = nt * 32 + lane;        // hidden unit owned by this lane
   const int col = g * H + u;           // its column in the gate-major [.., 4H] arrays
-  float v[32];
-  tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + g * 32, v);
-  if (X3) {
-    float w[32];
-    if (KC > 1) {
-      tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + tcg::kBN + g * 32, w);
 #pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] += w[j];
-    }
-    tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + 2 * tcg::kBN + g * 32, w);
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] += w[j];
-  }
-  __syncwarp();
-#pragma unroll
-  for (int j = 0; j < 32; ++j) stg[lane][j] = v[j];   // thread = row  ->  lane = column
+  for (int r = 0; r < 32; ++r) stg[r][lane] = ctile[(q * 32 + r) * tcg::kCPitch + g * 32 + lane];
   __syncwarp();
   float wsmp[8];
 #pragma unroll
@@ -185,66 +168,25 @@ __global__ void __launch_bounds__(tcg::kThreads, 1) k_lstm_step(const Step* __re
   const int mt = local / P.tiles_n, nt = local % P.tiles_n;   // nt = block of 32 hidden units
   const int KC = (P.io.H + 31) / 32;
 
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < tcg::kStages; ++s) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], 1); }
-    mbar_init(&sm.tmem_full, 1);
+  if (warp == tcg::kProducerWarp && lane == 0) {
+    for (int s = 0; s < tcg::kStages; ++s) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], tcg::kEpiWarps); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<tcg::kTmemCols>(&sm.tmem_base);
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem = sm.tmem_base;
+  const tcg::Ring R{sm.a_hi[0], sm.a_lo[0], sm.b_hi[0], sm.b_lo[0], kTileFloats, tcg::kStages, sm.full, sm.empty};
 
-  if (warp == 0) {
-    if (lane == 0) {
-      const uint32_t bytes = (tcg::stage_bytes(P.a, mt) + tcg::stage_bytes(P.b, nt)) * (X3 ? 2u : 1u);
-      for (int c = 0; c < KC; ++c) {
-        int s = c % tcg::kStages;
-        uint32_t ph = (c / tcg::kStages) & 1;
-        mbar_wait(&sm.empty[s], ph ^ 1);
-        mbar_expect_tx(&sm.full[s], bytes);
-        tcg::load_operand(P.a, mt, c, sm.a_hi[s], sm.a_lo[s], X3, &sm.full[s]);
-        tcg::load_operand(P.b, nt, c, sm.b_hi[s], sm.b_lo[s], X3, &sm.full[s]);
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = idesc_tf32(128, tcg::kBN, 0, 0);
-      for (int c = 0; c < KC; ++c) {
-        int s = c % tcg::kStages;
-        uint32_t ph = (c / tcg::kStages) & 1;
-        mbar_wait(&sm.full[s], ph);
-        fence_after_sync();
-        uint32_t sa_hi = smem_u32(sm.a_hi[s]), sa_lo = smem_u32(sm.a_lo[s]);
-        uint32_t sb_hi = smem_u32(sm.b_hi[s]), sb_lo = smem_u32(sm.b_lo[s]);
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) {
-          uint64_t ah = tcg::operand_desc(false, sa_hi, ks), bh = tcg::operand_desc(false, sb_hi, ks);
-          if (X3) {
-            uint64_t al = tcg::operand_desc(false, sa_lo, ks), bl = tcg::operand_desc(false, sb_lo, ks);
-            mma_tf32(tmem + 2 * tcg::kBN, al, bh, idesc, (c == 0 && ks == 0) ? 0u : 1u);
-            mma_tf32(tmem + 2 * tcg::kBN, ah, bl, idesc, 1u);
-            mma_tf32(tmem + (c & 1) * tcg::kBN, ah, bh, idesc, (c < 2 && ks == 0) ? 0u : 1u);
-          } else {
-            mma_tf32(tmem, ah, bh, idesc, (c == 0 && ks == 0) ? 0u : 1u);
-          }
-        }
-        mma_commit(&sm.empty[s]);
-      }
-      mma_commit(&sm.tmem_full);
-    }
+  if (warp == tcg::kProducerWarp) {
+    if (lane == 0) tcg::produce<X3>(R, P.a, P.b, mt, nt, 0, KC, 0);
   } else {
-    mbar_wait(&sm.tmem_full, 0);
-    fence_after_sync();
-    cell_epilogue<X3>(reinterpret_cast<float*>(sm.a_hi), P.io, tmem, warp, lane, KC, nt, (int64_t)P.row0 + mt * 128);
+    float acc[32];
+    tcg::mma_mainloop<X3>(R, 0, KC, false, false, warp, lane, acc);
+    float* const ctile = sm.b_hi[0];
+    tcg::consumer_sync();
+    tcg::store_acc(acc, warp, lane, [&](int r, int c) { return ctile + r * tcg::kCPitch + c; });
+    tcg::consumer_sync();
+    cell_epilogue(reinterpret_cast<float*>(sm.a_hi), ctile, P.io, warp, lane, nt, (int64_t)P.row0 + mt * 128);
   }
-  fence_before_sync();
   __syncthreads();
-  if (warp == 1) {
-    fence_after_sync();
-    tmem_dealloc<tcg::kTmemCols>(tmem);
-  }
 }
 
 // ---- persistent variant: ALL time steps t >= 1 of every sub-batch in one launch ---------------------------------------------
@@ -284,22 +226,18 @@ __global__ void __launch_bounds__(tcg::kThreads, 1) k_lstm_seq(const Seq* __rest
   const int mt = local / P.tiles_n, nt = local % P.tiles_n;
   const int KC = (P.io.H + 31) / 32;
 
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < tcg::kStages; ++s) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], 1); }
-    mbar_init(&sm.tmem_full, 1);
+  if (warp == tcg::kProducerWarp && lane == 0) {
+    for (int s = 0; s < tcg::kStages; ++s) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], tcg::kEpiWarps); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<tcg::kTmemCols>(&sm.tmem_base);
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem = sm.tmem_base;
+  const tcg::Ring R{sm.a_hi[0], sm.a_lo[0], sm.b_hi[0], sm.b_lo[0], kTileFloats, tcg::kStages, sm.full, sm.empty};
   int* counter = P.progress + P.prog0 + mt;
 
   for (int t = 1; t < P.T; ++t) {
     const int row0 = __ldg(P.row_off + t) + P.seg_off, prev0 = __ldg(P.row_off + t - 1) + P.seg_off;
-    const int cbase = (t - 1) * KC;     // the stage ring and its phases keep running across the steps
-    if (warp == 0) {
+    const uint32_t cbase = (uint32_t)(t - 1) * KC;     // the stage ring and its phases keep running across the steps
+    if (warp == tcg::kProducerWarp) {
       if (lane == 0) {
         if (t > 1) {
           const int target = (t - 1) * P.tiles_n;
@@ -311,60 +249,27 @@ __global__ void __launch_bounds__(tcg::kThreads, 1) k_lstm_seq(const Seq* __rest
         }
         tcg::Operand a = P.a;
         a.row0 = prev0;
-        const uint32_t bytes = (tcg::stage_bytes(a, mt) + tcg::stage_bytes(P.b, nt)) * (X3 ? 2u : 1u);
-        for (int c = 0; c < KC; ++c) {
-          const int cg = cbase + c, s = cg % tcg::kStages;
-          const uint32_t ph = (cg / tcg::kStages) & 1;
-          mbar_wait(&sm.empty[s], ph ^ 1);
-          mbar_expect_tx(&sm.full[s], bytes);
-          tcg::load_operand(a, mt, c, sm.a_hi[s], sm.a_lo[s], X3, &sm.full[s]);
-          tcg::load_operand(P.b, nt, c, sm.b_hi[s], sm.b_lo[s], X3, &sm.full[s]);
-        }
-      }
-    } else if (warp == 1) {
-      if (lane == 0) {
-        const uint32_t idesc = idesc_tf32(128, tcg::kBN, 0, 0);
-        for (int c = 0; c < KC; ++c) {
-          const int cg = cbase + c, s = cg % tcg::kStages;
-          const uint32_t ph = (cg / tcg::kStages) & 1;
-          mbar_wait(&sm.full[s], ph);
-          fence_after_sync();
-          uint32_t sa_hi = smem_u32(sm.a_hi[s]), sa_lo = smem_u32(sm.a_lo[s]);
-          uint32_t sb_hi = smem_u32(sm.b_hi[s]), sb_lo = smem_u32(sm.b_lo[s]);
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-            uint64_t ah = tcg::operand_desc(false, sa_hi, ks), bh = tcg::operand_desc(false, sb_hi, ks);
-            if (X3) {
-              uint64_t al = tcg::operand_desc(false, sa_lo, ks), bl = tcg::operand_desc(false, sb_lo, ks);
-              mma_tf32(tmem + 2 * tcg::kBN, al, bh, idesc, (c == 0 && ks == 0) ? 0u : 1u);
-              mma_tf32(tmem + 2 * tcg::kBN, ah, bl, idesc, 1u);
-              mma_tf32(tmem + (c & 1) * tcg::kBN, ah, bh, idesc, (c < 2 && ks == 0) ? 0u : 1u);
-            } else {
-              mma_tf32(tmem, ah, bh, idesc, (c == 0 && ks == 0) ? 0u : 1u);
-            }
-          }
-          mma_commit(&sm.empty[s]);
-        }
-        mma_commit(&sm.tmem_full);
+        tcg::produce<X3>(R, a, P.b, mt, nt, 0, KC, cbase);
       }
     } else {
-      mbar_wait(&sm.tmem_full, (uint32_t)((t - 1) & 1));
-      fence_after_sync();
-      cell_epilogue<X3>(reinterpret_cast<float*>(sm.a_hi), P.io, tmem, warp, lane, KC, nt, (int64_t)row0 + mt * 128);
+      float acc[32];
+      tcg::mma_mainloop<X3>(R, cbase, KC, false, false, warp, lane, acc);
+      float* const ctile = sm.b_hi[0];
+      tcg::consumer_sync();
+      tcg::store_acc(acc, warp, lane, [&](int r, int c) { return ctile + r * tcg::kCPitch + c; });
+      tcg::consumer_sync();
+      cell_epilogue(reinterpret_cast<float*>(sm.a_hi), ctile, P.io, warp, lane, nt, (int64_t)row0 + mt * 128);
       __threadfence();   // this thread's h / c / image stores are visible device-wide before the arrival below
     }
-    // the accumulators are drained and the staging blocks (aliasing the operand stages) are free again; the next
-    // step's bulk copies (async proxy) overwrite shared memory this step's epilogue wrote through the generic proxy
+    // the staging blocks and the result tile (aliasing the operand stages) are free again; the next step's bulk copies
+    // (async proxy) overwrite shared memory this step's epilogue wrote through the generic proxy
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    fence_before_sync();
     __syncthreads();
-    fence_after_sync();
     if (threadIdx.x == 0) {
       __threadfence();
       atomicAdd(counter, 1);
     }
   }
-  if (warp == 1) tmem_dealloc<tcg::kTmemCols>(tmem);
 }
 
 inline size_t smem_bytes() { return sizeof(Smem) + 1024; }

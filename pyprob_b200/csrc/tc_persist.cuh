@@ -1,16 +1,10 @@
-// Persistent form of the grouped tcgen05 GEMM (tc_grouped.cuh): one CTA per SM walks output tiles blockIdx.x, + gridDim.x, ...
+// Persistent form of the grouped wgmma GEMM (tc_grouped.cuh): one CTA per SM walks output tiles blockIdx.x, + gridDim.x, ...
 //
-// Why: with one tile per CTA every tile pays the prologue (barrier init, TMEM allocation, descriptor fetch, first operand
-// latency: ~2.5 us) and an epilogue during which the tensor pipe idles — 1-2.5 us for a plain fp32 store, 7-10 us for the
-// image epilogue (five words per element at ~32 B/clk of SM store bandwidth).  For a 16-chunk tile (K = 512, 10 us of
-// mainloop) that is half of the time.  Here the roles run free of each other across tiles:
-//   producer   : streams operand chunks of tile after tile into a 2-stage ring (full/empty mbarriers, one running chunk counter)
-//   MMA thread : waits until the accumulators are drained (tmem_empty), issues the tile's MMAs, commits tmem_full
-//   epilogue   : drains TMEM into a DEDICATED staging buffer (16 warps x 32 x 33 floats), releases the accumulators
-//                (tmem_empty) and only then runs the store loop — while the MMAs of the next tile are already running.
-// 3xTF32 needs three accumulators (384 of the 512 TMEM columns), so there is no second accumulator set to ping-pong with;
-// the early release after the drain is what overlaps epilogue and mainloop.  128 KB of operand stages (2 x 64 KB in 3xTF32,
-// 4 x 32 KB single-pass) + 67.6 KB of staging.
+// Why: with one tile per CTA every tile pays the prologue (barrier init, descriptor fetch, first operand latency) and an
+// epilogue during which no operands are in flight.  Here the producer runs free of the consumers across tiles: it streams
+// operand chunks of tile after tile into the stage ring (full/empty mbarriers, one running chunk counter), so the next tile's
+// first stages are loaded while the consumer warps run the previous tile's epilogue out of a DEDICATED result tile.
+// 128 KB of operand stages (2 x 64 KB in 3xTF32, 4 x 32 KB single-pass) + 66 KB result tile.
 // Same Problem descriptors, same arithmetic and the same epilogue flavours as tcg::k_grouped; results are identical.
 #pragma once
 #include "tc_grouped.cuh"
@@ -26,12 +20,9 @@ template <bool X3> struct StageCfg { static constexpr int kStages = X3 ? 2 : 4; 
 constexpr int kMaxStages = 4;
 struct __align__(1024) Smem {
   float ring[8 * kTileFloats];            // 128 KB: stage s at s * kFloats: [a_hi | b_hi | a_lo | b_lo] (lo parts: 3xTF32 only)
-  float stg[tcg::kEpiWarps][32][33];
+  float ctile[tcg::kCFloats];
   uint64_t full[kMaxStages];
   uint64_t empty[kMaxStages];
-  uint64_t tmem_full;
-  uint64_t tmem_empty;
-  uint32_t tmem_base;
 };
 inline size_t smem_bytes() { return sizeof(Smem) + 1024; }
 
@@ -65,89 +56,43 @@ __global__ void __launch_bounds__(tcg::kThreads, 1) k_grouped_persistent(const t
   Smem& sm = *reinterpret_cast<Smem*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   constexpr int kStages = StageCfg<X3>::kStages, kStageFloats = StageCfg<X3>::kFloats;
-  auto st_a_hi = [&](int s) { return sm.ring + s * kStageFloats; };
-  auto st_b_hi = [&](int s) { return sm.ring + s * kStageFloats + kTileFloats; };
-  auto st_a_lo = [&](int s) { return sm.ring + s * kStageFloats + 2 * kTileFloats; };   // 3xTF32 only
-  auto st_b_lo = [&](int s) { return sm.ring + s * kStageFloats + 3 * kTileFloats; };
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < kStages; ++s) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], 1); }
-    mbar_init(&sm.tmem_full, 1);
-    mbar_init(&sm.tmem_empty, tcg::kEpiWarps);
+  const tcg::Ring R{sm.ring, sm.ring + 2 * kTileFloats, sm.ring + kTileFloats, sm.ring + 3 * kTileFloats, kStageFloats, kStages,
+                    sm.full, sm.empty};   // lo parts: 3xTF32 only
+  if (warp == tcg::kProducerWarp && lane == 0) {
+    for (int s = 0; s < kStages; ++s) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], tcg::kEpiWarps); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<tcg::kTmemCols>(&sm.tmem_base);
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem = sm.tmem_base;
   ppb_pdl_trigger();
   ppb_pdl_wait();
 
-  if (warp == 0) {
+  if (warp == tcg::kProducerWarp) {
     if (lane == 0) {
       uint32_t kc = 0;   // chunks issued so far (all tiles)
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const tcg::Problem& P = probs[find_problem(probs, n_probs, tile)];
         const TileGeom g = tile_geom(P, tile);
-        const tcg::Operand A = P.a, B = P.b;
-        const uint32_t bytes = (tcg::stage_bytes(A, g.mt) + tcg::stage_bytes(B, g.nt)) * (X3 ? 2u : 1u);
-        for (int c = g.c0; c < g.c1; ++c, ++kc) {
-          const int s = kc % kStages;
-          const uint32_t ph = (kc / kStages) & 1;
-          mbar_wait(&sm.empty[s], ph ^ 1);
-          mbar_expect_tx(&sm.full[s], bytes);
-          tcg::load_operand(A, g.mt, c, st_a_hi(s), st_a_lo(s), X3, &sm.full[s]);
-          tcg::load_operand(B, g.nt, c, st_b_hi(s), st_b_lo(s), X3, &sm.full[s]);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      uint32_t kc = 0;
-      int it = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-        const tcg::Problem& P = probs[find_problem(probs, n_probs, tile)];
-        const TileGeom g = tile_geom(P, tile);
-        const bool amn = P.a.mn != 0, bmn = P.b.mn != 0;
-        const uint32_t idesc = idesc_tf32(128, tcg::kBN, amn, bmn);
-        // the accumulators are free once the epilogue warps have drained the previous tile (a fresh barrier passes parity 1)
-        mbar_wait(&sm.tmem_empty, (uint32_t)(it & 1) ^ 1u);
-        fence_after_sync();
-        for (int c = g.c0; c < g.c1; ++c, ++kc) {
-          const int s = kc % kStages;
-          const uint32_t ph = (kc / kStages) & 1;
-          mbar_wait(&sm.full[s], ph);
-          fence_after_sync();
-          const uint32_t sa_hi = smem_u32(st_a_hi(s)), sa_lo = smem_u32(st_a_lo(s));
-          const uint32_t sb_hi = smem_u32(st_b_hi(s)), sb_lo = smem_u32(st_b_lo(s));
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-            const uint64_t ah = tcg::operand_desc(amn, sa_hi, ks), bh = tcg::operand_desc(bmn, sb_hi, ks);
-            if (X3) {
-              const uint64_t al = tcg::operand_desc(amn, sa_lo, ks), bl = tcg::operand_desc(bmn, sb_lo, ks);
-              mma_tf32(tmem + 2 * tcg::kBN, al, bh, idesc, (c == g.c0 && ks == 0) ? 0u : 1u);
-              mma_tf32(tmem + 2 * tcg::kBN, ah, bl, idesc, 1u);
-              mma_tf32(tmem + (c & 1) * tcg::kBN, ah, bh, idesc, (c - g.c0 < 2 && ks == 0) ? 0u : 1u);
-            } else {
-              mma_tf32(tmem, ah, bh, idesc, (c == g.c0 && ks == 0) ? 0u : 1u);
-            }
-          }
-          mma_commit(&sm.empty[s]);
-        }
-        mma_commit(&sm.tmem_full);
+        tcg::produce<X3>(R, P.a, P.b, g.mt, g.nt, g.c0, g.c1 - g.c0, kc);
+        kc += (uint32_t)(g.c1 - g.c0);
       }
     }
   } else {
-    const int q = warp & 3;                 // TMEM lane quadrant this warp may read
-    const int cb = (warp - 2) >> 2;         // its 32-column chunk of the 128-column tile
-    float (*stg)[33] = sm.stg[warp - 2];
-    int it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
+    const int q = warp & 3;                 // 32-row block of the tile
+    const int cb = warp >> 2;               // 32-column chunk of the tile
+    const float* stg = sm.ctile + (q * 32) * tcg::kCPitch + cb * 32;
+    uint32_t kc = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       int pi = 0;
       if (lane == 0) pi = find_problem(probs, n_probs, tile);
       pi = __shfl_sync(0xffffffffu, pi, 0);
       const tcg::Problem& P = probs[pi];
       const TileGeom g = tile_geom(P, tile);
+      float acc[32];
+      tcg::mma_mainloop<X3>(R, kc, g.c1 - g.c0, P.a.mn != 0, P.b.mn != 0, warp, lane, acc);
+      kc += (uint32_t)(g.c1 - g.c0);
+      tcg::consumer_sync();   // the previous tile's epilogue is done with the result tile
+      tcg::store_acc(acc, warp, lane, [&](int r, int c) { return sm.ctile + r * tcg::kCPitch + c; });
+      tcg::consumer_sync();
       const int pM = P.M, pN = P.N, flags = P.flags;
       const int m_base = g.mt * 128 + q * 32;
       const bool do_relu = (flags & tcg::kRelu) != 0, do_mask = (flags & tcg::kMaskImg) != 0;
@@ -160,36 +105,7 @@ __global__ void __launch_bounds__(tcg::kThreads, 1) k_grouped_persistent(const t
       const int64_t ldc = P.ldc, o_kb = P.o_kb, orow0 = (int64_t)P.o_row0 + m_base, ocb0 = P.o_col0 / 32 + g.nt * 4;
       const int n0 = g.nt * tcg::kBN + cb * 32;
       const bool work = n0 < ((pN + 31) & ~31) && m_base < pM;   // warp-uniform
-      mbar_wait(&sm.tmem_full, (uint32_t)(it & 1));
-      fence_after_sync();
-      float v[32];
-      if (work) {
-        if (g.c1 > g.c0) {
-          tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + (X3 ? (g.c0 & 1) * tcg::kBN : 0) + cb * 32, v);
-          if (X3) {
-            float u[32];
-            if (g.c1 - g.c0 > 1) {
-              tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + ((g.c0 & 1) ^ 1) * tcg::kBN + cb * 32, u);
-#pragma unroll
-              for (int j = 0; j < 32; ++j) v[j] += u[j];
-            }
-            tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + 2 * tcg::kBN + cb * 32, u);
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] += u[j];
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = 0.0f;
-        }
-      }
-      // the accumulators are in registers: hand TMEM back to the MMA thread before the (long) store loop
-      fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&sm.tmem_empty);
       if (!work) continue;
-#pragma unroll
-      for (int j = 0; j < 32; ++j) stg[lane][j] = v[j];
-      __syncwarp();
       const int n = n0 + lane;
       const bool col_ok = n < pN;
       const float bias = (bias_p && col_ok) ? __ldg(bias_p + n) : 0.0f;
@@ -211,7 +127,7 @@ __global__ void __launch_bounds__(tcg::kThreads, 1) k_grouped_persistent(const t
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           const int r = rb + j;
-          float x = stg[r][lane] + bias;
+          float x = stg[r * tcg::kCPitch + lane] + bias;
           x = do_relu ? fmaxf(x, 0.0f) : x;
           const bool live = r < rows;
           x = (col_ok && r < valid_rows) ? x : 0.0f;
@@ -234,15 +150,9 @@ __global__ void __launch_bounds__(tcg::kThreads, 1) k_grouped_persistent(const t
           }
         }
       }
-      __syncwarp();   // the staging block is overwritten by this warp's next tile
     }
   }
-  fence_before_sync();
   __syncthreads();
-  if (warp == 1) {
-    fence_after_sync();
-    tmem_dealloc<tcg::kTmemCols>(tmem);
-  }
 }
 
 }  // namespace tcp

@@ -33,7 +33,7 @@ for (M, N, R) in [(2048, 64, 256), (271, 512, 256), (2048, 512, 4096)]:
 t = timeit(lambda: torch.empty(1, device=dev).zero_())
 print('torch tiny kernel launch: %.1f us' % t)
 
-# device-side durations (CUPTI) of the bring-up kernel for tiny problems: the fixed cost of one tcgen05 tile
+# device-side durations (CUPTI) of the bring-up kernel for tiny problems: the fixed cost of one tensor-core tile
 from torch.profiler import profile, ProfilerActivity
 for (M, N, K) in [(128, 128, 32), (128, 128, 128), (128, 128, 512), (256, 2048, 64)]:
     a = torch.randn(M, K, device=dev); b = torch.randn(N, K, device=dev); c = torch.empty(M, N, device=dev)

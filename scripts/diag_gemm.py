@@ -1,4 +1,4 @@
-"""Bring-up diagnostic: 3xTF32 / TF32 error of the tcgen05 packed GEMM vs fp64, as a function of shape."""
+"""Bring-up diagnostic: 3xTF32 / TF32 error of the wgmma packed GEMM vs fp64, as a function of shape."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch

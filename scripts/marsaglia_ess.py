@@ -1,23 +1,59 @@
-"""Spread of the Marsaglia IC acceptance statistic (ESS of 8192 proposals) over seeds and training budgets."""
-import os, sys, time
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'tests'))
-import torch
-import pyprob_b200 as pyprob
-from pyprob_b200 import InferenceEngine, InferenceNetwork
-from test_model_gpu import GaussianUnknownMeanMarsaglia
+"""Spread of the Marsaglia IC acceptance statistic (tests/test_model_gpu.py::test_marsaglia_inference_compilation) over seeds.
+
+    python scripts/marsaglia_ess.py [--traces 600000] [--batch 256] [--lstm 128] [--seeds 5 6 7] [--draws 3] [--precision 0]
+
+For every seed: one training run, then --draws independent posteriors of 8192 proposals; prints each draw's ESS, their
+median (what the test holds against the reference floor 0.016 * 8192), the posterior means and the best training loss.
+--precision selects the network arithmetic (0 = 3xTF32 tensor cores, 1 = TF32, 2 = exact-fp32 SIMT GEMMs)."""
+import argparse
+import os
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, 'tests'))
+import pyprob_b200 as pyprob  # noqa: E402
+from pyprob_b200 import InferenceEngine, InferenceNetwork  # noqa: E402
+from pyprob_b200 import network as pnet  # noqa: E402
+from test_model_gpu import GaussianUnknownMeanMarsaglia  # noqa: E402
+
+ap = argparse.ArgumentParser()
+ap.add_argument('--traces', type=int, default=600000)
+ap.add_argument('--batch', type=int, default=256)
+ap.add_argument('--lstm', type=int, default=128)
+ap.add_argument('--seeds', type=int, nargs='+', default=[5, 6, 7])
+ap.add_argument('--draws', type=int, default=3)
+ap.add_argument('--precision', type=int, default=0, choices=[0, 1, 2])
+args = ap.parse_args()
+
+if args.precision:
+    _init = pnet.InferenceNetworkLSTM.__init__
+
+    def _init_with_precision(self, *a, **kw):
+        kw['precision'] = args.precision
+        _init(self, *a, **kw)
+    pnet.InferenceNetworkLSTM.__init__ = _init_with_precision
 
 pyprob.set_verbosity(0)
-for name, kw in (('300k/512/h128', dict(num_traces=300000, batch_size=512, lstm_dim=128)),
-                 ('600k/256/h128', dict(num_traces=600000, batch_size=256, lstm_dim=128)),
-                 ('300k/128/h128', dict(num_traces=300000, batch_size=128, lstm_dim=128))):
-    for seed in (5, 6, 7):
-        pyprob.seed(seed)
-        m = GaussianUnknownMeanMarsaglia()
-        t0 = time.time()
-        m.learn_inference_network(inference_network=InferenceNetwork.LSTM,
-                                  observe_embeddings={'obs0': {'dim': 16}, 'obs1': {'dim': 16}}, **kw)
-        t1 = time.time()
-        post = m.posterior_results(8192, InferenceEngine.IMPORTANCE_SAMPLING_WITH_INFERENCE_NETWORK, observe={'obs0': 8, 'obs1': 9})
-        print('%-16s seed %d: train %.1f s, ESS %.1f (floor %.1f), mean %.3f, loss %.4f' % (
-            name, seed, t1 - t0, post.effective_sample_size, 0.016 * 8192, float(post.mean), m._inference_network._loss_min), flush=True)
+floor = 0.016 * 8192
+print('budget %d traces, batch %d, h %d, precision %d, env %s' % (
+    args.traces, args.batch, args.lstm, args.precision,
+    ' '.join('%s=%s' % kv for kv in sorted(os.environ.items()) if kv[0].startswith('PPB_')) or '-'), flush=True)
+for seed in args.seeds:
+    pyprob.seed(seed)
+    m = GaussianUnknownMeanMarsaglia()
+    t0 = time.time()
+    m.learn_inference_network(num_traces=args.traces, batch_size=args.batch, inference_network=InferenceNetwork.LSTM,
+                              lstm_dim=args.lstm, observe_embeddings={'obs0': {'dim': 16}, 'obs1': {'dim': 16}})
+    t1 = time.time()
+    ess, means = [], []
+    for _ in range(args.draws):
+        post = m.posterior_results(8192, InferenceEngine.IMPORTANCE_SAMPLING_WITH_INFERENCE_NETWORK,
+                                   observe={'obs0': 8, 'obs1': 9})
+        ess.append(float(post.effective_sample_size))
+        means.append(float(post.mean))
+    med = sorted(ess)[len(ess) // 2]
+    print('seed %d: train %.1f s, loss %.4f, ESS %s median %.1f (floor %.1f%s), means %s' % (
+        seed, t1 - t0, m._inference_network._loss_min, ' / '.join('%.1f' % e for e in ess), med, floor,
+        '' if med > floor else ' FAIL', ' / '.join('%.3f' % x for x in means)), flush=True)

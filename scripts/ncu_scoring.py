@@ -1,5 +1,5 @@
 """One launch of every scoring / sampling / normalisation kernel at 2^24 particles (per-particle parameters, every operand
-array 64 MiB: far beyond the 126 MB L2 together) — the target of the `ncu --set full` capture whose dram__bytes and
+array 64 MiB: far beyond the 50 MB L2 together) — the target of the `ncu --set full` capture whose dram__bytes and
 throughput numbers go to profiles/ (scripts/summarise_ncu.py).  Warm-up launches first; ncu is told to skip them."""
 import os
 import sys

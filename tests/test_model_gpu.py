@@ -124,22 +124,23 @@ def test_gum_inference_compilation_end_to_end(cuda, tmp_path):
 def test_marsaglia_inference_compilation(cuda):
     """Reference acceptance (tests/test_inference.py:335-360): posterior mean within 0.75, ESS above 1.6 % of the draws.
     The ESS of an importance sampler is a heavy-tailed statistic (one large weight halves it) and training is not
-    run-to-run reproducible (fp32 reductions with atomics), so the floor is checked on the median of three independent
-    posterior draws of a 600k-trace training run: scripts/marsaglia_ess.py measured 514 / 887 / 1055 for three seeds of this
-    setting against the floor of 131 (profiles/r02d_marsaglia_ess.txt); the shorter 300k run scattered from 64 to 950."""
+    run-to-run reproducible (fp32 reductions with atomics), so the floor is checked on the median of five independent
+    posterior draws of a 600k-trace training run.  scripts/marsaglia_ess.py on an H100 (seeds 5-10, three draws each):
+    per-run medians 416-1711 against the floor of 131, single draws down to 228 (one draw of 36 over three kernel paths
+    fell to 126) — the median over five draws keeps one or two such draws from deciding the test."""
     pyprob.seed(5)
     pyprob.set_verbosity(0)
     model = GaussianUnknownMeanMarsaglia()
     model.learn_inference_network(num_traces=600000, batch_size=256, inference_network=InferenceNetwork.LSTM,
                                   lstm_dim=128, observe_embeddings={'obs0': {'dim': 16}, 'obs1': {'dim': 16}})
     ess, means = [], []
-    for _ in range(3):
+    for _ in range(5):
         post = model.posterior_results(8192, InferenceEngine.IMPORTANCE_SAMPLING_WITH_INFERENCE_NETWORK,
                                        observe={'obs0': 8, 'obs1': 9})
         ess.append(float(post.effective_sample_size))
         means.append(float(post.mean))
-    assert abs(sorted(means)[1] - TRUE_MEAN) < 0.5
-    assert sorted(ess)[1] > 0.016 * 8192, ess  # reference floor: tests/test_inference.py:344
+    assert abs(sorted(means)[2] - TRUE_MEAN) < 0.5
+    assert sorted(ess)[2] > 0.016 * 8192, ess  # reference floor: tests/test_inference.py:344
 
 
 def test_online_minibatches_are_disjoint_between_ranks(cuda, monkeypatch):

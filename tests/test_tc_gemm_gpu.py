@@ -1,4 +1,4 @@
-"""GPU: tcgen05 building blocks — operand packing (bit-exact layout + TF32 split) and the packed GEMM
+"""GPU: tensor-core building blocks — operand packing (bit-exact layout + TF32 split) and the packed GEMM
 against an fp64 CPU matmul.  3xTF32 must be fp32-faithful (<= 2e-6 relative to the fp64 result scale);
 single-pass TF32 is only held to TF32 accuracy."""
 import numpy as np
