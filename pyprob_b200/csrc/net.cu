@@ -169,9 +169,9 @@ Ws carve(const ppb_net* net, Dims d, void* base) {
   w.dh_rec = take((int64_t)d.R * H);
   w.dc = take((int64_t)d.R * H);
   w.d_pobs = take((int64_t)d.B * 4 * H);
-  w.d_pstep = take((int64_t)d.NS * 4 * H);
   w.d_smp = take((int64_t)d.R * S);
   w.d_embcat = take((int64_t)d.NS * C2);
+  w.d_pstep = take((int64_t)d.NS * 4 * H);   // d_pstep and d_obs_emb are adjacent: the tensor-core backward zeroes both at once
   w.d_obs_emb = take((int64_t)d.B * E);
   for (int l = 0; l + 1 < D.obs_final.num_layers; ++l) w.d_fin_act[l] = take((int64_t)d.B * D.obs_final.layers[l].out_dim);
   w.d_obs_cat = take((int64_t)d.B * E);
