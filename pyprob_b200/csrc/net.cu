@@ -41,6 +41,9 @@ struct PackEntry {  // one matrix of the weight-packing table
   int tile_start, pad_;
 };
 
+// how the tensor-core pipeline runs the observe embedding (obs_embed.inc)
+enum class ObsForm { fused, tensor_core, simt };
+
 struct ppb_net {
   // tensor-core path: packed tf32 images of every GEMM weight, refreshed from the arena each forward
   float* wimg = nullptr;
@@ -50,10 +53,10 @@ struct ppb_net {
   int pack_tiles = 0;
   WImg w_ihE, w_hh;
   std::vector<WImg> w1, w2;
-  // wide observe-embedding layers on the tensor cores (layers >= 1 of every observable chain, the final chain)
+  ObsForm obs_form = ObsForm::simt;   // chosen when the tables are set
+  // tensor-core form of the observe embedding: layers >= 1 of every observable chain, the final chain
   WImg w_obs[PPB_MAX_OBS][PPB_MAX_FF_LAYERS];
   WImg w_fin[PPB_MAX_FF_LAYERS];
-  int obs_tc = 0;
   // content hashes of the problem lists last uploaded to each device region: identical lists are not re-sent,
   // which also makes a repeated step capturable in a CUDA graph (no host->device copy inside the capture)
   uint64_t slot_hash[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
@@ -243,39 +246,6 @@ inline Problem linear_dw(const float* dY, int64_t lddy, const float* X, int64_t 
   p.C = dW; p.ldc = ldw;
   p.M = N; p.N = K; p.K = M; p.flags = gemm::kAccumulate;
   return p;
-}
-
-// observe-embedding forward phases (inference_network.py:132-139); one phase per depth level of the
-// per-observable FFs, then one per layer of the final FF
-void add_obs_embed(Builder& bl, const ppb_net_desc& D, const float* arena, const float* obs, int B,
-                   float* const (*obs_act)[PPB_MAX_FF_LAYERS], float* obs_cat, float* const* fin_act, float* obs_emb) {
-  const int E = D.obs_dim;
-  int max_depth = 0;
-  for (int j = 0; j < D.num_obs; ++j) max_depth = D.obs_ff[j].num_layers > max_depth ? D.obs_ff[j].num_layers : max_depth;
-  std::vector<int> in_off(D.num_obs), out_off(D.num_obs);
-  { int ci = 0, co = 0; for (int j = 0; j < D.num_obs; ++j) { in_off[j] = ci; out_off[j] = co; ci += D.obs_ff[j].in_dim; co += D.obs_ff[j].out_dim; } }
-  for (int l = 0; l < max_depth; ++l) {
-    bl.begin();
-    for (int j = 0; j < D.num_obs; ++j) {
-      const ppb_ff_desc& ff = D.obs_ff[j];
-      if (l >= ff.num_layers) continue;
-      const ppb_linear_desc& L = ff.layers[l];
-      const float* X = l == 0 ? obs + in_off[j] : obs_act[j][l - 1];
-      int64_t ldx = l == 0 ? D.obs_in_total : ff.layers[l - 1].out_dim;
-      bool last = (l == ff.num_layers - 1);
-      float* Y = last ? obs_cat + out_off[j] : obs_act[j][l];
-      int64_t ldy = last ? E : L.out_dim;
-      bl.add(linear_fwd(X, ldx, arena + L.w_off, L.in_dim, arena + L.b_off, Y, ldy, B, L.out_dim, L.in_dim, gemm::kRelu));
-    }
-  }
-  for (int l = 0; l < D.obs_final.num_layers; ++l) {
-    bl.begin();
-    const ppb_linear_desc& L = D.obs_final.layers[l];
-    const float* X = l == 0 ? obs_cat : fin_act[l - 1];
-    bool last = (l == D.obs_final.num_layers - 1);
-    float* Y = last ? obs_emb : fin_act[l];
-    bl.add(linear_fwd(X, L.in_dim, arena + L.w_off, L.in_dim, arena + L.b_off, Y, L.out_dim, B, L.out_dim, L.in_dim, gemm::kRelu));
-  }
 }
 
 inline uint64_t fnv1a(const void* data, size_t n, uint64_t h = 1469598103934665603ULL) {
@@ -1304,7 +1274,7 @@ int ppb_ic_loss_forward(ppb_net* net, const float* arena, const ppb_batch* b, vo
 
   // ---- problem lists for all forward GEMM phases -------------------------------------------------
   Builder bl;
-  add_obs_embed(bl, D, arena, b->obs, d.B, w.obs_act, w.obs_cat, w.fin_act, w.obs_emb);
+  obs_fp32_plan_fwd(bl, D, arena, b->obs, d.B, w, w.obs_emb);
   const int ph_obs0 = 0;
   const int ph_p = (int)bl.phases.size();
   bl.begin();
@@ -1447,47 +1417,7 @@ int ppb_ic_loss_backward(ppb_net* net, const float* arena, float* grad, const pp
     bl.add(linear_dx(w.d_pobs, H4, arena + D.w_ih_off, I, w.d_obs_emb, E, d.B, H4, E, 0));
     bl.add(linear_dx(w.d_pstep, H4, arena + D.w_ih_off + E + S, I, w.d_embcat, C2, d.NS, H4, C2, 0));
   }
-  // observe-embedding final FF backward (each layer: mask by relu, dW, dX)
-  std::vector<int> ph_fin;
-  for (int l = D.obs_final.num_layers - 1; l >= 0; --l) {
-    const ppb_linear_desc& L = D.obs_final.layers[l];
-    const float* X = l == 0 ? w.obs_cat : w.fin_act[l - 1];
-    float* dY = (l == D.obs_final.num_layers - 1) ? w.d_obs_emb : w.d_fin_act[l];
-    float* dX = l == 0 ? w.d_obs_cat : w.d_fin_act[l - 1];
-    ph_fin.push_back((int)bl.phases.size());
-    bl.begin();
-    bl.add(linear_dw(dY, L.out_dim, X, L.in_dim, grad + L.w_off, L.in_dim, d.B, L.out_dim, L.in_dim));
-    Problem px = linear_dx(dY, L.out_dim, arena + L.w_off, L.in_dim, dX, L.in_dim, d.B, L.out_dim, L.in_dim, gemm::kMaskAux);
-    px.aux = X; px.ld_aux = L.in_dim;  // relu' of the layer below: its output is this layer's input
-    if (l == 0) { px.aux = w.obs_cat; px.ld_aux = E; }
-    bl.add(px);
-  }
-  // per-observable FF backward by depth level (from the top)
-  int max_depth = 0;
-  for (int j = 0; j < D.num_obs; ++j) max_depth = D.obs_ff[j].num_layers > max_depth ? D.obs_ff[j].num_layers : max_depth;
-  std::vector<int> in_off(D.num_obs), out_off(D.num_obs);
-  { int ci = 0, co = 0; for (int j = 0; j < D.num_obs; ++j) { in_off[j] = ci; out_off[j] = co; ci += D.obs_ff[j].in_dim; co += D.obs_ff[j].out_dim; } }
-  std::vector<int> ph_obs;
-  for (int l = max_depth - 1; l >= 0; --l) {
-    ph_obs.push_back((int)bl.phases.size());
-    bl.begin();
-    for (int j = 0; j < D.num_obs; ++j) {
-      const ppb_ff_desc& ff = D.obs_ff[j];
-      if (l >= ff.num_layers) continue;
-      const ppb_linear_desc& L = ff.layers[l];
-      bool last = (l == ff.num_layers - 1);
-      const float* X = l == 0 ? b->obs + in_off[j] : w.obs_act[j][l - 1];
-      int64_t ldx = l == 0 ? D.obs_in_total : ff.layers[l - 1].out_dim;
-      const float* dY = last ? w.d_obs_cat + out_off[j] : w.d_obs_act[j][l];
-      int64_t lddy = last ? E : L.out_dim;
-      bl.add(linear_dw(dY, lddy, X, ldx, grad + L.w_off, L.in_dim, d.B, L.out_dim, L.in_dim));
-      if (l > 0) {
-        Problem px = linear_dx(dY, lddy, arena + L.w_off, L.in_dim, w.d_obs_act[j][l - 1], ff.layers[l - 1].out_dim, d.B, L.out_dim, L.in_dim, gemm::kMaskAux);
-        px.aux = w.obs_act[j][l - 1]; px.ld_aux = ff.layers[l - 1].out_dim;
-        bl.add(px);
-      }
-    }
-  }
+  const int ph_obs = obs_fp32_plan_bwd(bl, D, arena, grad, b->obs, d.B, w);
   Problem* dprobs = w.problems + w.max_problems / 2;
   rc = upload_and_get(net, bl, dprobs, w.max_problems / 2, st, 1);
   if (rc) return rc;
@@ -1533,32 +1463,7 @@ int ppb_ic_loss_backward(ppb_net* net, const float* arena, float* grad, const pp
     k_wsmp_grad<<<g, 256, 0, st>>>(dgates, w.smp_emb, d.R, H4, S, I, E, grad + D.w_ih_off, rpb);
     PPB_LAUNCH_CHECK();
   }
-  // observe embedding backward; relu' of the final output masks d_obs_emb first
-  k_mask_nonpos<<<ew_grid((int64_t)d.B * E), 256, 0, st>>>(w.d_obs_emb, w.obs_emb, (int64_t)d.B * E);
-  PPB_LAUNCH_CHECK();
-  for (size_t k = 0; k < ph_fin.size(); ++k) {
-    int l = D.obs_final.num_layers - 1 - (int)k;
-    const ppb_linear_desc& L = D.obs_final.layers[l];
-    float* dY = (l == D.obs_final.num_layers - 1) ? w.d_obs_emb : w.d_fin_act[l];
-    k_colsum_gather<<<dim3((L.out_dim + 31) / 32, 8), 256, 0, st>>>(dY, L.out_dim, nullptr, d.B, L.out_dim, grad + L.b_off);
-    PPB_LAUNCH_CHECK();
-    rc = run_phase(bl.phases[ph_fin[k]], dprobs, st); if (rc) return rc;
-  }
-  for (size_t k = 0; k < ph_obs.size(); ++k) {
-    int l = max_depth - 1 - (int)k;
-    for (int j = 0; j < D.num_obs; ++j) {
-      const ppb_ff_desc& ff = D.obs_ff[j];
-      if (l >= ff.num_layers) continue;
-      const ppb_linear_desc& L = ff.layers[l];
-      bool last = (l == ff.num_layers - 1);
-      const float* dY = last ? w.d_obs_cat + out_off[j] : w.d_obs_act[j][l];
-      int64_t lddy = last ? E : L.out_dim;
-      k_colsum_gather<<<dim3((L.out_dim + 31) / 32, 8), 256, 0, st>>>(dY, lddy, nullptr, d.B, L.out_dim, grad + L.b_off);
-      PPB_LAUNCH_CHECK();
-    }
-    rc = run_phase(bl.phases[ph_obs[k]], dprobs, st); if (rc) return rc;
-  }
-  return PPB_OK;
+  return obs_fp32_bwd(bl, ph_obs, dprobs, D, grad, d.B, w, st);
 }
 
 }  // extern "C"
@@ -1940,7 +1845,7 @@ int ppb_ic_embed_observe(ppb_net* net, const float* arena, const float* obs, flo
     if (rcw) return rcw;
   }
   Builder bl;
-  add_obs_embed(bl, net->desc, arena, obs, (int)n, w.obs_act, w.obs_cat, w.fin_act, obs_emb_out);
+  obs_fp32_plan_fwd(bl, net->desc, arena, obs, (int)n, w, obs_emb_out);
   int rc = upload_and_get(net, bl, w.problems, w.max_problems, st, 5);
   if (rc) return rc;
   for (auto& ph : bl.phases) { rc = run_phase(ph, w.problems, st); if (rc) return rc; }
