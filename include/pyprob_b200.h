@@ -33,6 +33,7 @@ extern "C" {
 #define PPB_FAMILY_UNIFORM 1     /* prior Uniform     -> proposal mixture of K TruncatedNormals   */
 #define PPB_FAMILY_POISSON 2     /* prior Poisson     -> proposal mixture of K TruncatedNormals   */
 #define PPB_FAMILY_CATEGORICAL 3 /* prior Categorical -> proposal Categorical                     */
+#define PPB_FAMILY_BERNOULLI 4   /* prior Bernoulli   -> proposal Bernoulli, head_out = 1, smp_in = 1 */
 
 const char* ppb_last_error(void);
 int ppb_version(void);
@@ -66,6 +67,10 @@ int ppb_uniform_log_prob(const float* value, const float* low, int low_stride, c
                          void* stream);
 int ppb_poisson_log_prob(const float* value, const float* rate, int rate_stride, float* lp_out,
                          double* acc, double acc_scale, int64_t n, void* stream);
+/* pyprob/distributions/bernoulli.py (torch Bernoulli(probs=)): v log(pc) + (1 - v) log(1 - pc), pc = clamp_probs(p);
+ * a value outside {0, 1} scores NaN (the reference's argument validation raises). */
+int ppb_bernoulli_log_prob(const float* value, const float* probs, int probs_stride, float* lp_out,
+                           double* acc, double acc_scale, int64_t n, void* stream);
 /* probs: [n, C] (probs_row_stride = C) or [C] shared (probs_row_stride = 0); unnormalised, as given to
  * pyprob/distributions/categorical.py:8-21.  value holds category indices stored as fp32. */
 int ppb_categorical_log_prob(const float* value, const float* probs, int64_t probs_row_stride,
@@ -102,6 +107,9 @@ int ppb_uniform_sample(const float* low, int low_stride, const float* high, int 
                        int64_t first_index, void* stream);
 int ppb_poisson_sample(const float* rate, int rate_stride, float* value_out, float* lp_out, int64_t n,
                        uint64_t seed, uint64_t offset, int64_t first_index, void* stream);
+/* value = 1 if u < p else 0, u uniform in [0, 1) from Philox word 0 */
+int ppb_bernoulli_sample(const float* probs, int probs_stride, float* value_out, float* lp_out, int64_t n,
+                         uint64_t seed, uint64_t offset, int64_t first_index, void* stream);
 int ppb_categorical_sample(const float* probs, int64_t probs_row_stride, int num_categories,
                            float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset,
                            int64_t first_index, void* stream);
@@ -346,7 +354,8 @@ int ppb_dp_adam_step(int world, int rank, void* const* peer_blocks /* host array
 /* Batched proposal step for IC posterior sampling (inference_network_lstm.py:82-134 for n particles in
  * lock-step at the same address).  h/c: fp32[n,H] LSTM state, updated in place (zeros at t=0).
  * prev_addr < 0 means first step.  Writes the proposal parameters:
- *   mixtures: params_out[n, 3K] = (means | stddevs | probs), categorical: params_out[n, C] = probs. */
+ *   mixtures: params_out[n, 3K] = (means | stddevs | probs), categorical: params_out[n, C] = probs,
+ *   bernoulli: params_out[n, 1] = probs. */
 int ppb_ic_infer_step(ppb_net* net, const float* arena, const float* obs_emb /*[n or 1, E]*/,
                       int obs_emb_row_stride, int32_t prev_addr, const float* prev_value,
                       int32_t cur_addr, const float* prior0, int prior0_stride, const float* prior1,

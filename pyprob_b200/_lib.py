@@ -31,6 +31,7 @@ _SIGNATURES = {
     'ppb_normal_log_prob': [c_f, c_f, c_int, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
     'ppb_uniform_log_prob': [c_f, c_f, c_int, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
     'ppb_poisson_log_prob': [c_f, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
+    'ppb_bernoulli_log_prob': [c_f, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
     'ppb_categorical_log_prob': [c_f, c_f, c_i64, c_int, c_f, c_f, c_dbl, c_i64, c_f],
     'ppb_mixture_normal_log_prob': [c_f, c_f, c_f, c_f, c_i64, c_int, c_f, c_f, c_dbl, c_i64, c_f],
     'ppb_mixture_truncated_normal_log_prob': [c_f, c_f, c_f, c_f, c_i64, c_int, c_f, c_int, c_f, c_int, c_f, c_f,
@@ -38,6 +39,7 @@ _SIGNATURES = {
     'ppb_normal_sample': [c_f, c_int, c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
     'ppb_uniform_sample': [c_f, c_int, c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
     'ppb_poisson_sample': [c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
+    'ppb_bernoulli_sample': [c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
     'ppb_categorical_sample': [c_f, c_i64, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
     'ppb_mixture_normal_sample': [c_f, c_f, c_f, c_i64, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
     'ppb_mixture_truncated_normal_sample': [c_f, c_f, c_f, c_i64, c_int, c_f, c_int, c_f, c_int, c_f, c_f, c_i64,

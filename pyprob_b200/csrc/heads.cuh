@@ -1,7 +1,8 @@
 // Proposal-head parameter transforms, log-probabilities and their hand-derived gradients.
 // Mirrors pyprob/nn/proposal_normal_normal_mixture.py:18-35, proposal_uniform_truncated_normal_mixture.py:18-36,
-// proposal_poisson_truncated_normal_mixture.py:20-36, proposal_categorical_categorical.py:16-20 and the
-// distributions they build (mixture.py:8-45, truncated_normal.py:11-54, torch Categorical(probs)).
+// proposal_poisson_truncated_normal_mixture.py:20-36, proposal_categorical_categorical.py:16-20,
+// proposal_bernoulli_bernoulli.py:16-20 and the distributions they build (mixture.py:8-45, truncated_normal.py:11-54,
+// torch Categorical(probs), torch Bernoulli(probs)).
 #pragma once
 #include "common.cuh"
 
@@ -134,6 +135,9 @@ __device__ __forceinline__ void categorical_probs(const float* x, int C, float* 
   for (int c = 0; c < C; ++c) { prob[c] = expf(x[c] - mx); s += prob[c]; }
   for (int c = 0; c < C; ++c) prob[c] = prob[c] / s + PPB_UTIL_EPSILON;
 }
+
+// Bernoulli head (proposal_bernoulli_bernoulli.py): probs = sigmoid(x) + 1e-8; torch Bernoulli(probs) clamps.
+__device__ __forceinline__ float bernoulli_prob(float x) { return sigmoidf_(x) + PPB_UTIL_EPSILON; }
 
 __device__ __forceinline__ float categorical_nll(const float* x, int C, float v, float* gx, bool want_grad) {
   float q[CMAX];

@@ -482,13 +482,27 @@ __device__ __forceinline__ void nll_row(const NllArgs& A, const float* x, int ro
   float g0 = 0.f, g1 = 0.f, g2 = 0.f, g3 = 0.f;  // this lane's gradient entries (mixture: m,s,p ; categorical: 4 cats)
   float lp = 0.0f;
   int O = 0;
-  bool is_cat = false;
+  bool is_cat = false, is_bern = false;
   if (valid) {
     const ppb_addr_desc a = addrs[step_addr[row_step[row]]];
     const float v = values[row];
     O = a.head_out;
     is_cat = a.family == PPB_FAMILY_CATEGORICAL;
-    if (is_cat) {
+    is_bern = a.family == PPB_FAMILY_BERNOULLI;
+    if (is_bern) {
+      // one output: p = sigmoid(x) + 1e-8, lp = v log pc + (1 - v) log(1 - pc); every lane computes it, lane 0's counts.
+      // d(-lp)/dx = -(v / pc - (1 - v) / (1 - pc)) sigma (1 - sigma), zero where the clamp is active
+      if (v != 0.0f && v != 1.0f) {
+        lp = NAN;
+      } else {
+        const float sg = heads::sigmoidf_(x[0]);
+        const float p = sg + PPB_UTIL_EPSILON;
+        const float pc = ppb_clamp_prob(p);
+        lp = (v == 1.0f) ? logf(pc) : log1pf(-pc);
+        const bool clamped = (p < PPB_EPS32) || (p > 1.0f - PPB_EPS32);
+        if (!clamped) g0 = -((v == 1.0f) ? 1.0f / pc : -1.0f / (1.0f - pc)) * (sg * (1.0f - sg));
+      }
+    } else if (is_cat) {
       const int C = a.num_categories;
       float q[4], xs[4];
       float mx = -INFINITY;
@@ -605,6 +619,8 @@ __device__ __forceinline__ void nll_row(const NllArgs& A, const float* x, int ro
         if (lane + 32 < O) put(lane + 32, g1);
         if (lane + 64 < O) put(lane + 64, g2);
         if (lane + 96 < O) put(lane + 96, g3);
+      } else if (is_bern) {
+        if (lane == 0) put(0, g0);
       } else if (lane < K) {
         put(lane, g0); put(K + lane, g1); put(2 * K + lane, g2);
       }
@@ -656,7 +672,9 @@ __global__ void __launch_bounds__(256) k_head_nll(const float* __restrict__ out_
 // wait: the weights are not written inside a training step — and each warp walks its rows: hidden activations = hi + lo of the
 // K-format tile image the h1 GEMM wrote (the same two words the tensor-core path multiplies), 4-way split dot products,
 // then nll_row on the outputs in shared memory.
-__global__ void __launch_bounds__(256) k_head_out_nll(const float* __restrict__ arena, const float* __restrict__ hid_hi,
+// Four blocks per SM: without the bound, the Bernoulli branch of nll_row lets ptxas take 103 registers (two blocks per SM);
+// with it the kernel keeps the 64 registers and no spills it had with four families.
+__global__ void __launch_bounds__(256, 4) k_head_out_nll(const float* __restrict__ arena, const float* __restrict__ hid_hi,
                                                        const float* __restrict__ hid_lo, int64_t hid_kb,
                                                        const int* __restrict__ step_row0, const int* __restrict__ step_nrows,
                                                        int rows_per_block, NllArgs A, float* __restrict__ out_raw,
@@ -1200,9 +1218,11 @@ int ppb_net_set_tables(ppb_net* net, const ppb_addr_desc* addrs, int32_t n_addrs
   net->arena_floats = arena_floats;
   int dh = 4, op = 4;
   for (auto& a : net->addrs) {
-    PPB_CHECK_ARG(a.family >= 0 && a.family <= 3, "unknown family");
+    PPB_CHECK_ARG(a.family >= 0 && a.family <= PPB_FAMILY_BERNOULLI, "unknown family");
     PPB_CHECK_ARG(a.family != PPB_FAMILY_CATEGORICAL || (a.num_categories > 0 && a.num_categories <= heads::CMAX),
                   "categorical head: 1..128 categories supported");
+    PPB_CHECK_ARG(a.family != PPB_FAMILY_BERNOULLI || (a.head_out == 1 && a.smp_in == 1 && a.num_categories == 0),
+                  "bernoulli head: head_out = 1, smp_in = 1, num_categories = 0");
     PPB_CHECK_ARG(a.type_id >= 0 && a.type_id < n_types, "type id out of range");
     if (a.head_hidden > dh) dh = a.head_hidden;
     if (a.head_out > op) op = a.head_out;
@@ -1646,7 +1666,9 @@ __global__ void __launch_bounds__(128) k_head_params(const float* __restrict__ o
                                                       float* __restrict__ params, int64_t n) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const float* x = out_raw + i * out_pad;
-    if (a.family == PPB_FAMILY_CATEGORICAL) {
+    if (a.family == PPB_FAMILY_BERNOULLI) {
+      params[i] = heads::bernoulli_prob(x[0]);
+    } else if (a.family == PPB_FAMILY_CATEGORICAL) {
       float xs[heads::CMAX], q[heads::CMAX];
       for (int c = 0; c < a.num_categories; ++c) xs[c] = x[c];
       heads::categorical_probs(xs, a.num_categories, q);

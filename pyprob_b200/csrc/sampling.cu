@@ -89,6 +89,22 @@ __global__ void __launch_bounds__(kThreads) k_poisson(P rate, float* __restrict_
   }
 }
 
+// Bernoulli: 1 if u < p (u uniform in [0, 1) from word 0), so p = 0 never and p = 1 always draws 1
+__global__ void __launch_bounds__(kThreads) k_bernoulli(P probs, float* __restrict__ out, float* __restrict__ lp,
+                                                         int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
+  int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, nth = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = tid; i < n; i += nth) {
+    ppb_philox r = ppb_philox4x32_10(seed, (uint64_t)(first + i), offset);
+    const float p = probs.at(i);
+    const bool one = ppb_u01(r.c[0]) < p;
+    out[i] = one ? 1.0f : 0.0f;
+    if (lp) {
+      const float pc = ppb_clamp_prob(p);
+      lp[i] = one ? logf(pc) : log1pf(-pc);
+    }
+  }
+}
+
 __device__ __forceinline__ int pick_category(const float* __restrict__ p, int C, float u, float* p_sel, float* p_sum) {
   float s = 0.0f;
   for (int c = 0; c < C; ++c) s += __ldg(p + c);
@@ -200,6 +216,17 @@ int ppb_poisson_sample(const float* rate, int rate_stride, float* value_out, flo
   if (n == 0) return PPB_OK;
   k_poisson<<<ppb_grid_for(n, kThreads, 1), kThreads, 0, (cudaStream_t)stream>>>(P{rate, rate_stride}, value_out,
                                                                                  lp_out, n, seed, offset, first_index);
+  PPB_LAUNCH_CHECK();
+  return PPB_OK;
+}
+
+int ppb_bernoulli_sample(const float* probs, int probs_stride, float* value_out, float* lp_out, int64_t n, uint64_t seed,
+                         uint64_t offset, int64_t first_index, void* stream) {
+  if (n == 0) return PPB_OK;
+  PPB_CHECK_ARG(n >= 0 && probs && value_out, "bad arguments");
+  PPB_CHECK_ARG((probs_stride | 1) == 1, "strides must be 0 or 1");
+  k_bernoulli<<<ppb_grid_for(n, kThreads, 1), kThreads, 0, (cudaStream_t)stream>>>(P{probs, probs_stride}, value_out,
+                                                                                   lp_out, n, seed, offset, first_index);
   PPB_LAUNCH_CHECK();
   return PPB_OK;
 }

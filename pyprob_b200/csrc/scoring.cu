@@ -1,6 +1,6 @@
 // Per-family log_prob over the particle axis — warp-coalesced, 128-bit vectorised, HBM-bound.
 // Replaces pyprob/distributions/distribution.py:38-43 as driven per particle by pyprob/state.py.
-// Algorithmic bytes per element (SURVEY §8d): Normal/Uniform 16 B, Poisson 12 B, Categorical 4C+12 B,
+// Algorithmic bytes per element (SURVEY §8d): Normal/Uniform 16 B, Poisson/Bernoulli 12 B, Categorical 4C+12 B,
 // Mixture-Normal (3K+2)*4 B, Mixture-TruncatedNormal (3K+4)*4 B.
 #include <stdlib.h>
 
@@ -101,6 +101,15 @@ struct PoissonOp {
     const int k = (int)v;
     const float lg = (v >= 0.0f && v < 64.0f && (float)k == v) ? tab[k] : lgammaf(v + 1.0f);
     return xl - rate - lg;
+  }
+};
+struct BernoulliOp {
+  static constexpr bool kTable = false;
+  // torch/distributions/bernoulli.py log_prob: -BCEWithLogits(log pc - log1p(-pc), v) = v log pc + (1 - v) log(1 - pc),
+  // pc = clamp_probs(p); values outside {0, 1} are rejected by the reference's argument validation: NaN here
+  __device__ __forceinline__ float operator()(float v, float p, float, const float*) const {
+    const float pc = ppb_clamp_prob(p);
+    return (v == 1.0f) ? logf(pc) : (v == 0.0f) ? log1pf(-pc) : NAN;
   }
 };
 
@@ -382,6 +391,15 @@ int ppb_poisson_log_prob(const float* value, const float* rate, int rate_stride,
   }
   return launch_score2(value, Param{rate, rate_stride}, Param{rate, 0}, Sink{lp_out, acc, acc_scale}, n, stream,
                        PoissonOp{});
+}
+
+int ppb_bernoulli_log_prob(const float* value, const float* probs, int probs_stride, float* lp_out, double* acc,
+                           double acc_scale, int64_t n, void* stream) {
+  if (n == 0) return PPB_OK;
+  PPB_CHECK_ARG(n >= 0 && value && probs, "null pointer or negative n");
+  PPB_CHECK_ARG((probs_stride | 1) == 1, "strides must be 0 or 1");
+  return launch_score2(value, Param{probs, probs_stride}, Param{probs, 0}, Sink{lp_out, acc, acc_scale}, n, stream,
+                       BernoulliOp{});
 }
 
 int ppb_categorical_log_prob(const float* value, const float* probs, int64_t probs_row_stride, int num_categories,

@@ -152,6 +152,48 @@ class Poisson(Distribution):
         return 'Poisson({})'.format(self.rate)
 
 
+class Bernoulli(Distribution):
+    """probs (or logits, converted with a sigmoid): a scalar shared by all particles or one per particle (reference:
+    bernoulli.py, torch Bernoulli).  Values are 0. / 1.; any other value scores NaN.
+
+    log_prob always works from probs clamped to [eps32, 1 - eps32], so it is at least log(eps32) = -15.9.  Built from
+    logits, torch's Bernoulli scores with the raw logits instead and agrees only while |logits| < about 16: at
+    logits = -30 it gives -30 for the value 1 where this gives -15.9 (DESIGN.md section 8)."""
+
+    def __init__(self, probs=None, logits=None):
+        super().__init__('Bernoulli', 'Bernoulli')
+        if probs is None:
+            if logits is None:
+                raise ValueError('Either probs or logits must be given.')
+            probs = torch.sigmoid(torch.as_tensor(logits, dtype=torch.float32))
+        self.probs = _as_param(probs)
+
+    @property
+    def batch_length(self):
+        return _length(self.probs)
+
+    @property
+    def logits(self):
+        p = self.probs
+        return torch.log(p) - torch.log1p(-p) if torch.is_tensor(p) else math.log(p) - math.log1p(-p)
+
+    mean = property(lambda self: self.probs)
+    variance = property(lambda self: self.probs * (1 - self.probs))
+
+    def _draw(self, n, with_log_prob):
+        s, o, f = self._seed_args()
+        return ops.bernoulli_sample(self.probs, n, s, o, f, with_log_prob)
+
+    def _log_prob(self, value):
+        return ops.bernoulli_log_prob(_value(value, self.batch_length), self.probs)
+
+    def score_into(self, value, acc, scale):
+        ops.bernoulli_log_prob(value, self.probs, acc=acc, acc_scale=scale)
+
+    def __repr__(self):
+        return 'Bernoulli({})'.format(self.probs)
+
+
 class Categorical(Distribution):
     """probs: [C] shared or [n, C] per particle (unnormalised, like the reference: categorical.py:8-21)."""
 

@@ -30,9 +30,9 @@ from .util import LearningRateScheduler, ObserveEmbedding, Optimizer
 
 _OPTIMIZER_KIND = {Optimizer.ADAM: 0, Optimizer.ADAM_LARC: 1, Optimizer.SGD: 2, Optimizer.SGD_LARC: 3}
 
-FAMILY_NORMAL, FAMILY_UNIFORM, FAMILY_POISSON, FAMILY_CATEGORICAL = 0, 1, 2, 3
+FAMILY_NORMAL, FAMILY_UNIFORM, FAMILY_POISSON, FAMILY_CATEGORICAL, FAMILY_BERNOULLI = 0, 1, 2, 3, 4
 _FAMILY_OF = {'Normal': FAMILY_NORMAL, 'Uniform': FAMILY_UNIFORM, 'Poisson': FAMILY_POISSON,
-              'Categorical': FAMILY_CATEGORICAL}
+              'Categorical': FAMILY_CATEGORICAL, 'Bernoulli': FAMILY_BERNOULLI}
 MAX_OBS, MAX_FF_LAYERS = 8, 4
 
 
@@ -306,7 +306,8 @@ class InferenceNetworkLSTM(nn.Module):
                         (self._distribution_type_embedding_dim,),
                         torch.zeros(self._distribution_type_embedding_dim).normal_())
             self._types[dist_name] = len(self._types)
-        out = num_categories if family == FAMILY_CATEGORICAL else 3 * K
+        # proposal_categorical_categorical.py: C logits; proposal_bernoulli_bernoulli.py: one logit; mixtures: 3K
+        out = num_categories if family == FAMILY_CATEGORICAL else 1 if family == FAMILY_BERNOULLI else 3 * K
         hidden = int((H + out) / 2)
         p = '_layers_proposal.{}._ff._layers'.format(address)
         self._linear(p + '.0', H, hidden)
@@ -925,7 +926,8 @@ class InferenceNetworkLSTM(nn.Module):
     def _infer_step_lanes(self, address, prev_address, prev_value, prior0, prior1, h, c):
         """One proposal step for the particles whose LSTM state rows are `h`, `c` ([m, H] contiguous, updated in place):
         all m particles sit at `address` and came from `prev_address` (None: first controlled site) with values
-        `prev_value` [m].  Returns the proposal parameters [m, 3K] (means|stddevs|probs) or [m, C]."""
+        `prev_value` [m].  Returns the proposal parameters [m, 3K] (means|stddevs|probs), [m, C] or [m, 1] (Bernoulli
+        probs)."""
         info = self._addresses[address]
         m = h.size(0)
         width = info['head_out'] if info['family'] != FAMILY_CATEGORICAL else info['num_categories']
@@ -949,7 +951,7 @@ class InferenceNetworkLSTM(nn.Module):
     def _infer_step_batched(self, address, prev_address, prev_value, prior0, prior1, n):
         """Proposal parameters for n particles in lock-step at `address`.
 
-        Returns a [n, 3K] (means|stddevs|probs) or [n, C] tensor, or None if the address is unknown
+        Returns a [n, 3K] (means|stddevs|probs), [n, C] or [n, 1] (Bernoulli probs) tensor, or None if the address is unknown
         (the caller then falls back to the prior, as the reference does with a warning)."""
         if address not in self._addresses or (prev_address is not None and prev_address not in self._addresses):
             warnings.warn('Address unknown by inference network: {}'.format(address))

@@ -76,6 +76,15 @@ def poisson_log_prob(value, rate, lp_out=None, acc=None, acc_scale=1.0):
     return lp_out
 
 
+def bernoulli_log_prob(value, probs, lp_out=None, acc=None, acc_scale=1.0):
+    value = _f32(value, value.device).reshape(-1)
+    n = value.numel()
+    p, pp, ps = _param(probs, n, value.device)
+    lp_out, acc = _sink(n, value.device, lp_out, acc)
+    call('ppb_bernoulli_log_prob', ptr(value), pp, ps, ptr(lp_out), ptr(acc), float(acc_scale), n, stream())
+    return lp_out
+
+
 def _rows(t, n, device):
     """[C] shared or [n, C] per particle -> (tensor, row_stride, C)"""
     if torch.is_tensor(t) and t.is_cuda and t.dtype == torch.float32 and t.dim() == 2 and t.stride(1) == 1 \
@@ -160,6 +169,13 @@ def poisson_sample(rate, n, seed, offset, first_index=0, with_log_prob=False, de
     r, rp, rs = _param(rate, n, device)
     v, lp = _out(n, device, with_log_prob)
     call('ppb_poisson_sample', rp, rs, ptr(v), ptr(lp), n, seed, offset, first_index, stream())
+    return (v, lp) if with_log_prob else v
+
+
+def bernoulli_sample(probs, n, seed, offset, first_index=0, with_log_prob=False, device='cuda'):
+    p, pp, ps = _param(probs, n, device)
+    v, lp = _out(n, device, with_log_prob)
+    call('ppb_bernoulli_sample', pp, ps, ptr(v), ptr(lp), n, seed, offset, first_index, stream())
     return (v, lp) if with_log_prob else v
 
 

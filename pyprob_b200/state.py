@@ -14,7 +14,7 @@ import warnings
 import torch
 
 from . import util
-from .distributions import Categorical, Distribution, Mixture, Normal, Poisson, Uniform
+from .distributions import Bernoulli, Categorical, Distribution, Mixture, Normal, Poisson, Uniform
 from .trace import BatchedTrace, Site
 from .util import InferenceEngine, PriorInflation, TraceMode
 
@@ -243,7 +243,7 @@ def _sample_from_proposal(trace, distribution, addr, n):
         uniq = torch.unique(ids).tolist()
         groups = [(u, None if len(uniq) == 1 else (ids == u)) for u in uniq]
     is_cat = isinstance(distribution, Categorical)
-    width = distribution.num_categories if is_cat else 3 * K
+    width = distribution.num_categories if is_cat else 1 if isinstance(distribution, Bernoulli) else 3 * K
     params = None
     covered = True        # every executing lane got a proposal from the network
     by_id = net._address_by_id()
@@ -273,6 +273,8 @@ def _sample_from_proposal(trace, distribution, addr, n):
     else:
         if is_cat:
             proposal = Categorical(probs=params)
+        elif isinstance(distribution, Bernoulli):   # proposal_bernoulli_bernoulli.py: prior parameters are not inputs
+            proposal = Bernoulli(probs=params[:, 0])
         elif isinstance(distribution, Normal):
             proposal = Mixture.from_rows(params[:, :K], params[:, K:2 * K], params[:, 2 * K:])
         elif isinstance(distribution, Uniform):
@@ -319,6 +321,8 @@ def _default_params(distribution, n, K, width):
     p = torch.zeros(n, width, device='cuda')
     if isinstance(distribution, Categorical):
         p.fill_(1.0 / width)
+    elif isinstance(distribution, Bernoulli):
+        p.fill_(0.5)
     else:
         if isinstance(distribution, Uniform):
             lo, hi = distribution.low, distribution.high

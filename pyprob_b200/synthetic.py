@@ -87,6 +87,8 @@ def random_sub_batch(rng, addresses, B, obs_dim):
             values[t] = p0[t] + (p1[t] - p0[t]) * rng.uniform(0.02, 0.98, B)
         elif fam == 'Poisson':
             values[t] = rng.poisson(3.0, B)
+        elif fam == 'Bernoulli':
+            values[t] = rng.integers(0, 2, B)
         else:
             values[t] = rng.integers(0, C, B)
     return {'addresses': [a for a, _, _ in addresses], 'families': [f for _, f, _ in addresses],
