@@ -74,17 +74,12 @@ struct ppb_net {
   int I = 0;        // LSTM input width  E + S + 2 (td + ad)
   int dh_pad = 4;   // max head hidden width, padded to 4
   int out_pad = 4;  // max head output width, padded to 4
-  // LSTM cell fused into the recurrent GEMM (tc_lstm.cuh, tc_cluster.cuh); PPB_FUSED_CELL selects the variant
-  int fused_cell = 3;
+  // LSTM cell fused into the recurrent GEMM (tc_lstm.cuh, tc_cluster.cuh); PPB_FUSED_CELL=0: GEMM and cell kernels
+  bool fused_cell = true;
   float* whh_il = nullptr;          // gate-interleaved K-format image of W_hh: hi part, then lo part
   int64_t whh_il_floats = 0;        // floats per part
-  void* d_lstm_steps = nullptr;     // device list of tcl::Step (level 1) or tcl::Seq + row_off (level 2)
+  void* d_lstm_steps = nullptr;     // device list of tcl::Step
   size_t lstm_steps_cap = 0;        // bytes
-  int* d_lstm_progress = nullptr;   // level 2: arrival counters (one per 128-row tile) + error flag
-  int lstm_progress_cap = 0;        // ints
-  int fused_cell_bwd = 1;           // BPTT: input-gradient GEMM + cell backward in one cluster kernel (PPB_FUSED_CELL_BWD=0: off)
-  void* d_bsteps = nullptr;         // device list of tcc::BStep
-  size_t bsteps_cap = 0;            // bytes
   // side streams: independent branches of the step run beside the critical path (captured into the same CUDA graph)
   cudaStream_t side[2] = {nullptr, nullptr};
   cudaEvent_t fork_ev[16] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
@@ -1193,11 +1188,9 @@ int ppb_net_create(ppb_net** out, const ppb_net_desc* d) {
   n->desc = *d;
   n->I = d->obs_dim + d->sample_dim + 2 * (d->type_dim + d->addr_dim);
   const char* fc = getenv("PPB_FUSED_CELL");
-  // LSTM steps t >= 1: 3 (default) = recurrent GEMM + cell in one kernel per step, cluster split-K when the step has few
-  // tiles (tc_cluster.cuh); 1 = same without clusters; 2 = one persistent launch for all steps; 0 = GEMM and cell kernels
-  n->fused_cell = (fc && fc[0] >= '0' && fc[0] <= '3') ? fc[0] - '0' : 3;
-  const char* fb = getenv("PPB_FUSED_CELL_BWD");
-  n->fused_cell_bwd = (fb && fb[0] == '0') ? 0 : 1;
+  // LSTM steps t >= 1: recurrent GEMM + cell in one kernel per step, cluster split-K when the step has few tiles
+  // (tc_cluster.cuh); PPB_FUSED_CELL=0 = GEMM and cell kernels, the reference the fused step is tested against
+  n->fused_cell = !(fc && fc[0] == '0');
   const char* hg = getenv("PPB_HOST_STEP_GRAPH");
   n->host_graph = (hg && hg[0] == '0') ? 0 : 1;   // on by default (PPB_HOST_STEP_GRAPH=0: always launch eagerly)
   const char* ss = getenv("PPB_SINGLE_STREAM");
@@ -1254,8 +1247,6 @@ int ppb_net_destroy(ppb_net* net) {
   if (net->d_pack) cudaFree(net->d_pack);
   if (net->whh_il) cudaFree(net->whh_il);
   if (net->d_lstm_steps) cudaFree(net->d_lstm_steps);
-  if (net->d_lstm_progress) cudaFree(net->d_lstm_progress);
-  if (net->d_bsteps) cudaFree(net->d_bsteps);
   if (net->host_exec) cudaGraphExecDestroy(net->host_exec);
   if (net->host_stream) cudaStreamDestroy(net->host_stream);
   if (net->host_hyper_dev) cudaFree(net->host_hyper_dev);

@@ -11,7 +11,7 @@
 // fixed summation order, and the epilogue work is spread over the cluster too.
 //
 // Epilogues (reduce phase; one thread owns one row x four columns {lane, lane+32, lane+64, lane+96} of the tile):
-//   k_cluster<X3, CS, 0>   fp32 store (+bias, ReLU, zero-invalid rows)           BPTT dX, head dX
+//   k_cluster<X3, CS, 0>   fp32 store (+bias, ReLU, zero-invalid rows)           head dX
 //   k_cluster<X3, CS, 2>   tile images (+fp32, ReLU-mask from an image)          head hidden layer and its gradient
 //   k_lstm_cluster<X3, CS> LSTM cell: with gate-interleaved W_hh the four columns of a thread are the gates i, f, g, o
 //                          of ONE hidden unit, so the cell update is thread-local (tc_lstm.cuh has the layout)
@@ -53,28 +53,6 @@ __device__ __forceinline__ float ld_cluster(uint32_t cluster_addr) {
   return v;
 }
 
-struct BwdIO {                // element-wise operands of the LSTM cell backward, shared by all segments of a launch
-  const float* gates;         // [rows, 4H] activated gates i, f, g, o (forward pass)
-  const float* c;             // [rows, H]
-  const float* dh;            // [rows, H]  d loss / d h_t from the proposal heads
-  float* dc;                  // [rows, H]  d loss / d c carried to the previous step
-  float* dgates;              // [rows, 4H] d loss / d gate pre-activations (fp32: column sums, sample-embedding gradients)
-  float* d_pobs;              // [traces, 4H] sum over the steps of a trace
-  const int* row_prev; const int* row_next; const int* row_trace;
-  float* gk_hi; float* gk_lo; float* gmn_hi; float* gmn_lo;   // tile images of dgates (next BPTT GEMM, weight gradients)
-  int gkb;                    // column blocks of the dgates images (4H / 32)
-  int H;
-};
-struct BStep {                // BPTT at time t for one (t + 1, sub-batch) segment: dh_rec = dgates_{t+1} W_hh, then the cell
-  tcg::Operand a;             // dgates image, rows of the segment at step t + 1 (K-major)
-  tcg::Operand b;             // W_hh image read MN-major (reduction over its 4H rows)
-  int M;                      // segment rows, padded to 128
-  int row0;                   // first global row of the segment at step t (multiple of 128)
-  int t;                      // time index of the rows being finished (c_{t-1} = 0 at t = 0)
-  int tile_start, tiles_m, tiles_n;
-  BwdIO io;
-};
-
 struct __align__(1024) Smem {
   float a_hi[tcg::kStages][kTileFloats];
   float a_lo[tcg::kStages][kTileFloats];
@@ -82,7 +60,7 @@ struct __align__(1024) Smem {
   float b_lo[tcg::kStages][kTileFloats];
   uint64_t full[tcg::kStages];
   uint64_t empty[tcg::kStages];
-  union { tcg::Problem prob; tcl::Step step; BStep bstep; };
+  union { tcg::Problem prob; tcl::Step step; };
 };
 inline size_t smem_bytes() { return sizeof(Smem) + 1024; }
 
@@ -305,7 +283,6 @@ __global__ void __launch_bounds__(tcg::kThreads, 1) k_lstm_cluster(const tcl::St
   if (warp == tcg::kProducerWarp && lane == 0) {
     const uint32_t bytes = (tcg::stage_bytes(P.a, mt) + tcg::stage_bytes(P.b, nt)) * (X3 ? 2u : 1u);
     b_pre = (c1 - c0) < tcg::kStages ? (c1 - c0) : tcg::kStages;
-    if (P.io.no_b_prefetch) b_pre = 0;
     for (int i = 0; i < b_pre; ++i) {
       mbar_expect_tx(&sm.full[i], bytes);
       tcg::load_operand(P.b, nt, c0 + i, sm.b_hi[i], sm.b_lo[i], X3, &sm.full[i]);
@@ -414,124 +391,6 @@ __global__ void __launch_bounds__(tcg::kThreads, 1) k_lstm_cluster(const tcl::St
     trace[8] = (unsigned long long)dm[0]; trace[9] = (unsigned long long)dm[1]; trace[10] = (unsigned long long)dm[2];
     trace[11] = (unsigned long long)gridDim.x; trace[12] = (unsigned long long)(c1 - c0);
   }
-}
-
-// ---- BPTT time step: recurrent input-gradient GEMM + cell backward in the reduce phase ----------------------------------------
-// Output tile = 128 rows of step t x 128 hidden units; a thread of the reduce phase holds dh_rec of one row and four units and
-// finishes them: d gates (fp32 + both image formats), d c_{t-1}, the per-trace sum d_pobs.  Mirrors k_cell_bwd (net.cu).
-template <bool X3, int CS>
-__global__ void __launch_bounds__(tcg::kThreads, 1) k_lstm_bwd_cluster(const BStep* __restrict__ steps, int n_steps) {
-  extern __shared__ uint8_t smem_raw[];
-  Smem& sm = *reinterpret_cast<Smem*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int tile = blockIdx.x / CS;
-  const int split = (int)cluster_ctarank();
-  int lo_i = 0, hi_i = n_steps - 1;
-  while (lo_i < hi_i) {
-    int mid = (lo_i + hi_i + 1) >> 1;
-    if (steps[mid].tile_start <= tile) lo_i = mid; else hi_i = mid - 1;
-  }
-  for (int i = threadIdx.x; i < (int)(sizeof(BStep) / 4); i += blockDim.x)
-    reinterpret_cast<uint32_t*>(&sm.bstep)[i] = reinterpret_cast<const uint32_t*>(steps + lo_i)[i];
-  __syncthreads();
-  const BStep& P = sm.bstep;
-  const BwdIO& io = P.io;
-  const int local = tile - P.tile_start;
-  const int mt = local / P.tiles_n, nt = local % P.tiles_n;   // nt = block of 128 hidden units
-  const int H = io.H, H4 = 4 * io.H;
-  const int KC = H4 / 32;
-  const int c0 = (int)((int64_t)KC * split / CS), c1 = (int)((int64_t)KC * (split + 1) / CS);
-  common_setup(sm, warp, lane);
-  // row metadata while the mainloop runs (it heads the dependency chain of the reduce phase)
-  constexpr int kRowsPerCta = 128 / CS, kRowsPerWarp = kRowsPerCta / tcg::kEpiWarps;
-  int m_tr[kRowsPerWarp], m_nx[kRowsPerWarp], m_rp[kRowsPerWarp];
-  if (warp < tcg::kEpiWarps) {
-#pragma unroll
-    for (int rr = 0; rr < kRowsPerWarp; ++rr) {
-      const int64_t row = (int64_t)P.row0 + mt * 128 + split * kRowsPerCta + warp * kRowsPerWarp + rr;
-      m_tr[rr] = __ldg(io.row_trace + row);
-      m_nx[rr] = __ldg(io.row_next + row);
-      m_rp[rr] = (P.t > 0) ? __ldg(io.row_prev + row) : 0;
-    }
-  }
-  mainloop_and_park<X3>(sm, P.a, P.b, mt, nt, c0, c1, warp, lane);
-
-  if (warp < tcg::kEpiWarps) {
-    const int ew = warp;
-    // descriptor fields in registers (P sits in shared memory behind a generic pointer, every io.x would be a dependent load)
-    const float* const g_gates = io.gates; const float* const g_c = io.c; const float* const g_dh = io.dh;
-    float* const g_dc = io.dc; float* const g_dp = io.d_pobs; float* const g_dg = io.dgates;
-    float* const gk_hi = io.gk_hi; float* const gk_lo = io.gk_lo; float* const gmn_hi = io.gmn_hi; float* const gmn_lo = io.gmn_lo;
-    const int64_t gkb = io.gkb;
-    const bool has_prev = P.t > 0;
-    const int64_t seg_row0 = (int64_t)P.row0;
-    const int n_blocks = (H - nt * 128 + 31) >> 5;     // 32-unit blocks of this tile inside H (warp-uniform)
-#pragma unroll
-    for (int rr = 0; rr < kRowsPerWarp; ++rr) {
-      const int trow = split * kRowsPerCta + ew * kRowsPerWarp + rr;
-      const int64_t row = seg_row0 + mt * 128 + trow;
-      const bool live = m_tr[rr] >= 0;
-      // pass 1 — ONE basic block: partial sums from the peers' shared memory and every element-wise operand of the row's four
-      // unit blocks in flight together; padding rows / unit blocks beyond H read a valid address and are zeroed afterwards
-      const int64_t lrow = live ? row : seg_row0;
-      const int64_t ltr = live ? m_tr[rr] : 0, lnx = (live && m_nx[rr] >= 0) ? m_nx[rr] : 0, lrp = live ? m_rp[rr] : 0;
-      float v[4];
-      reduce_row<CS>(sm, trow, lane, v);
-      float d[4][4], dcf[4], pob[4][4];
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        const int u = (g < n_blocks) ? nt * 128 + g * 32 + lane : lane;
-        const float* gr = g_gates + lrow * H4 + u;
-        const float* dp = g_dp + ltr * H4 + u;
-        const float ig = __ldg(gr), fg = __ldg(gr + H), gg = __ldg(gr + 2 * H), og = __ldg(gr + 3 * H);
-        const float cn = __ldg(g_c + lrow * H + u);
-        const float cpv = __ldg(g_c + lrp * H + u);
-        const float dh_head = __ldg(g_dh + lrow * H + u);
-        const float dc_next = __ldcg(g_dc + lnx * H + u);
-        float old[4];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) old[q] = __ldcg(dp + q * H);
-        const float cp = has_prev ? cpv : 0.0f;
-        const float tc = ppb_cell_tanh(cn);
-        const float dht = dh_head + v[g];
-        const float dct = (m_nx[rr] >= 0 ? dc_next : 0.0f) + dht * og * (1.0f - tc * tc);
-        d[g][0] = live ? dct * gg * ig * (1.0f - ig) : 0.0f;
-        d[g][1] = live ? dct * cp * fg * (1.0f - fg) : 0.0f;
-        d[g][2] = live ? dct * ig * (1.0f - gg * gg) : 0.0f;
-        d[g][3] = live ? dht * tc * og * (1.0f - og) : 0.0f;
-        dcf[g] = dct * fg;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) pob[g][q] = old[q] + d[g][q];
-      }
-      // pass 2 — stores
-      const int64_t img_row = ((row >> 7) * gkb) * kTileFloats + (row & 127) * 32;
-      const int pk = ((((lane >> 2) ^ (int)(row & 7))) << 2) + (lane & 3);
-      const int pmn = ((((lane >> 3) ^ (int)(row & 3))) << 3) + (lane & 7);
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        if (g >= n_blocks) continue;   // warp-uniform: unit block beyond H (H < 128 * tiles_n)
-        const int u = nt * 128 + g * 32 + lane;
-        if (live) {
-          tcg::st_global(g_dc + row * H + u, dcf[g]);
-          float* dp = g_dp + (int64_t)m_tr[rr] * H4 + u;
-#pragma unroll
-          for (int q = 0; q < 4; ++q) tcg::st_global(dp + q * H, pob[g][q]);
-        }
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          tcg::st_global(g_dg + row * H4 + q * H + u, d[g][q]);
-          const int64_t span = img_row + (int64_t)((q * H + u - lane) >> 5) * kTileFloats;
-          float hh, hl;
-          split_tf32(d[g][q], hh, hl);
-          tcg::st_global(gk_hi + span + pk, hh);
-          tcg::st_global(gk_lo + span + pk, hl);
-          tcg::st_global(gmn_hi + span + pmn, hh);
-          tcg::st_global(gmn_lo + span + pmn, hl);
-        }
-      }
-    }
-  }
-  cluster_sync_all();
 }
 
 // host-side launch with a (CS, 1, 1) cluster (and the PDL attribute, common.cuh)

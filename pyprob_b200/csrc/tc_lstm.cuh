@@ -14,8 +14,9 @@
 //
 // Mainloop, pipeline, descriptors and the 3xTF32 scheme are those of tc_grouped.cuh.
 //
-// Opt-in: PPB_FUSED_CELL=1 launches k_lstm_step once per time step, PPB_FUSED_CELL=2 runs all steps in one persistent
-// launch (k_lstm_seq).
+// The default step runs k_lstm_step, one launch per time step, whenever pick_cluster (net_tc.inc) finds no cluster split
+// worth making: H < 128 (K too short to split) or more than SMs / 2 tiles (two CTAs per tile would not fit one wave).
+// Otherwise the step runs tcc::k_lstm_cluster (tc_cluster.cuh), which shares the step list, CellIO and the W_hh layout.
 #pragma once
 #include "tc_grouped.cuh"
 
@@ -37,7 +38,6 @@ struct CellIO {               // element-wise operands of the cell update, share
   float* hk_hi; float* hk_lo; float* hmn_hi; float* hmn_lo;   // tile images of h (both formats)
   int hkb;                    // column blocks of the h images (H / 32)
   int H, S;                   // hidden size (reduction length; N = 4H), sample-embedding width (<= 8)
-  int no_b_prefetch;          // 1: the cluster kernel does not request W_hh tiles ahead of its PDL wait (A/B switch)
 };
 
 struct Step {                 // one (time step t >= 1, sub-batch) segment: one launch per time step
@@ -49,20 +49,6 @@ struct Step {                 // one (time step t >= 1, sub-batch) segment: one 
   CellIO io;
 };
 
-struct Seq {                  // one sub-batch, ALL its steps t = 1 .. T-1: persistent launch (k_lstm_seq)
-  tcg::Operand a;             // h image (K-major); the row origin is set per step
-  tcg::Operand b;             // gate-interleaved W_hh image
-  int M;                      // rows of the sub-batch, padded to 128 (constant over its steps)
-  int T;                      // trace length of the sub-batch
-  int seg_off;                // offset of the sub-batch inside every step's row block
-  int prog0;                  // index of its first progress counter (one counter per 128-row tile)
-  int tile_start, tiles_m, tiles_n;
-  const int* row_off;         // [T_max + 1] device: first row of step t
-  int* progress;              // device counters, zero before the launch; [n_counters] = error flag
-  int n_counters;
-  CellIO io;
-};
-
 struct __align__(1024) Smem {
   float a_hi[tcg::kStages][kTileFloats];
   float a_lo[tcg::kStages][kTileFloats];
@@ -70,7 +56,7 @@ struct __align__(1024) Smem {
   float b_lo[tcg::kStages][kTileFloats];
   uint64_t full[tcg::kStages];
   uint64_t empty[tcg::kStages];
-  union { Step step; Seq seq; };
+  Step step;
 };
 static_assert(tcg::kEpiWarps * 32 * 33 * 4 <= 2 * tcg::kStages * kTileBytes, "staging blocks must fit in the A stages");
 
@@ -187,89 +173,6 @@ __global__ void __launch_bounds__(tcg::kThreads, 1) k_lstm_step(const Step* __re
     cell_epilogue(reinterpret_cast<float*>(sm.a_hi), ctile, P.io, warp, lane, nt, (int64_t)P.row0 + mt * 128);
   }
   __syncthreads();
-}
-
-// ---- persistent variant: ALL time steps t >= 1 of every sub-batch in one launch ---------------------------------------------
-// Grid = (128-row tiles) x (32-unit blocks) of the sub-batches, at most one CTA per SM so that every CTA is resident.
-// CTA (sub-batch, mt, nt) loops over t; step t needs h_{t-1} of ALL unit blocks of its row tile, so a launch
-// boundary is replaced by one arrival counter per row tile: after its h-image stores of step t a CTA does
-// __threadfence + atomicAdd; before the first bulk load of step t the producer thread spins (ld.acquire.gpu) until the
-// counter shows (t-1) * tiles_n arrivals, then orders the async proxy after the acquire (fence.proxy.async) because
-// the bulk copies read what other CTAs wrote with ordinary stores.  Waits give up after 2 s and raise the error flag.
-__device__ __forceinline__ int ld_acquire_gpu(const int* p) {
-  int v;
-  asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ unsigned long long timer_ns() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
-
-template <bool X3>
-__global__ void __launch_bounds__(tcg::kThreads, 1) k_lstm_seq(const Seq* __restrict__ seqs, int n_seqs) {
-  extern __shared__ uint8_t smem_raw[];
-  Smem& sm = *reinterpret_cast<Smem*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int tile = blockIdx.x;
-  int lo_i = 0, hi_i = n_seqs - 1;
-  while (lo_i < hi_i) {
-    int mid = (lo_i + hi_i + 1) >> 1;
-    if (seqs[mid].tile_start <= tile) lo_i = mid; else hi_i = mid - 1;
-  }
-  for (int i = threadIdx.x; i < (int)(sizeof(Seq) / 4); i += blockDim.x)
-    reinterpret_cast<uint32_t*>(&sm.seq)[i] = reinterpret_cast<const uint32_t*>(seqs + lo_i)[i];
-  __syncthreads();
-  const Seq& P = sm.seq;
-  const int local = tile - P.tile_start;
-  const int mt = local / P.tiles_n, nt = local % P.tiles_n;
-  const int KC = (P.io.H + 31) / 32;
-
-  if (warp == tcg::kProducerWarp && lane == 0) {
-    for (int s = 0; s < tcg::kStages; ++s) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], tcg::kEpiWarps); }
-    fence_barrier_init();
-  }
-  __syncthreads();
-  const tcg::Ring R{sm.a_hi[0], sm.a_lo[0], sm.b_hi[0], sm.b_lo[0], kTileFloats, tcg::kStages, sm.full, sm.empty};
-  int* counter = P.progress + P.prog0 + mt;
-
-  for (int t = 1; t < P.T; ++t) {
-    const int row0 = __ldg(P.row_off + t) + P.seg_off, prev0 = __ldg(P.row_off + t - 1) + P.seg_off;
-    const uint32_t cbase = (uint32_t)(t - 1) * KC;     // the stage ring and its phases keep running across the steps
-    if (warp == tcg::kProducerWarp) {
-      if (lane == 0) {
-        if (t > 1) {
-          const int target = (t - 1) * P.tiles_n;
-          const unsigned long long t0 = timer_ns();
-          while (ld_acquire_gpu(counter) < target) {
-            if (timer_ns() - t0 > 2000000000ull) { P.progress[P.n_counters] = 1; break; }
-          }
-          asm volatile("fence.proxy.async;" ::: "memory");
-        }
-        tcg::Operand a = P.a;
-        a.row0 = prev0;
-        tcg::produce<X3>(R, a, P.b, mt, nt, 0, KC, cbase);
-      }
-    } else {
-      float acc[32];
-      tcg::mma_mainloop<X3>(R, cbase, KC, false, false, warp, lane, acc);
-      float* const ctile = sm.b_hi[0];
-      tcg::consumer_sync();
-      tcg::store_acc(acc, warp, lane, [&](int r, int c) { return ctile + r * tcg::kCPitch + c; });
-      tcg::consumer_sync();
-      cell_epilogue(reinterpret_cast<float*>(sm.a_hi), ctile, P.io, warp, lane, nt, (int64_t)row0 + mt * 128);
-      __threadfence();   // this thread's h / c / image stores are visible device-wide before the arrival below
-    }
-    // the staging blocks and the result tile (aliasing the operand stages) are free again; the next step's bulk copies
-    // (async proxy) overwrite shared memory this step's epilogue wrote through the generic proxy
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      __threadfence();
-      atomicAdd(counter, 1);
-    }
-  }
 }
 
 inline size_t smem_bytes() { return sizeof(Smem) + 1024; }

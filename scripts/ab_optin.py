@@ -1,52 +1,13 @@
-"""A/B timing of the opt-in kernels against the defaults, each arm in its own process (the switches are read from
-the environment when the library / network handle is created):
-  PPB_FUSED_CELL=1|2   synthetic 50-address training step (B=512), forward+backward+Adam, CUDA events
+"""A/B timing of the opt-in kernels against the defaults, each arm in its own process (the switches are read once per
+process):
   PPB_MIXTURE_STAGED=1 mixture-of-Normals / mixture-of-TruncatedNormals log_prob at 2^24 particles, K=10
-Prints one JSON object.  Timings only — correctness is the job of tests/test_fused_cell_gpu.py and
-tests/test_scoring_staged_gpu.py."""
+Prints one JSON object.  Timings only — correctness is the job of tests/test_scoring_staged_gpu.py."""
 import json
 import os
 import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-_STEP = r'''
-import sys, json, ctypes as C, numpy as np, torch
-sys.path.insert(0, %r)
-from pyprob_b200 import synthetic
-from pyprob_b200._lib import call, ptr
-from pyprob_b200.network import BatchStruct
-from pyprob_b200.util import Optimizer
-dev = torch.device('cuda:0'); rng = np.random.default_rng(0); B, T = 512, 50
-net = synthetic.synthetic50_network(precision=0, T=T)
-net._optimizer_type, net._learning_rate_init, net._weight_decay = Optimizer.ADAM, 1e-3, 0.0
-net._create_optimizer(); net._sync_native()
-enc = synthetic.synthetic50_batch(rng, B, T=T).encode(net)
-grad = torch.zeros_like(net._arena.data)
-img = torch.from_numpy(enc.pack().copy()).pin_memory(); dimg = img.to(dev)
-bs = BatchStruct(); call('ppb_batch_from_image', img.data_ptr(), dimg.data_ptr(), img.numel(), C.byref(bs))
-need = net._ensure_workspace(enc)
-st = torch.cuda.current_stream().cuda_stream
-loss = torch.empty((), device=dev); status = torch.zeros(1, dtype=torch.int32, device=dev)
-step_no = [0]
-def step():
-    grad.zero_()
-    call('ppb_ic_loss_forward', net._handle, ptr(net._arena.data), C.byref(bs), ptr(net._workspace), need, 0, ptr(loss),
-         ptr(status), None, 1, st)
-    call('ppb_ic_loss_backward', net._handle, ptr(net._arena.data), ptr(grad), C.byref(bs), ptr(net._workspace), need, 0,
-         1.0, st)
-    step_no[0] += 1
-    call('ppb_adam_step', ptr(net._arena.data), ptr(grad), ptr(net._exp_avg), ptr(net._exp_avg_sq), grad.numel(), 1e-3,
-         0.9, 0.999, 1e-8, 0.0, step_no[0], 1.0, st)
-for _ in range(5): step()
-torch.cuda.synchronize()
-e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-e0.record()
-for _ in range(20): step()
-e1.record(); torch.cuda.synchronize()
-print(json.dumps({'ms_per_step': e0.elapsed_time(e1) / 20, 'loss': float(loss)}))
-''' % ROOT
 
 _MIX = r'''
 import sys, json, torch
@@ -76,8 +37,7 @@ print(json.dumps(out))
 
 def run(script, env_extra):
     env = dict(os.environ)
-    for k in ('PPB_FUSED_CELL', 'PPB_MIXTURE_STAGED'):
-        env.pop(k, None)
+    env.pop('PPB_MIXTURE_STAGED', None)
     env.update(env_extra)
     r = subprocess.run([sys.executable, '-c', script], env=env, capture_output=True, text=True, timeout=180)
     if r.returncode != 0:
@@ -86,9 +46,5 @@ def run(script, env_extra):
 
 
 if __name__ == '__main__':
-    res = {}
-    if len(sys.argv) < 2 or sys.argv[1] != 'mix':
-        res['synthetic50_step'] = {'default': run(_STEP, {}), 'fused_cell': run(_STEP, {'PPB_FUSED_CELL': '1'}),
-                                   'persistent': run(_STEP, {'PPB_FUSED_CELL': '2'})}
-    res['mixture_scoring'] = {'default': run(_MIX, {}), 'staged': run(_MIX, {'PPB_MIXTURE_STAGED': '1'})}
+    res = {'mixture_scoring': {'default': run(_MIX, {}), 'staged': run(_MIX, {'PPB_MIXTURE_STAGED': '1'})}}
     print(json.dumps(res, indent=1))
