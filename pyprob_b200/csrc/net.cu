@@ -463,27 +463,41 @@ struct NllArgs {
   float* row_lp; float* d_out; int out_pad;
   HImg dimg;
 };
-__device__ __forceinline__ void nll_row(const NllArgs& A, const float* x, int row, int lane, float& local, int& bad) {
-  const ppb_addr_desc* addrs = A.addrs;
-  const int* row_step = A.row_step; const int* step_addr = A.step_addr;
-  const float* values = A.values; const float* prior0 = A.prior0; const float* prior1 = A.prior1;
-  const int* row_trace = A.row_trace;
+// what the NLL of a row reads besides its head outputs: a chain of dependent loads (row -> step -> address), which a caller
+// may issue long before the outputs exist (NllRowEpi: before the GEMM mainloop)
+struct NllRowIn {
+  bool valid;
+  int O, family, C;
+  float v, p0, p1;
+};
+__device__ __forceinline__ NllRowIn nll_row_in(const NllArgs& A, int row) {
+  NllRowIn in;
+  in.valid = A.row_trace[row] >= 0;
+  in.O = 0; in.family = 0; in.C = 0; in.v = 0.f; in.p0 = 0.f; in.p1 = 0.f;
+  if (in.valid) {
+    const ppb_addr_desc& a = A.addrs[A.step_addr[A.row_step[row]]];
+    in.O = a.head_out; in.family = a.family; in.C = a.num_categories;
+    in.v = A.values[row]; in.p0 = A.prior0[row]; in.p1 = A.prior1[row];
+  }
+  return in;
+}
+__device__ __forceinline__ void nll_row(const NllArgs& A, const NllRowIn& in, const float* x, int row, int lane, float& local,
+                                        int& bad) {
   const int K = A.K, out_pad = A.out_pad;
   const float inv_batch = A.inv_batch;
   float* row_lp = A.row_lp; float* d_out = A.d_out;
   const HImg dimg = A.dimg;
   const int img_cols = (int)dimg.kb * 32;
-  const bool valid = row_trace[row] >= 0;
+  const bool valid = in.valid;
   float g0 = 0.f, g1 = 0.f, g2 = 0.f, g3 = 0.f;  // this lane's gradient entries (mixture: m,s,p ; categorical: 4 cats)
   float lp = 0.0f;
   int O = 0;
   bool is_cat = false, is_bern = false;
   if (valid) {
-    const ppb_addr_desc a = addrs[step_addr[row_step[row]]];
-    const float v = values[row];
-    O = a.head_out;
-    is_cat = a.family == PPB_FAMILY_CATEGORICAL;
-    is_bern = a.family == PPB_FAMILY_BERNOULLI;
+    const float v = in.v;
+    O = in.O;
+    is_cat = in.family == PPB_FAMILY_CATEGORICAL;
+    is_bern = in.family == PPB_FAMILY_BERNOULLI;
     if (is_bern) {
       // one output: p = sigmoid(x) + 1e-8, lp = v log pc + (1 - v) log(1 - pc); every lane computes it, lane 0's counts.
       // d(-lp)/dx = -(v / pc - (1 - v) / (1 - pc)) sigma (1 - sigma), zero where the clamp is active
@@ -498,7 +512,7 @@ __device__ __forceinline__ void nll_row(const NllArgs& A, const float* x, int ro
         if (!clamped) g0 = -((v == 1.0f) ? 1.0f / pc : -1.0f / (1.0f - pc)) * (sg * (1.0f - sg));
       }
     } else if (is_cat) {
-      const int C = a.num_categories;
+      const int C = in.C;
       float q[4], xs[4];
       float mx = -INFINITY;
 #pragma unroll
@@ -541,8 +555,8 @@ __device__ __forceinline__ void nll_row(const NllArgs& A, const float* x, int ro
       }
     } else {
       const bool on = lane < K;
-      const int fam = a.family;
-      const float p0 = prior0[row], p1 = prior1[row];
+      const int fam = in.family;
+      const float p0 = in.p0, p1 = in.p1;
       const float xm = on ? x[lane] : 0.f, xsd = on ? x[K + lane] : 0.f, xp = on ? x[2 * K + lane] : -INFINITY;
       float mx = ppb_warp_max(xp);
       float e = on ? expf(xp - mx) : 0.0f;
@@ -624,6 +638,10 @@ __device__ __forceinline__ void nll_row(const NllArgs& A, const float* x, int ro
   }
   }
 
+__device__ __forceinline__ void nll_row(const NllArgs& A, const float* x, int row, int lane, float& local, int& bad) {
+  nll_row(A, nll_row_in(A, row), x, row, lane, local, bad);
+}
+
 // sum of -log q and count of failed rows -> loss accumulators; the last block to finish publishes the totals
 // (loss_acc[2] counts finished blocks; zeroed with the accumulators)
 __device__ __forceinline__ void nll_finish(float local, int bad, int lane, float inv_batch, unsigned int n_blocks,
@@ -646,6 +664,24 @@ __device__ __forceinline__ void nll_finish(float local, int bad, int lane, float
     if (status_out) *status_out = atomicAdd(reinterpret_cast<int*>(loss_acc + 1), 0);
   }
 }
+
+// Epilogue 3 of tcc::k_cluster (tc_cluster.cuh) for the h2 phase when it runs as a cluster: each output row goes through
+// nll_row as soon as the cluster has reduced it, and the grid publishes the loss as k_head_nll does — the output layer and
+// the NLL in one launch.  The row's other inputs (nll_row_in) are loaded before the mainloop, so that only the arithmetic
+// of the row follows the reduction.  No row-major copy of the outputs is written: in a training step nothing else reads it.
+struct NllRowEpi {
+  NllArgs A;
+  float* loss_acc; float* loss_out; int* status_out;
+  struct State { float local; int bad; };
+  using RowIn = NllRowIn;
+  __device__ __forceinline__ RowIn load(int64_t row) const { return nll_row_in(A, (int)row); }
+  __device__ __forceinline__ void row(State& s, const RowIn& in, const float* x, int64_t row, int lane) const {
+    nll_row(A, in, x, (int)row, lane, s.local, s.bad);
+  }
+  __device__ __forceinline__ void finish(const State& s, int lane) const {
+    nll_finish(s.local, s.bad, lane, A.inv_batch, gridDim.x, loss_acc, loss_out, status_out);
+  }
+};
 
 __global__ void __launch_bounds__(256) k_head_nll(const float* __restrict__ out_raw, NllArgs A, int R,
                                                    float* __restrict__ loss_acc, float* __restrict__ loss_out,
@@ -747,8 +783,69 @@ __global__ void __launch_bounds__(256, 4) k_head_out_nll(const float* __restrict
   nll_finish(local, bad, lane, A.inv_batch, gridDim.x * gridDim.y, loss_acc, loss_out, status_out);
 }
 
+// LSTM cell backward of one (row, unit) (torch.nn.LSTM gate order i, f, g, o): dht = dL/dh_t, dc_next = dL/dc_t carried back
+// from step t + 1 (0 without a successor), cp = c_{t-1}.  dv = dL/d(gate pre-activations); returns dL/dc_t.
+__device__ __forceinline__ float cell_bwd_unit(float ig, float fg, float gg, float og, float cn, float cp, float dht,
+                                               float dc_next, float (&dv)[4]) {
+  const float tc_ = ppb_cell_tanh(cn);
+  const float dct = dc_next + dht * og * (1.0f - tc_ * tc_);
+  dv[0] = dct * gg * ig * (1.0f - ig);
+  dv[1] = dct * cp * fg * (1.0f - fg);
+  dv[2] = dct * ig * (1.0f - gg * gg);
+  dv[3] = dht * tc_ * og * (1.0f - og);
+  return dct;
+}
+
+// tile-image stores of the four gate entries of unit j in image row `row`: with H % 32 == 0 the columns j + q H sit
+// gate_stride = (H / 32) column blocks apart in the image as well
+__device__ __forceinline__ void img_store_gates(const HImg& img, int64_t row, int j, int64_t gate_stride, const float (&v)[4]) {
+  const int64_t ok = tc::packed_offset(row, j, img.kb), omn = tc::packed_offset_mn(row, j, img.kb);
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    float hi, lo;
+    tc::split_tf32(v[q], hi, lo);
+    img.k_hi[ok + q * gate_stride] = hi;
+    if (img.k_lo) img.k_lo[ok + q * gate_stride] = lo;
+    if (img.mn_hi) {
+      img.mn_hi[omn + q * gate_stride] = hi;
+      if (img.mn_lo) img.mn_lo[omn + q * gate_stride] = lo;
+    }
+  }
+}
+
+// Epilogue 4 of tcc::k_cluster (tc_cluster.cuh) for the dh phase of a T = 1 step: the cell backward of (row, unit j) where the
+// cluster has reduced dh[row, j], so that neither dh nor a k_cell_bwd launch sits on the chain.  At T = 1 no row has a
+// successor (no dh_rec, no carried dc) and the trace's d_pobs is its one row's dgates; of d_pobs only the tile images are
+// read (the W_ih[:, :E] gradient and d obs_emb GEMMs), of dgates the fp32 rows (k_dgates_reduce).  H % 32 == 0, B % 128 == 0.
+struct CellBwdT1Epi {
+  const float* gates; const float* c; const int* row_trace;
+  float* dgates; HImg pimg; int H;
+  __device__ __forceinline__ void cells(int64_t row, int j0, const float (&dh)[4]) const {
+    const int tr = __ldg(row_trace + row);
+    const int64_t gate_stride = (int64_t)(H >> 5) * tc::kTileFloats;
+    float gv[4][4], cv[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {   // loads of all four units first
+      const int j = min(j0 + 32 * u, H - 1);   // columns >= H are loaded in range and not stored
+#pragma unroll
+      for (int q = 0; q < 4; ++q) gv[u][q] = __ldg(gates + row * 4 * H + q * H + j);
+      cv[u] = __ldg(c + row * H + j);
+    }
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const int j = j0 + 32 * u;
+      if (j >= H) continue;   // warp-uniform (H % 32 == 0)
+      float dv[4] = {0.f, 0.f, 0.f, 0.f};
+      if (tr >= 0) cell_bwd_unit(gv[u][0], gv[u][1], gv[u][2], gv[u][3], cv[u], 0.0f, dh[u], 0.0f, dv);
+#pragma unroll
+      for (int q = 0; q < 4; ++q) dgates[row * 4 * H + q * H + j] = dv[q];
+      if (tr >= 0) img_store_gates(pimg, tr, j, gate_stride, dv);
+    }
+  }
+};
+
 // LSTM cell backward, one time step (reverse order).  dgates rows of this step are produced here;
-// dh_rec = dgates[t+1] W_hh (prefix of this step's rows), dc carries d c_t across steps.
+// dh_rec = dgates[t+1] W_hh (prefix of this step's rows), dc carries d c_t across steps (dc == nullptr: not written, T = 1).
 // 8 blocks of 256 threads per SM: the 1024 blocks of a 512-row, H = 512 step are ONE wave (at 40 registers it was 6 per SM,
 // a second wave of 136 blocks, and the kernel went from 9.2 to 10.7 us)
 // FINAL (the t = 0 launch, which ends every trace's sum): the per-trace gradient d_pobs is also written as tile images
@@ -781,15 +878,10 @@ __global__ void __launch_bounds__(256, FINAL ? 4 : 8) k_cell_bwd(const float* __
       const float ig = g[0], fg = g[H], gg = g[2 * H], og = g[3 * H];
       const float cn = c[rH];
       const float cp = (t > 0) ? c[(int64_t)__ldg(row_prev + row) * H + j] : 0.0f;
-      const float tc_ = ppb_cell_tanh(cn);
       const bool has_next = nx >= 0;
       const float dht = dh[rH] + (has_next ? dh_rec[rH] : 0.0f);
-      const float dct = (has_next ? dc[(int64_t)nx * H + j] : 0.0f) + dht * og * (1.0f - tc_ * tc_);
-      dv[0] = dct * gg * ig * (1.0f - ig);
-      dv[1] = dct * cp * fg * (1.0f - fg);
-      dv[2] = dct * ig * (1.0f - gg * gg);
-      dv[3] = dht * tc_ * og * (1.0f - og);
-      dc[rH] = dct * fg;
+      const float dct = cell_bwd_unit(ig, fg, gg, og, cn, cp, dht, has_next ? dc[(int64_t)nx * H + j] : 0.0f, dv);
+      if (dc) dc[rH] = dct * fg;
       float* dp = d_pobs + (int64_t)tr * 4 * H + j;
       float tot[4];
 #pragma unroll
@@ -797,37 +889,13 @@ __global__ void __launch_bounds__(256, FINAL ? 4 : 8) k_cell_bwd(const float* __
         tot[q] = has_next ? dp[q * H] + dv[q] : dv[q];
         dp[q * H] = tot[q];
       }
-      if (FINAL && pimg.k_hi) {   // H % 32 == 0 on this path: the gate blocks sit gate_stride apart in the image as well
-        const int64_t pk = tc::packed_offset(tr, j, pimg.kb), pmn = tc::packed_offset_mn(tr, j, pimg.kb);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          float hi, lo;
-          tc::split_tf32(tot[q], hi, lo);
-          pimg.k_hi[pk + q * gate_stride] = hi;
-          if (pimg.k_lo) pimg.k_lo[pk + q * gate_stride] = lo;
-          if (pimg.mn_hi) {
-            pimg.mn_hi[pmn + q * gate_stride] = hi;
-            if (pimg.mn_lo) pimg.mn_lo[pmn + q * gate_stride] = lo;
-          }
-        }
-      }
+      if (FINAL && pimg.k_hi) img_store_gates(pimg, tr, j, gate_stride, tot);   // H % 32 == 0 on this path
     }
 #pragma unroll
     for (int q = 0; q < 4; ++q) dgr[q * H] = dv[q];
     if (gimg.k_hi) {
       if (h32) {
-        const int64_t ok = tc::packed_offset(row, j, gimg.kb), omn = tc::packed_offset_mn(row, j, gimg.kb);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          float hi, lo;
-          tc::split_tf32(dv[q], hi, lo);
-          gimg.k_hi[ok + q * gate_stride] = hi;
-          if (gimg.k_lo) gimg.k_lo[ok + q * gate_stride] = lo;
-          if (gimg.mn_hi) {
-            gimg.mn_hi[omn + q * gate_stride] = hi;
-            if (gimg.mn_lo) gimg.mn_lo[omn + q * gate_stride] = lo;
-          }
-        }
+        img_store_gates(gimg, row, j, gate_stride, dv);
       } else {
 #pragma unroll
         for (int q = 0; q < 4; ++q)

@@ -13,6 +13,14 @@
 // Epilogues (reduce phase; one thread owns one row x four columns {lane, lane+32, lane+64, lane+96} of the tile):
 //   k_cluster<X3, CS, 0>   fp32 store (+bias, ReLU, zero-invalid rows)           head dX
 //   k_cluster<X3, CS, 2>   tile images (+fp32, ReLU-mask from an image)          head hidden layer and its gradient
+//   k_cluster<X3, CS, 3, RE> whole-row epilogue of a caller type RE (N <= 128: one warp holds a whole output row): what
+//                          re.load(row) returns is fetched before the mainloop; the bias-added row goes to a per-warp
+//                          shared-memory buffer and re.row(state, loaded, x, row, lane) reads it as one warp; then EVERY
+//                          thread calls re.finish(state, lane) (it may hold CTA barriers)
+//                                                                                head output layer + NLL
+//   k_cluster<X3, CS, 4, RE> element epilogue: re.cells(row, col0, v) gets a thread's four sums (columns col0 + 32 g)
+//                                                                                T = 1 dh + LSTM cell backward
+//   No fp32 store in 3 and 4: the caller's routine writes what its consumers read.
 //   k_lstm_cluster<X3, CS> LSTM cell: with gate-interleaved W_hh the four columns of a thread are the gates i, f, g, o
 //                          of ONE hidden unit, so the cell update is thread-local (tc_lstm.cuh has the layout)
 // Mainloop, descriptors, the 3xTF32 scheme: tc_grouped.cuh.
@@ -138,9 +146,12 @@ __device__ __forceinline__ void common_setup(Smem& sm, int warp, int lane, bool 
 
 // ---- generic flavours -------------------------------------------------------------------------------------------------
 // grid = (sum of tiles) * CS, cluster (CS, 1, 1): blockIdx.x / CS = tile, %cluster_ctarank = K-split.
-template <bool X3, int CS, int EPI>
+struct NoRowEpi {};   // RE of the epilogues 0 and 2
+template <typename RE, int EPI> struct RowInOf { struct type {}; };
+template <typename RE> struct RowInOf<RE, 3> { using type = typename RE::RowIn; };
+template <bool X3, int CS, int EPI, typename RE = NoRowEpi>
 __global__ void __launch_bounds__(tcg::kThreads, 1) k_cluster(const tcg::Problem* __restrict__ probs, int n_probs,
-                                                                 unsigned long long* __restrict__ trace) {
+                                                                 unsigned long long* __restrict__ trace, const RE re) {
   if (threadIdx.x == 0) TCC_TRACE(0);
   extern __shared__ uint8_t smem_raw[];
   Smem& sm = *reinterpret_cast<Smem*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -162,10 +173,64 @@ __global__ void __launch_bounds__(tcg::kThreads, 1) k_cluster(const tcg::Problem
   const int c0 = (int)((int64_t)KC * split / CS), c1 = (int)((int64_t)KC * (split + 1) / CS);
   common_setup(sm, warp, lane);
   if (threadIdx.x == 0) TCC_TRACE(1);
+  constexpr int kRowsPerCta = 128 / CS, kRowsPerWarp = kRowsPerCta / tcg::kEpiWarps;
+  // epilogue 3: the inputs of the row routine that do not depend on the product are loaded while the operands stream in
+  typename RowInOf<RE, EPI>::type rin[kRowsPerWarp];
+  if constexpr (EPI == 3) {
+    if (warp < tcg::kEpiWarps) {
+#pragma unroll
+      for (int rr = 0; rr < kRowsPerWarp; ++rr)   // every row of a tile exists (M is a multiple of 128)
+        rin[rr] = re.load(P.o_row0 + mt * 128 + split * kRowsPerCta + warp * kRowsPerWarp + rr);
+    }
+  }
   mainloop_and_park<X3>(sm, P.a, P.b, mt, nt, c0, c1, warp, lane, trace);
 
-  if (warp < tcg::kEpiWarps) {
-    constexpr int kRowsPerCta = 128 / CS, kRowsPerWarp = kRowsPerCta / tcg::kEpiWarps;
+  if constexpr (EPI == 3) {
+    // the sums of all rows of the warp first (their remote loads overlap), then one row at a time through the buffer: the
+    // B stages are idle once the mainloop is through, and the parked partials live in the A stages
+    typename RE::State rs{};
+    if (warp < tcg::kEpiWarps) {
+      const int pM = P.M, pN = P.N;
+      const int64_t orow0 = P.o_row0;
+      float bias[4];
+#pragma unroll
+      for (int g = 0; g < 4; ++g) bias[g] = (P.bias && g * 32 + lane < pN) ? __ldg(P.bias + g * 32 + lane) : 0.0f;
+      float r_x[kRowsPerWarp][4];
+#pragma unroll
+      for (int rr = 0; rr < kRowsPerWarp; ++rr) {
+        float v[4];
+        reduce_row<CS>(sm, split * kRowsPerCta + warp * kRowsPerWarp + rr, lane, v);
+#pragma unroll
+        for (int g = 0; g < 4; ++g) r_x[rr][g] = g * 32 + lane < pN ? v[g] + bias[g] : 0.0f;
+      }
+      float* const xrow = sm.b_hi[0] + warp * 128;
+#pragma unroll
+      for (int rr = 0; rr < kRowsPerWarp; ++rr) {
+        const int m = mt * 128 + split * kRowsPerCta + warp * kRowsPerWarp + rr;
+        if (m >= pM) continue;   // warp-uniform
+#pragma unroll
+        for (int g = 0; g < 4; ++g) xrow[g * 32 + lane] = r_x[rr][g];
+        __syncwarp();
+        re.row(rs, rin[rr], xrow, orow0 + m, lane);
+        __syncwarp();
+      }
+    }
+    re.finish(rs, lane);
+  } else if constexpr (EPI == 4) {
+    if (warp < tcg::kEpiWarps) {
+      const int pM = P.M;
+      const int64_t orow0 = P.o_row0;
+      float r_v[kRowsPerWarp][4];
+#pragma unroll
+      for (int rr = 0; rr < kRowsPerWarp; ++rr) reduce_row<CS>(sm, split * kRowsPerCta + warp * kRowsPerWarp + rr, lane, r_v[rr]);
+#pragma unroll
+      for (int rr = 0; rr < kRowsPerWarp; ++rr) {
+        const int m = mt * 128 + split * kRowsPerCta + warp * kRowsPerWarp + rr;
+        if (m < pM) re.cells(orow0 + m, nt * 128 + lane, r_v[rr]);
+      }
+    }
+  }
+  if (EPI <= 2 && warp < tcg::kEpiWarps) {
     const int ew = warp;
     const bool do_relu = (P.flags & tcg::kRelu) != 0, do_mask = (P.flags & tcg::kMaskImg) != 0;
     const int m_valid = (P.flags & tcg::kZeroInvalid) ? P.m_valid : P.M;

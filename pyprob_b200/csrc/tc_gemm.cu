@@ -85,7 +85,7 @@ int launch_single_cluster(const tcg::Problem& hp, cudaStream_t st) {
   if (!g_dev_problem) PPB_CUDA(cudaMalloc((void**)&g_dev_problem, sizeof(tcg::Problem)));
   PPB_CUDA(cudaMemcpyAsync(g_dev_problem, &hp, sizeof(hp), cudaMemcpyHostToDevice, st));
   PPB_CUDA(tcc::launch_cluster(tcc::k_cluster<X3, CS, 0>, hp.tiles_m * hp.tiles_n * CS, CS, tcc::smem_bytes(), st,
-                               (const tcg::Problem*)g_dev_problem, 1, (unsigned long long*)nullptr));
+                               (const tcg::Problem*)g_dev_problem, 1, (unsigned long long*)nullptr, tcc::NoRowEpi{}));
   PPB_LAUNCH_CHECK();
   return PPB_OK;
 }
