@@ -180,7 +180,16 @@ typedef struct {
   ppb_ff_desc obs_ff[PPB_MAX_OBS]; /* per-observable embedding (inference_network.py:117)   */
   ppb_ff_desc obs_final;  /* _layers_observe_embedding_final, E->E->E (:129)                */
   int64_t w_ih_off, w_hh_off, b_ih_off, b_hh_off; /* nn.LSTM(I,H,1): [4H,I],[4H,H],[4H],[4H]   */
+  int32_t network_type;   /* PPB_NET_*; 0 (zero-initialised callers) = the LSTM network         */
+  int32_t reserved_;
 } ppb_net_desc;
+
+/* ppb_net_desc.network_type.  PPB_NET_FEEDFORWARD is InferenceNetworkFeedForward
+ * (pyprob/nn/inference_network_feedforward.py:13-98): every proposal head reads the observation embedding directly, so
+ * lstm_dim, sample_dim, addr_dim and type_dim are 0, the LSTM offsets are ignored, and a head's first layer is
+ * Linear(E -> head_hidden) with head_hidden = int((E + out) / 2). */
+#define PPB_NET_LSTM 0
+#define PPB_NET_FEEDFORWARD 1
 
 typedef struct {
   int32_t family;         /* PPB_FAMILY_*                                                    */
@@ -198,7 +207,9 @@ typedef struct ppb_net ppb_net; /* opaque: device copies of the tables above */
 
 int ppb_net_create(ppb_net** out, const ppb_net_desc* desc_host);
 /* (Re)load the address table and the type-embedding offsets after _polymorph grew the network
- * (inference_network_lstm.py:34-80).  type_emb_off_host[n_types] are arena offsets of [type_dim]. */
+ * (inference_network_lstm.py:34-80, inference_network_feedforward.py:21-51).  type_emb_off_host[n_types] are arena
+ * offsets of [type_dim].  A feed-forward net takes n_types = 0 (type_emb_off_host may be NULL) and ignores
+ * addr_emb_off, smp_* and type_id; its w1 is [head_hidden, E]. */
 int ppb_net_set_tables(ppb_net* net, const ppb_addr_desc* addrs_host, int32_t n_addrs,
                        const int64_t* type_emb_off_host, int32_t n_types, int64_t arena_floats);
 int ppb_net_destroy(ppb_net* net);
@@ -274,7 +285,9 @@ int64_t ppb_sizeof(int which);
 
 int64_t ppb_ic_workspace_bytes(const ppb_net* net, int32_t n_traces, int32_t n_rows, int32_t t_max,
                                int32_t n_steps, int32_t n_groups);
-/* loss = sum over rows of -log q(value | h_row) / n_traces  (inference_network_lstm.py:218-220);
+/* Both calls dispatch on the net's network_type; a feed-forward net's workspace holds no LSTM buffers.
+ * loss = sum over rows of -log q(value | h_row) / n_traces  (inference_network_lstm.py:218-220; feed-forward:
+ * inference_network_feedforward.py:68-98, h_row = the observation embedding of the row's trace);
  * -inf log-probs are replaced by log(1e-8) with zero gradient (:207-217, util.py:278-284).
  * status_out[0] = number of rows whose log-prob is NaN/+inf after the repair (reference returns
  * (False, 0) when that is non-zero).  row_lp_out (nullable) fp32[R] per-row log q. */
@@ -355,7 +368,10 @@ int ppb_dp_adam_step(int world, int rank, void* const* peer_blocks /* host array
  * lock-step at the same address).  h/c: fp32[n,H] LSTM state, updated in place (zeros at t=0).
  * prev_addr < 0 means first step.  Writes the proposal parameters:
  *   mixtures: params_out[n, 3K] = (means | stddevs | probs), categorical: params_out[n, C] = probs,
- *   bernoulli: params_out[n, 1] = probs. */
+ *   bernoulli: params_out[n, 1] = probs.
+ * Feed-forward net (inference_network_feedforward.py:53-66): prev_addr and prev_value are ignored, h and c may be NULL;
+ * the head runs on the one shared observation row and its output is expanded over the n particles (only the priors
+ * differ per particle). */
 int ppb_ic_infer_step(ppb_net* net, const float* arena, const float* obs_emb /*[n or 1, E]*/,
                       int obs_emb_row_stride, int32_t prev_addr, const float* prev_value,
                       int32_t cur_addr, const float* prior0, int prior0_stride, const float* prior1,

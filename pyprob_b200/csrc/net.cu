@@ -144,6 +144,9 @@ Ws carve(const ppb_net* net, Dims d, void* base) {
     return r;
   };
   const int H = D.lstm_dim, E = D.obs_dim, S = D.sample_dim, C2 = 2 * (D.type_dim + D.addr_dim);
+  // h / dh: the rows the heads read and their gradient — the LSTM output, or (feed-forward, fp32 path) the observation
+  // embedding of each row's trace.  A feed-forward net has H = S = C2 = 0: none of the LSTM buffers take space.
+  const int HX = D.network_type == PPB_NET_FEEDFORWARD ? E : H;
   for (int j = 0; j < D.num_obs; ++j)
     for (int l = 0; l + 1 < D.obs_ff[j].num_layers; ++l) w.obs_act[j][l] = take((int64_t)d.B * D.obs_ff[j].layers[l].out_dim);
   w.obs_cat = take((int64_t)d.B * E);
@@ -156,14 +159,14 @@ Ws carve(const ppb_net* net, Dims d, void* base) {
   w.smp_emb = take((int64_t)d.R * S);
   w.gates = take((int64_t)d.R * 4 * H);
   w.c = take((int64_t)d.R * H);
-  w.h = take((int64_t)d.R * H);
+  w.h = take((int64_t)d.R * HX);
   w.hid = take((int64_t)d.R * net->dh_pad);
   w.out_raw = take((int64_t)d.R * net->out_pad);
   w.row_lp = take(d.R);
   w.d_out = take((int64_t)d.R * net->out_pad);
   w.loss_acc = take(64);
   w.d_hid = take((int64_t)d.R * net->dh_pad);
-  w.dh = take((int64_t)d.R * H);
+  w.dh = take((int64_t)d.R * HX);
   w.dh_rec = take((int64_t)d.R * H);
   w.dc = take((int64_t)d.R * H);
   w.d_pobs = take((int64_t)d.B * 4 * H);
@@ -1240,16 +1243,104 @@ int check_batch(const ppb_net* net, const ppb_batch* b) {
   return PPB_OK;
 }
 
+// ---- proposal heads on the fp32 path, shared by the LSTM and the feed-forward networks ------------------------------------
+// The heads read w.h [R, kx]: the LSTM output, or the observation embedding of each row's trace.
+// Forward phases: hid = relu(h W1^T + b1), out_raw = hid W2^T + b2 (one problem per address group)
+void simt_head_fwd(Builder& bl, const ppb_net* net, const float* arena, const ppb_batch* b, const Ws& w, int kx, int& ph_h1,
+                   int& ph_h2) {
+  const int G = b->n_groups;
+  ph_h1 = (int)bl.phases.size();
+  bl.begin();
+  for (int g = 0; g < G; ++g) {
+    const ppb_addr_desc& a = net->addrs[b->group_addr_host[g]];
+    int s0 = b->group_start_host[g], cnt = b->group_start_host[g + 1] - s0;
+    Problem p = linear_fwd(w.h, kx, arena + a.w1_off, kx, arena + a.b1_off, w.hid, net->dh_pad, cnt, a.head_hidden, kx, gemm::kRelu);
+    p.m_gather = b->head_rows + s0;
+    bl.add(p);
+  }
+  ph_h2 = (int)bl.phases.size();
+  bl.begin();
+  for (int g = 0; g < G; ++g) {
+    const ppb_addr_desc& a = net->addrs[b->group_addr_host[g]];
+    int s0 = b->group_start_host[g], cnt = b->group_start_host[g + 1] - s0;
+    Problem p = linear_fwd(w.hid, net->dh_pad, arena + a.w2_off, a.head_hidden, arena + a.b2_off, w.out_raw, net->out_pad, cnt, a.head_out, a.head_hidden, 0);
+    p.m_gather = b->head_rows + s0;
+    bl.add(p);
+  }
+}
+
+// Runs the two head phases (uploaded to w.problems) and the NLL
+int simt_head_nll(const ppb_net* net, const ppb_batch* b, const Ws& w, const Builder& bl, int ph_h1, int ph_h2, float* loss_out,
+                  int32_t* status_out, float* row_lp_out, int want_grad, cudaStream_t st) {
+  int rc = run_phase(bl.phases[ph_h1], w.problems, st); if (rc) return rc;
+  rc = run_phase(bl.phases[ph_h2], w.problems, st); if (rc) return rc;
+  NllArgs na;
+  na.addrs = net->d_addrs; na.row_step = b->row_step; na.step_addr = b->step_addr;
+  na.values = b->values; na.prior0 = b->prior0; na.prior1 = b->prior1; na.row_trace = b->row_trace;
+  na.K = net->desc.mixture_k; na.inv_batch = 1.0f / (float)b->n_traces;
+  na.row_lp = row_lp_out ? row_lp_out : w.row_lp; na.d_out = want_grad ? w.d_out : nullptr; na.out_pad = net->out_pad;
+  na.dimg = HImg();
+  k_head_nll<<<ew_grid((int64_t)b->n_rows * 32, 256), 256, 0, st>>>(w.out_raw, na, b->n_rows, w.loss_acc, loss_out, status_out);
+  PPB_LAUNCH_CHECK();
+  return PPB_OK;
+}
+
+// Backward phases: d_hid = (d_out W2) * relu'(hid) ; then dW2 += d_out^T hid ; dW1 += d_hid^T h ; dh = d_hid W1
+void simt_head_bwd(Builder& bl, const ppb_net* net, const float* arena, float* grad, const ppb_batch* b, const Ws& w, int kx) {
+  const int G = b->n_groups;
+  bl.begin();
+  for (int g = 0; g < G; ++g) {
+    const ppb_addr_desc& a = net->addrs[b->group_addr_host[g]];
+    int s0 = b->group_start_host[g], cnt = b->group_start_host[g + 1] - s0;
+    Problem p = linear_dx(w.d_out, net->out_pad, arena + a.w2_off, a.head_hidden, w.d_hid, net->dh_pad, cnt, a.head_out, a.head_hidden, gemm::kMaskAux);
+    p.aux = w.hid; p.ld_aux = net->dh_pad; p.m_gather = b->head_rows + s0;
+    bl.add(p);
+  }
+  bl.begin();
+  for (int g = 0; g < G; ++g) {
+    const ppb_addr_desc& a = net->addrs[b->group_addr_host[g]];
+    int s0 = b->group_start_host[g], cnt = b->group_start_host[g + 1] - s0;
+    Problem p2 = linear_dw(w.d_out, net->out_pad, w.hid, net->dh_pad, grad + a.w2_off, a.head_hidden, cnt, a.head_out, a.head_hidden);
+    p2.ka_gather = b->head_rows + s0; p2.kb_gather = b->head_rows + s0;
+    bl.add(p2);
+    Problem p1 = linear_dw(w.d_hid, net->dh_pad, w.h, kx, grad + a.w1_off, kx, cnt, a.head_hidden, kx);
+    p1.ka_gather = b->head_rows + s0; p1.kb_gather = b->head_rows + s0;
+    bl.add(p1);
+    Problem px = linear_dx(w.d_hid, net->dh_pad, arena + a.w1_off, kx, w.dh, kx, cnt, a.head_hidden, kx, 0);
+    px.m_gather = b->head_rows + s0;
+    bl.add(px);
+  }
+}
+
+// head bias gradients
+int simt_head_bias_grad(const ppb_net* net, const ppb_batch* b, const Ws& w, float* grad, cudaStream_t st) {
+  for (int g = 0; g < b->n_groups; ++g) {
+    const ppb_addr_desc& a = net->addrs[b->group_addr_host[g]];
+    int s0 = b->group_start_host[g], cnt = b->group_start_host[g + 1] - s0;
+    k_colsum_gather<<<dim3((a.head_out + 31) / 32, 8), 256, 0, st>>>(w.d_out, net->out_pad, b->head_rows + s0, cnt, a.head_out, grad + a.b2_off);
+    PPB_LAUNCH_CHECK();
+    k_colsum_gather<<<dim3((a.head_hidden + 31) / 32, 8), 256, 0, st>>>(w.d_hid, net->dh_pad, b->head_rows + s0, cnt, a.head_hidden, grad + a.b1_off);
+    PPB_LAUNCH_CHECK();
+  }
+  return PPB_OK;
+}
+
 }  // namespace
 
 #include "net_tc.inc"
+#include "net_ff.inc"
 
 // =====================================================================================================
 extern "C" {
 
 int ppb_net_create(ppb_net** out, const ppb_net_desc* d) {
   PPB_CHECK_ARG(out && d, "null argument");
-  PPB_CHECK_ARG(d->lstm_dim > 0 && d->obs_dim > 0 && d->sample_dim > 0 && d->sample_dim <= 8, "bad dims");
+  PPB_CHECK_ARG(d->network_type == PPB_NET_LSTM || d->network_type == PPB_NET_FEEDFORWARD, "unknown network type");
+  if (d->network_type == PPB_NET_FEEDFORWARD)
+    PPB_CHECK_ARG(d->obs_dim > 0 && d->lstm_dim == 0 && d->sample_dim == 0 && d->addr_dim == 0 && d->type_dim == 0,
+                  "bad dims (a feed-forward net has obs_dim > 0 and no LSTM, sample, address or type embedding)");
+  else
+    PPB_CHECK_ARG(d->lstm_dim > 0 && d->obs_dim > 0 && d->sample_dim > 0 && d->sample_dim <= 8, "bad dims");
   PPB_CHECK_ARG(d->num_obs > 0 && d->num_obs <= PPB_MAX_OBS, "bad observable count");
   PPB_CHECK_ARG(d->mixture_k > 0 && d->mixture_k <= heads::KMAX, "mixture components must be in [1,32]");
   ppb_net* n = new ppb_net();
@@ -1273,7 +1364,8 @@ int ppb_net_create(ppb_net** out, const ppb_net_desc* d) {
 
 int ppb_net_set_tables(ppb_net* net, const ppb_addr_desc* addrs, int32_t n_addrs, const int64_t* type_off,
                        int32_t n_types, int64_t arena_floats) {
-  PPB_CHECK_ARG(net && addrs && type_off && n_addrs > 0 && n_types > 0, "bad arguments");
+  const bool ff = net && net->desc.network_type == PPB_NET_FEEDFORWARD;
+  PPB_CHECK_ARG(net && addrs && n_addrs > 0 && (ff ? n_types == 0 : (type_off && n_types > 0)), "bad arguments");
   net->addrs.assign(addrs, addrs + n_addrs);
   net->type_off.assign(type_off, type_off + n_types);
   net->arena_floats = arena_floats;
@@ -1284,7 +1376,7 @@ int ppb_net_set_tables(ppb_net* net, const ppb_addr_desc* addrs, int32_t n_addrs
                   "categorical head: 1..128 categories supported");
     PPB_CHECK_ARG(a.family != PPB_FAMILY_BERNOULLI || (a.head_out == 1 && a.smp_in == 1 && a.num_categories == 0),
                   "bernoulli head: head_out = 1, smp_in = 1, num_categories = 0");
-    PPB_CHECK_ARG(a.type_id >= 0 && a.type_id < n_types, "type id out of range");
+    PPB_CHECK_ARG(ff || (a.type_id >= 0 && a.type_id < n_types), "type id out of range");
     if (a.head_hidden > dh) dh = a.head_hidden;
     if (a.head_out > op) op = a.head_out;
   }
@@ -1292,10 +1384,13 @@ int ppb_net_set_tables(ppb_net* net, const ppb_addr_desc* addrs, int32_t n_addrs
   net->out_pad = (int)align_up(op, 4);
   if (net->d_addrs) cudaFree(net->d_addrs);
   if (net->d_type_off) cudaFree(net->d_type_off);
+  net->d_type_off = nullptr;
   PPB_CUDA(cudaMalloc((void**)&net->d_addrs, sizeof(ppb_addr_desc) * n_addrs));
-  PPB_CUDA(cudaMalloc((void**)&net->d_type_off, sizeof(int64_t) * n_types));
   PPB_CUDA(cudaMemcpy(net->d_addrs, addrs, sizeof(ppb_addr_desc) * n_addrs, cudaMemcpyHostToDevice));
-  PPB_CUDA(cudaMemcpy(net->d_type_off, type_off, sizeof(int64_t) * n_types, cudaMemcpyHostToDevice));
+  if (n_types > 0) {
+    PPB_CUDA(cudaMalloc((void**)&net->d_type_off, sizeof(int64_t) * n_types));
+    PPB_CUDA(cudaMemcpy(net->d_type_off, type_off, sizeof(int64_t) * n_types, cudaMemcpyHostToDevice));
+  }
   return build_weight_images(net);
 }
 
@@ -1344,6 +1439,8 @@ int ppb_ic_loss_forward(ppb_net* net, const float* arena, const ppb_batch* b, vo
   Dims d = dims_of(b);
   PPB_CHECK_ARG(workspace_bytes >= ppb_ic_workspace_bytes(net, d.B, d.R, d.T, d.NS, d.G), "workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
+  if (D.network_type == PPB_NET_FEEDFORWARD)
+    return ff_loss_forward(net, arena, b, workspace, precision, loss_out, status_out, row_lp_out, want_grad, st);
   if (precision != PPB_PREC_FP32_SIMT)
     return tc_loss_forward(net, arena, b, workspace, precision, loss_out, status_out, row_lp_out, want_grad, st);
   PPB_CHECK_ARG(b->row_align == 1, "the SIMT path needs a batch encoded with row_align = 1");
@@ -1366,24 +1463,8 @@ int ppb_ic_loss_forward(ppb_net* net, const float* arena, const ppb_batch* b, vo
     int r0 = b->row_off_host[t], n = b->row_off_host[t + 1] - r0, rp = b->row_off_host[t - 1];
     bl.add(linear_fwd(w.h + (int64_t)rp * H, H, arena + D.w_hh_off, H, nullptr, w.gates + (int64_t)r0 * H4, H4, n, H4, H, 0));
   }
-  const int ph_h1 = (int)bl.phases.size();
-  bl.begin();
-  for (int g = 0; g < d.G; ++g) {
-    const ppb_addr_desc& a = net->addrs[b->group_addr_host[g]];
-    int s0 = b->group_start_host[g], cnt = b->group_start_host[g + 1] - s0;
-    Problem p = linear_fwd(w.h, H, arena + a.w1_off, H, arena + a.b1_off, w.hid, net->dh_pad, cnt, a.head_hidden, H, gemm::kRelu);
-    p.m_gather = b->head_rows + s0;
-    bl.add(p);
-  }
-  const int ph_h2 = (int)bl.phases.size();
-  bl.begin();
-  for (int g = 0; g < d.G; ++g) {
-    const ppb_addr_desc& a = net->addrs[b->group_addr_host[g]];
-    int s0 = b->group_start_host[g], cnt = b->group_start_host[g + 1] - s0;
-    Problem p = linear_fwd(w.hid, net->dh_pad, arena + a.w2_off, a.head_hidden, arena + a.b2_off, w.out_raw, net->out_pad, cnt, a.head_out, a.head_hidden, 0);
-    p.m_gather = b->head_rows + s0;
-    bl.add(p);
-  }
+  int ph_h1, ph_h2;
+  simt_head_fwd(bl, net, arena, b, w, H, ph_h1, ph_h2);
   rc = upload_and_get(net, bl, w.problems, w.max_problems / 2, st, 0);
   if (rc) return rc;
 
@@ -1410,19 +1491,7 @@ int ppb_ic_loss_forward(ppb_net* net, const float* arena, const ppb_batch* b, vo
                                                        b->row_prev, b->row_trace, w.c, w.h, HImg(), r0, n, H, S, t);
     PPB_LAUNCH_CHECK();
   }
-  rc = run_phase(bl.phases[ph_h1], w.problems, st); if (rc) return rc;
-  rc = run_phase(bl.phases[ph_h2], w.problems, st); if (rc) return rc;
-  {
-    NllArgs na;
-    na.addrs = net->d_addrs; na.row_step = b->row_step; na.step_addr = b->step_addr;
-    na.values = b->values; na.prior0 = b->prior0; na.prior1 = b->prior1; na.row_trace = b->row_trace;
-    na.K = D.mixture_k; na.inv_batch = 1.0f / (float)d.B;
-    na.row_lp = row_lp_out ? row_lp_out : w.row_lp; na.d_out = want_grad ? w.d_out : nullptr; na.out_pad = net->out_pad;
-    na.dimg = HImg();
-    k_head_nll<<<ew_grid((int64_t)d.R * 32, 256), 256, 0, st>>>(w.out_raw, na, d.R, w.loss_acc, loss_out, status_out);
-  }
-  PPB_LAUNCH_CHECK();
-  return PPB_OK;
+  return simt_head_nll(net, b, w, bl, ph_h1, ph_h2, loss_out, status_out, row_lp_out, want_grad, st);
 }
 
 int ppb_ic_loss_backward(ppb_net* net, const float* arena, float* grad, const ppb_batch* b, void* workspace,
@@ -1434,6 +1503,7 @@ int ppb_ic_loss_backward(ppb_net* net, const float* arena, float* grad, const pp
   Dims d = dims_of(b);
   PPB_CHECK_ARG(workspace_bytes >= ppb_ic_workspace_bytes(net, d.B, d.R, d.T, d.NS, d.G), "workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
+  if (D.network_type == PPB_NET_FEEDFORWARD) return ff_loss_backward(net, arena, grad, b, workspace, precision, grad_scale, st);
   if (precision != PPB_PREC_FP32_SIMT) return tc_loss_backward(net, arena, grad, b, workspace, precision, grad_scale, st);
   Ws w = carve(net, d, workspace);
   float* dgates = dgates_ptr(w, workspace);
@@ -1446,31 +1516,8 @@ int ppb_ic_loss_backward(ppb_net* net, const float* arena, float* grad, const pp
   }
 
   Builder bl;
-  // heads: d_hid = (d_out W2) * relu'(hid) ; dW2 += d_out^T hid ; dh = d_hid W1 ; dW1 += d_hid^T h
-  const int ph_dhid = 0;
-  bl.begin();
-  for (int g = 0; g < d.G; ++g) {
-    const ppb_addr_desc& a = net->addrs[b->group_addr_host[g]];
-    int s0 = b->group_start_host[g], cnt = b->group_start_host[g + 1] - s0;
-    Problem p = linear_dx(w.d_out, net->out_pad, arena + a.w2_off, a.head_hidden, w.d_hid, net->dh_pad, cnt, a.head_out, a.head_hidden, gemm::kMaskAux);
-    p.aux = w.hid; p.ld_aux = net->dh_pad; p.m_gather = b->head_rows + s0;
-    bl.add(p);
-  }
-  const int ph_hw = 1;
-  bl.begin();
-  for (int g = 0; g < d.G; ++g) {
-    const ppb_addr_desc& a = net->addrs[b->group_addr_host[g]];
-    int s0 = b->group_start_host[g], cnt = b->group_start_host[g + 1] - s0;
-    Problem p2 = linear_dw(w.d_out, net->out_pad, w.hid, net->dh_pad, grad + a.w2_off, a.head_hidden, cnt, a.head_out, a.head_hidden);
-    p2.ka_gather = b->head_rows + s0; p2.kb_gather = b->head_rows + s0;
-    bl.add(p2);
-    Problem p1 = linear_dw(w.d_hid, net->dh_pad, w.h, H, grad + a.w1_off, H, cnt, a.head_hidden, H);
-    p1.ka_gather = b->head_rows + s0; p1.kb_gather = b->head_rows + s0;
-    bl.add(p1);
-    Problem px = linear_dx(w.d_hid, net->dh_pad, arena + a.w1_off, H, w.dh, H, cnt, a.head_hidden, H, 0);
-    px.m_gather = b->head_rows + s0;
-    bl.add(px);
-  }
+  const int ph_dhid = 0, ph_hw = 1;
+  simt_head_bwd(bl, net, arena, grad, b, w, H);
   // BPTT recurrent: dh_rec[prefix rows of t-1] = dgates[rows of t] W_hh
   const int ph_rec0 = 2;
   for (int t = d.T - 1; t >= 1; --t) {
@@ -1504,15 +1551,7 @@ int ppb_ic_loss_backward(ppb_net* net, const float* arena, float* grad, const pp
   // ---- launches -----------------------------------------------------------------------------------
   rc = run_phase(bl.phases[ph_dhid], dprobs, st); if (rc) return rc;
   rc = run_phase(bl.phases[ph_hw], dprobs, st); if (rc) return rc;
-  // head bias gradients
-  for (int g = 0; g < d.G; ++g) {
-    const ppb_addr_desc& a = net->addrs[b->group_addr_host[g]];
-    int s0 = b->group_start_host[g], cnt = b->group_start_host[g + 1] - s0;
-    k_colsum_gather<<<dim3((a.head_out + 31) / 32, 8), 256, 0, st>>>(w.d_out, net->out_pad, b->head_rows + s0, cnt, a.head_out, grad + a.b2_off);
-    PPB_LAUNCH_CHECK();
-    k_colsum_gather<<<dim3((a.head_hidden + 31) / 32, 8), 256, 0, st>>>(w.d_hid, net->dh_pad, b->head_rows + s0, cnt, a.head_hidden, grad + a.b1_off);
-    PPB_LAUNCH_CHECK();
-  }
+  rc = simt_head_bias_grad(net, b, w, grad, st); if (rc) return rc;
   // BPTT
   for (int t = d.T - 1; t >= 0; --t) {
     int r0 = b->row_off_host[t], n = b->row_off_host[t + 1] - r0;
@@ -1937,11 +1976,40 @@ int ppb_ic_infer_step(ppb_net* net, const float* arena, const float* obs_emb, in
                       const float* prev_value, int32_t cur_addr, const float* prior0, int prior0_stride,
                       const float* prior1, int prior1_stride, float* h, float* c, float* params_out, int64_t n,
                       void* workspace, int64_t workspace_bytes, int precision, void* stream) {
-  PPB_CHECK_ARG(net && arena && obs_emb && h && c && params_out && workspace && n > 0, "bad arguments");
+  const bool ff = net && net->desc.network_type == PPB_NET_FEEDFORWARD;
+  PPB_CHECK_ARG(net && arena && obs_emb && (ff || (h && c)) && params_out && workspace && n > 0, "bad arguments");
   PPB_CHECK_ARG(cur_addr >= 0 && cur_addr < (int)net->addrs.size(), "unknown current address");
+  PPB_CHECK_ARG(workspace_bytes >= ppb_ic_infer_workspace_bytes(net, n), "workspace too small");
+  if (ff) {
+    if (obs_emb_row_stride != 0) {
+      ppb_set_error("ppb_ic_infer_step: per-particle observation embeddings are not supported yet (stride must be 0)");
+      return PPB_ENOTSUP;
+    }
+    // inference_network_feedforward.py:53-66: the head of the current address on the observation embedding.  With one
+    // shared observation every particle's head output is the same: ONE row, expanded over the particles by k_head_params
+    // (row stride 0), which applies each particle's prior.
+    const ppb_net_desc& D = net->desc;
+    cudaStream_t st = (cudaStream_t)stream;
+    InferWs w = carve_infer(net, n, workspace);
+    const ppb_addr_desc cur = net->addrs[cur_addr];
+    const int E = D.obs_dim;
+    Builder bl;
+    bl.begin();
+    bl.add(linear_fwd(obs_emb, E, arena + cur.w1_off, E, arena + cur.b1_off, w.hid, net->dh_pad, 1, cur.head_hidden, E, gemm::kRelu));
+    bl.begin();
+    bl.add(linear_fwd(w.hid, net->dh_pad, arena + cur.w2_off, cur.head_hidden, arena + cur.b2_off, w.out_raw, net->out_pad, 1,
+                      cur.head_out, cur.head_hidden, 0));
+    int rc = upload_and_get(net, bl, w.problems, w.max_problems, st, 5);
+    if (rc) return rc;
+    rc = run_phase(bl.phases[0], w.problems, st); if (rc) return rc;
+    rc = run_phase(bl.phases[1], w.problems, st); if (rc) return rc;
+    k_head_params<<<ew_grid(n, 128), 128, 0, st>>>(w.out_raw, 0, cur, D.mixture_k, prior0, prior0_stride, prior1, prior1_stride,
+                                                   params_out, n);
+    PPB_LAUNCH_CHECK();
+    return PPB_OK;
+  }
   PPB_CHECK_ARG(prev_addr < (int)net->addrs.size(), "unknown previous address");
   PPB_CHECK_ARG(prev_addr < 0 || prev_value, "previous value missing");
-  PPB_CHECK_ARG(workspace_bytes >= ppb_ic_infer_workspace_bytes(net, n), "workspace too small");
   if (obs_emb_row_stride != 0) {
     ppb_set_error("ppb_ic_infer_step: per-particle observation embeddings are not supported yet (stride must be 0)");
     return PPB_ENOTSUP;

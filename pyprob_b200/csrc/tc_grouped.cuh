@@ -36,7 +36,10 @@ enum : int {
 struct Operand {
   const float* hi;
   const float* lo;
-  const int* k_rows;  // MN-major only: image row origin of each 32-row reduction chunk (null: row0 + 32 c)
+  const int* k_rows;  // MN-major: image row origin of each 32-row reduction chunk (null: row0 + 32 c)
+                      // K-major, read only by the chunk-table instantiation (KTAB): pairs (first M/N row [mult of
+                      // 128], column block) of each 32-column reduction chunk — a reduction over column ranges of
+                      // different row blocks of one image (null: row0, col0 / 32 + c)
   int kb;             // column blocks of the image
   int mn;             // 0 = K-major, 1 = MN-major
   int row0, col0;     // K-major: (first M/N row [mult of 128], first reduction col [mult of 32])
@@ -89,10 +92,12 @@ __device__ __forceinline__ uint32_t stage_bytes(const Operand& o, int tile_idx) 
   return (uint32_t)n * kPiece;
 }
 
+template <bool KTAB = false>
 __device__ __forceinline__ void load_operand(const Operand& o, int tile_idx, int chunk, float* s_hi, float* s_lo,
                                              bool x3, uint64_t* bar) {
   if (!o.mn) {
     int64_t rt = o.row0 / 128 + tile_idx, cb = o.col0 / 32 + chunk;
+    if (KTAB && o.k_rows) { rt = o.k_rows[2 * chunk] / 128 + tile_idx; cb = o.k_rows[2 * chunk + 1]; }
     int64_t off = (rt * o.kb + cb) * kTileFloats;
     bulk_g2s(s_hi, o.hi + off, kTileBytes, bar);
     if (x3) bulk_g2s(s_lo, o.lo + off, kTileBytes, bar);
@@ -207,7 +212,7 @@ __device__ __forceinline__ void store_acc(const float (&acc)[32], int warp, int 
 }
 
 // Bulk-TMA producer: streams n chunks (c0 .. c0 + n - 1, ring positions kc0 ..) of tile (mt, nt) into the ring.
-template <bool X3>
+template <bool X3, bool KTAB = false>
 __device__ __forceinline__ void produce(const Ring& R, const Operand& A, const Operand& B, int mt, int nt, int c0, int n,
                                         uint32_t kc0) {
   const uint32_t bytes = (stage_bytes(A, mt) + stage_bytes(B, nt)) * (X3 ? 2u : 1u);
@@ -217,7 +222,7 @@ __device__ __forceinline__ void produce(const Ring& R, const Operand& A, const O
     const uint32_t ph = (kc / (uint32_t)R.stages) & 1;
     mbar_wait(&R.empty[s], ph ^ 1);
     mbar_expect_tx(&R.full[s], bytes);
-    load_operand(A, mt, c0 + i, R.a_hi + s * R.stride, R.a_lo + s * R.stride, X3, &R.full[s]);
+    load_operand<KTAB>(A, mt, c0 + i, R.a_hi + s * R.stride, R.a_lo + s * R.stride, X3, &R.full[s]);
     load_operand(B, nt, c0 + i, R.b_hi + s * R.stride, R.b_lo + s * R.stride, X3, &R.full[s]);
   }
 }
@@ -228,7 +233,9 @@ __device__ __forceinline__ Ring ring_of(Smem& sm) {
 
 // EPI selects the (compile-time) epilogue flavour so that the row loop is straight-line code:
 //   0 = fp32 store (+bias, relu)   1 = fp32 reduction (red.add: weight gradients, split-K)   2 = tile images (+fp32)
-template <bool X3, int EPI>
+// KTAB: the A operand may be K-major with a chunk table (Operand::k_rows); a separate instantiation, so that the other
+// kernels keep their loader unchanged.
+template <bool X3, int EPI, bool KTAB = false>
 __global__ void __launch_bounds__(kThreads, 1) k_grouped(const Problem* __restrict__ probs, int n_probs,
                                                           unsigned long long* __restrict__ trace) {
 #define TCG_TRACE(slot)                                                                                   \
@@ -273,7 +280,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_grouped(const Problem* __restri
   const Ring R = ring_of(sm);
 
   if (warp == kProducerWarp) {
-    if (lane == 0) produce<X3>(R, P.a, P.b, mt, nt, c0, c1 - c0, 0);
+    if (lane == 0) produce<X3, KTAB>(R, P.a, P.b, mt, nt, c0, c1 - c0, 0);
   } else {
     float acc[32];
     mma_mainloop<X3>(R, 0, c1 - c0, P.a.mn != 0, P.b.mn != 0, warp, lane, acc);

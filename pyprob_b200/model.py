@@ -11,7 +11,7 @@ from . import ops, state, util
 from .dataset import OnlineDataset
 from .distributions import set_shard_first_index
 from .empirical import Empirical
-from .network import InferenceNetworkLSTM
+from .network import InferenceNetwork as _InferenceNetworkBase, InferenceNetworkFeedForward, InferenceNetworkLSTM
 from .offline import OfflineDataset
 from .util import InferenceEngine, InferenceNetwork, LearningRateScheduler, Optimizer, PriorInflation, TraceMode
 
@@ -161,8 +161,6 @@ class Model:
                                 distributed_backend=None, distributed_params_sync_every_iter=10000,
                                 distributed_num_buckets=None, dataloader_offline_num_workers=0, stop_with_bad_loss=True,
                                 log_file_name=None, lstm_dim=512, lstm_depth=1, proposal_mixture_components=10):
-        if inference_network != InferenceNetwork.LSTM:
-            raise NotImplementedError('pyprob_b200 implements InferenceNetwork.LSTM (the path north_star names)')
         names = list(observe_embeddings)   # dict (or set) of observable names
         if dataset_dir is None:
             dataset = OnlineDataset(model=self, prior_inflation=prior_inflation)
@@ -175,9 +173,16 @@ class Model:
             dataset_valid.select_observables(names if names else dataset_valid.observe_names)
         if self._inference_network is None:
             print('Creating new inference network...')
-            self._inference_network = InferenceNetworkLSTM(model=self, observe_embeddings=observe_embeddings,
-                                                           lstm_dim=lstm_dim, lstm_depth=lstm_depth,
-                                                           proposal_mixture_components=proposal_mixture_components)
+            if inference_network == InferenceNetwork.FEEDFORWARD:   # reference model.py:199-200
+                self._inference_network = InferenceNetworkFeedForward(
+                    model=self, observe_embeddings=observe_embeddings,
+                    proposal_mixture_components=proposal_mixture_components)
+            elif inference_network == InferenceNetwork.LSTM:
+                self._inference_network = InferenceNetworkLSTM(model=self, observe_embeddings=observe_embeddings,
+                                                               lstm_dim=lstm_dim, lstm_depth=lstm_depth,
+                                                               proposal_mixture_components=proposal_mixture_components)
+            else:
+                raise ValueError('Unknown inference_network: {}'.format(inference_network))
             if pre_generate_layers:
                 if dataset_valid is not None:
                     self._inference_network._pre_generate_layers(dataset_valid, batch_size=batch_size,
@@ -213,5 +218,5 @@ class Model:
         self._inference_network._save(file_name)
 
     def load_inference_network(self, file_name):
-        self._inference_network = InferenceNetworkLSTM._load(file_name)
+        self._inference_network = _InferenceNetworkBase._load(file_name)   # whichever network class was saved
         self._inference_network._model = self

@@ -1,7 +1,8 @@
-"""InferenceNetworkLSTM — host-side mirror of the reference network class for the CUDA hot path.
+"""InferenceNetworkLSTM and InferenceNetworkFeedForward — host-side mirrors of the reference network classes for the CUDA
+hot path.
 
-Same constructor keywords, attributes and method names as the reference
-(pyprob/nn/inference_network.py:24-78, pyprob/nn/inference_network_lstm.py:13-27) so that
+Same constructor keywords, attributes and method names as the reference (pyprob/nn/inference_network.py:24-78,
+pyprob/nn/inference_network_lstm.py:13-27, pyprob/nn/inference_network_feedforward.py:13-19) so that
 ``Model.learn_inference_network`` / ``posterior_results`` drive it unchanged, but:
 
 * all parameters live in ONE flat fp32 arena on the GPU (``_arena``), indexed by the reference's own
@@ -50,7 +51,11 @@ class NetDesc(C.Structure):
     _fields_ = [('lstm_dim', C.c_int32), ('obs_dim', C.c_int32), ('sample_dim', C.c_int32), ('addr_dim', C.c_int32),
                 ('type_dim', C.c_int32), ('mixture_k', C.c_int32), ('num_obs', C.c_int32), ('obs_in_total', C.c_int32),
                 ('obs_ff', FFDesc * MAX_OBS), ('obs_final', FFDesc),
-                ('w_ih_off', C.c_int64), ('w_hh_off', C.c_int64), ('b_ih_off', C.c_int64), ('b_hh_off', C.c_int64)]
+                ('w_ih_off', C.c_int64), ('w_hh_off', C.c_int64), ('b_ih_off', C.c_int64), ('b_hh_off', C.c_int64),
+                ('network_type', C.c_int32), ('reserved_', C.c_int32)]
+
+
+NET_LSTM, NET_FEEDFORWARD = 0, 1   # ppb_net_desc.network_type
 
 
 class AddrDesc(C.Structure):
@@ -91,24 +96,21 @@ class _LossFunction(torch.autograd.Function):
         return grad, None, None
 
 
-class InferenceNetworkLSTM(nn.Module):
-    def __init__(self, model=None, observe_embeddings={}, lstm_dim=512, lstm_depth=1, sample_embedding_dim=4,
-                 address_embedding_dim=64, distribution_type_embedding_dim=8, proposal_mixture_components=10,
-                 precision=0):
+class InferenceNetwork(nn.Module):
+    """What does not depend on the network type (reference pyprob/nn/inference_network.py): the parameter arena, the
+    observation layers, the loss call, the optimisers and the training loop, data-parallel training, checkpoints,
+    workspaces and `_infer_init`.  Subclasses add the proposal layers of an address (`_add_address`), the native
+    network description (`_fill_net_desc`, `_fill_addr_desc`), the infer step and `_segment_presence`."""
+
+    def __init__(self, model=None, observe_embeddings={}, proposal_mixture_components=10, precision=0,
+                 network_type=''):
         super().__init__()
-        if lstm_depth != 1:
-            raise NotImplementedError('pyprob_b200: lstm_depth != 1 is not implemented (reference default is 1)')
         self._model = model
-        self._network_type = 'InferenceNetworkLSTM'
+        self._network_type = network_type
         self._observe_embeddings = observe_embeddings
         self._observe_embedding_dim = None
         self._observe_names = []
         self._observe_in_dims = []
-        self._lstm_dim, self._lstm_depth = lstm_dim, lstm_depth
-        self._lstm_input_dim = None
-        self._sample_embedding_dim = sample_embedding_dim
-        self._address_embedding_dim = address_embedding_dim
-        self._distribution_type_embedding_dim = distribution_type_embedding_dim
         self._proposal_mixture_components = proposal_mixture_components
         self._precision = precision
         self._layers_initialized = False
@@ -276,15 +278,18 @@ class InferenceNetworkLSTM(nn.Module):
         self._final_ff = self._ff('_layers_observe_embedding_final', total, total, 2)
 
     def _init_layers(self):
-        E = self._observe_embedding_dim
-        self._lstm_input_dim = E + self._sample_embedding_dim + 2 * (self._address_embedding_dim +
-                                                                     self._distribution_type_embedding_dim)
-        ref = nn.LSTM(self._lstm_input_dim, self._lstm_dim, 1)
-        self._alloc('_layers_lstm.weight_ih_l0', (4 * self._lstm_dim, self._lstm_input_dim), ref.weight_ih_l0)
-        self._alloc('_layers_lstm.weight_hh_l0', (4 * self._lstm_dim, self._lstm_dim), ref.weight_hh_l0)
-        self._alloc('_layers_lstm.bias_ih_l0', (4 * self._lstm_dim,), ref.bias_ih_l0)
-        self._alloc('_layers_lstm.bias_hh_l0', (4 * self._lstm_dim,), ref.bias_hh_l0)
         self._rebind()
+
+    def _proposal_layers(self, address, family, num_categories, in_dim):
+        """The proposal head of an address (proposal_*.py: EmbeddingFeedForward(in_dim -> out, 2 layers)) -> its info."""
+        K = self._proposal_mixture_components
+        # proposal_categorical_categorical.py: C logits; proposal_bernoulli_bernoulli.py: one logit; mixtures: 3K
+        out = num_categories if family == FAMILY_CATEGORICAL else 1 if family == FAMILY_BERNOULLI else 3 * K
+        hidden = int((in_dim + out) / 2)
+        p = '_layers_proposal.{}._ff._layers'.format(address)
+        self._linear(p + '.0', in_dim, hidden)
+        self._linear(p + '.1', hidden, out)
+        return dict(head_hidden=hidden, head_out=out)
 
     def _ensure_initialized(self, example_trace):
         if not self._layers_initialized:
@@ -292,31 +297,6 @@ class InferenceNetworkLSTM(nn.Module):
             self._init_layers_observe_embedding(self._observe_embeddings, example_trace)
             self._init_layers()
             self._layers_initialized = True
-
-    def _add_address(self, address, dist_name, num_categories=0):
-        """New address: address/type embeddings, sample-embedding layer, proposal head (:42-72)."""
-        if dist_name not in _FAMILY_OF:
-            raise RuntimeError('Distribution currently unsupported: {}'.format(dist_name))
-        H, K = self._lstm_dim, self._proposal_mixture_components
-        family = _FAMILY_OF[dist_name]
-        self._alloc('_layers_address_embedding.{}'.format(address), (self._address_embedding_dim,),
-                    torch.zeros(self._address_embedding_dim).normal_())
-        if dist_name not in self._types:
-            self._alloc('_layers_distribution_type_embedding.{}'.format(dist_name),
-                        (self._distribution_type_embedding_dim,),
-                        torch.zeros(self._distribution_type_embedding_dim).normal_())
-            self._types[dist_name] = len(self._types)
-        # proposal_categorical_categorical.py: C logits; proposal_bernoulli_bernoulli.py: one logit; mixtures: 3K
-        out = num_categories if family == FAMILY_CATEGORICAL else 1 if family == FAMILY_BERNOULLI else 3 * K
-        hidden = int((H + out) / 2)
-        p = '_layers_proposal.{}._ff._layers'.format(address)
-        self._linear(p + '.0', H, hidden)
-        self._linear(p + '.1', hidden, out)
-        smp_in = num_categories if family == FAMILY_CATEGORICAL else 1
-        self._linear('_layers_sample_embedding.{}._layers.0'.format(address), smp_in, self._sample_embedding_dim)
-        self._addresses[address] = dict(id=len(self._addresses), family=family, num_categories=num_categories,
-                                        head_hidden=hidden, head_out=out, smp_in=smp_in, type=dist_name)
-        self._head_iterations[address] = 0
 
     def _polymorph(self, batch):
         """Create layers for addresses not seen before; returns True if the network changed."""
@@ -358,17 +338,12 @@ class InferenceNetworkLSTM(nn.Module):
         if self._handle is None:
             check_abi_struct_sizes()
             nd = NetDesc()
-            nd.lstm_dim, nd.obs_dim = self._lstm_dim, self._observe_embedding_dim
-            nd.sample_dim, nd.addr_dim = self._sample_embedding_dim, self._address_embedding_dim
-            nd.type_dim, nd.mixture_k = self._distribution_type_embedding_dim, self._proposal_mixture_components
+            nd.obs_dim, nd.mixture_k = self._observe_embedding_dim, self._proposal_mixture_components
             nd.num_obs, nd.obs_in_total = len(self._obs_ff), int(sum(self._observe_in_dims))
             for j, layers in enumerate(self._obs_ff):
                 nd.obs_ff[j] = self._ff_desc(layers)
             nd.obs_final = self._ff_desc(self._final_ff)
-            nd.w_ih_off = self.parameter_index['_layers_lstm.weight_ih_l0'][0]
-            nd.w_hh_off = self.parameter_index['_layers_lstm.weight_hh_l0'][0]
-            nd.b_ih_off = self.parameter_index['_layers_lstm.bias_ih_l0'][0]
-            nd.b_hh_off = self.parameter_index['_layers_lstm.bias_hh_l0'][0]
+            self._fill_net_desc(nd)
             h = C.c_void_p()
             call('ppb_net_create', C.byref(h), C.byref(nd))
             self._handle = h
@@ -380,11 +355,8 @@ class InferenceNetworkLSTM(nn.Module):
                 a = arr[info['id']]
                 a.family, a.num_categories = info['family'], info['num_categories']
                 a.head_hidden, a.head_out, a.smp_in = info['head_hidden'], info['head_out'], info['smp_in']
-                a.type_id = self._types[info['type']]
                 pi = self.parameter_index
-                a.addr_emb_off = pi['_layers_address_embedding.{}'.format(address)][0]
-                a.smp_w_off = pi['_layers_sample_embedding.{}._layers.0.weight'.format(address)][0]
-                a.smp_b_off = pi['_layers_sample_embedding.{}._layers.0.bias'.format(address)][0]
+                self._fill_addr_desc(a, address, info)
                 a.w1_off = pi['_layers_proposal.{}._ff._layers.0.weight'.format(address)][0]
                 a.b1_off = pi['_layers_proposal.{}._ff._layers.0.bias'.format(address)][0]
                 a.w2_off = pi['_layers_proposal.{}._ff._layers.1.weight'.format(address)][0]
@@ -392,7 +364,8 @@ class InferenceNetworkLSTM(nn.Module):
             toff = (C.c_int64 * len(self._types))()
             for name, tid in self._types.items():
                 toff[tid] = self.parameter_index['_layers_distribution_type_embedding.{}'.format(name)][0]
-            call('ppb_net_set_tables', self._handle, arr, n, toff, len(self._types), self._arena_used)
+            call('ppb_net_set_tables', self._handle, arr, n, toff if len(self._types) else None, len(self._types),
+                 self._arena_used)
             self._tables_dirty = False
 
     def __getstate__(self):
@@ -529,34 +502,6 @@ class InferenceNetworkLSTM(nn.Module):
 
     def _segment_names(self):
         return sorted(self.parameter_index, key=lambda k: self.parameter_index[k][0])
-
-    def _segment_presence(self, enc, force=False):
-        """int32[S]: 1 for every parameter tensor that took part in the forward pass of the encoded minibatch, i.e.
-        whose .grad the reference's autograd would populate (all others stay None and are skipped by torch.optim):
-        shared layers always; address / type embeddings and the proposal head of every address in the batch; the
-        sample-embedding layer of every address that is some step's PREVIOUS address (inference_network_lstm.py:
-        150-182)."""
-        names = self._seg['names'] if self._seg is not None else self._segment_names()
-        present = np.ones(len(names), dtype=np.int32)
-        if (not self._skip_absent_gradients and not force) or enc is None:
-            return present
-        by_id = {info['id']: (a, info) for a, info in self._addresses.items()}
-        cur = set(int(i) for i in np.unique(enc.arrays['step_addr']))
-        prev = set(int(i) for i in np.unique(enc.arrays['step_prev_addr']) if i >= 0)
-        types = set(by_id[i][1]['type'] for i in cur | prev)
-        for k, name in enumerate(names):
-            if name.startswith('_layers_address_embedding.'):
-                a = name[len('_layers_address_embedding.'):]
-                present[k] = int(self._addresses[a]['id'] in cur)
-            elif name.startswith('_layers_distribution_type_embedding.'):
-                present[k] = int(name[len('_layers_distribution_type_embedding.'):] in types)
-            elif name.startswith('_layers_proposal.'):
-                a = name[len('_layers_proposal.'):name.index('._ff._layers.')]
-                present[k] = int(self._addresses[a]['id'] in cur)
-            elif name.startswith('_layers_sample_embedding.'):
-                a = name[len('_layers_sample_embedding.'):name.index('._layers.')]
-                present[k] = int(self._addresses[a]['id'] in prev)
-        return present
 
     def _segmented_optimizer_step(self, grad_scale):
         seg = self._seg
@@ -923,6 +868,83 @@ class InferenceNetworkLSTM(nn.Module):
             self._by_id_cache = cache
         return cache
 
+
+class InferenceNetworkLSTM(InferenceNetwork):
+    """pyprob/nn/inference_network_lstm.py: observation embedding, previous-sample / address / type embeddings -> LSTM ->
+    the proposal head of each step's address."""
+
+    def __init__(self, model=None, observe_embeddings={}, lstm_dim=512, lstm_depth=1, sample_embedding_dim=4,
+                 address_embedding_dim=64, distribution_type_embedding_dim=8, proposal_mixture_components=10,
+                 precision=0):
+        if lstm_depth != 1:
+            raise NotImplementedError('pyprob_b200: lstm_depth != 1 is not implemented (reference default is 1)')
+        super().__init__(model=model, observe_embeddings=observe_embeddings,
+                         proposal_mixture_components=proposal_mixture_components, precision=precision,
+                         network_type='InferenceNetworkLSTM')
+        self._lstm_dim, self._lstm_depth = lstm_dim, lstm_depth
+        self._lstm_input_dim = None
+        self._sample_embedding_dim = sample_embedding_dim
+        self._address_embedding_dim = address_embedding_dim
+        self._distribution_type_embedding_dim = distribution_type_embedding_dim
+
+    def _init_layers(self):
+        E = self._observe_embedding_dim
+        self._lstm_input_dim = E + self._sample_embedding_dim + 2 * (self._address_embedding_dim +
+                                                                     self._distribution_type_embedding_dim)
+        ref = nn.LSTM(self._lstm_input_dim, self._lstm_dim, 1)
+        self._alloc('_layers_lstm.weight_ih_l0', (4 * self._lstm_dim, self._lstm_input_dim), ref.weight_ih_l0)
+        self._alloc('_layers_lstm.weight_hh_l0', (4 * self._lstm_dim, self._lstm_dim), ref.weight_hh_l0)
+        self._alloc('_layers_lstm.bias_ih_l0', (4 * self._lstm_dim,), ref.bias_ih_l0)
+        self._alloc('_layers_lstm.bias_hh_l0', (4 * self._lstm_dim,), ref.bias_hh_l0)
+        self._rebind()
+
+    def _add_address(self, address, dist_name, num_categories=0):
+        """New address: address/type embeddings, sample-embedding layer, proposal head (:42-72)."""
+        if dist_name not in _FAMILY_OF:
+            raise RuntimeError('Distribution currently unsupported: {}'.format(dist_name))
+        family = _FAMILY_OF[dist_name]
+        self._alloc('_layers_address_embedding.{}'.format(address), (self._address_embedding_dim,),
+                    torch.zeros(self._address_embedding_dim).normal_())
+        if dist_name not in self._types:
+            self._alloc('_layers_distribution_type_embedding.{}'.format(dist_name),
+                        (self._distribution_type_embedding_dim,),
+                        torch.zeros(self._distribution_type_embedding_dim).normal_())
+            self._types[dist_name] = len(self._types)
+        head = self._proposal_layers(address, family, num_categories, self._lstm_dim)
+        smp_in = num_categories if family == FAMILY_CATEGORICAL else 1
+        self._linear('_layers_sample_embedding.{}._layers.0'.format(address), smp_in, self._sample_embedding_dim)
+        self._addresses[address] = dict(id=len(self._addresses), family=family, num_categories=num_categories,
+                                        smp_in=smp_in, type=dist_name, **head)
+        self._head_iterations[address] = 0
+
+    def _segment_presence(self, enc, force=False):
+        """int32[S]: 1 for every parameter tensor that took part in the forward pass of the encoded minibatch, i.e.
+        whose .grad the reference's autograd would populate (all others stay None and are skipped by torch.optim):
+        shared layers always; address / type embeddings and the proposal head of every address in the batch; the
+        sample-embedding layer of every address that is some step's PREVIOUS address (inference_network_lstm.py:
+        150-182)."""
+        names = self._seg['names'] if self._seg is not None else self._segment_names()
+        present = np.ones(len(names), dtype=np.int32)
+        if (not self._skip_absent_gradients and not force) or enc is None:
+            return present
+        by_id = {info['id']: (a, info) for a, info in self._addresses.items()}
+        cur = set(int(i) for i in np.unique(enc.arrays['step_addr']))
+        prev = set(int(i) for i in np.unique(enc.arrays['step_prev_addr']) if i >= 0)
+        types = set(by_id[i][1]['type'] for i in cur | prev)
+        for k, name in enumerate(names):
+            if name.startswith('_layers_address_embedding.'):
+                a = name[len('_layers_address_embedding.'):]
+                present[k] = int(self._addresses[a]['id'] in cur)
+            elif name.startswith('_layers_distribution_type_embedding.'):
+                present[k] = int(name[len('_layers_distribution_type_embedding.'):] in types)
+            elif name.startswith('_layers_proposal.'):
+                a = name[len('_layers_proposal.'):name.index('._ff._layers.')]
+                present[k] = int(self._addresses[a]['id'] in cur)
+            elif name.startswith('_layers_sample_embedding.'):
+                a = name[len('_layers_sample_embedding.'):name.index('._layers.')]
+                present[k] = int(self._addresses[a]['id'] in prev)
+        return present
+
     def _infer_step_lanes(self, address, prev_address, prev_value, prior0, prior1, h, c):
         """One proposal step for the particles whose LSTM state rows are `h`, `c` ([m, H] contiguous, updated in place):
         all m particles sit at `address` and came from `prev_address` (None: first controlled site) with values
@@ -978,3 +1000,88 @@ class InferenceNetworkLSTM(nn.Module):
              ptr(p0), s0, ptr(p1), s1, ptr(h), ptr(c), ptr(params), n, ptr(self._infer_ws), need, self._precision,
              stream())
         return params
+
+    def _fill_net_desc(self, nd):
+        nd.network_type = NET_LSTM
+        nd.lstm_dim, nd.sample_dim = self._lstm_dim, self._sample_embedding_dim
+        nd.addr_dim, nd.type_dim = self._address_embedding_dim, self._distribution_type_embedding_dim
+        nd.w_ih_off = self.parameter_index['_layers_lstm.weight_ih_l0'][0]
+        nd.w_hh_off = self.parameter_index['_layers_lstm.weight_hh_l0'][0]
+        nd.b_ih_off = self.parameter_index['_layers_lstm.bias_ih_l0'][0]
+        nd.b_hh_off = self.parameter_index['_layers_lstm.bias_hh_l0'][0]
+
+    def _fill_addr_desc(self, a, address, info):
+        pi = self.parameter_index
+        a.type_id = self._types[info['type']]
+        a.addr_emb_off = pi['_layers_address_embedding.{}'.format(address)][0]
+        a.smp_w_off = pi['_layers_sample_embedding.{}._layers.0.weight'.format(address)][0]
+        a.smp_b_off = pi['_layers_sample_embedding.{}._layers.0.bias'.format(address)][0]
+
+
+class InferenceNetworkFeedForward(InferenceNetwork):
+    """pyprob/nn/inference_network_feedforward.py: every proposal head reads the observation embedding directly.  No LSTM
+    and no address, type or sample embeddings; lstm_dim and lstm_depth are accepted and ignored, as in the reference."""
+
+    def __init__(self, model=None, observe_embeddings={}, proposal_mixture_components=10, precision=0, lstm_dim=None,
+                 lstm_depth=None):
+        super().__init__(model=model, observe_embeddings=observe_embeddings,
+                         proposal_mixture_components=proposal_mixture_components, precision=precision,
+                         network_type='InferenceNetworkFeedForward')
+
+    def _add_address(self, address, dist_name, num_categories=0):
+        """New address: its proposal layer only (_polymorph, :21-51), Linear(E -> int((E + out) / 2)) -> out."""
+        if dist_name not in _FAMILY_OF:
+            raise RuntimeError('Distribution currently unsupported: {}'.format(dist_name))
+        family = _FAMILY_OF[dist_name]
+        head = self._proposal_layers(address, family, num_categories, self._observe_embedding_dim)
+        self._addresses[address] = dict(id=len(self._addresses), family=family, num_categories=num_categories,
+                                        smp_in=1 if family != FAMILY_CATEGORICAL else num_categories, type=dist_name,
+                                        **head)
+        self._head_iterations[address] = 0
+
+    def _fill_net_desc(self, nd):
+        nd.network_type = NET_FEEDFORWARD
+
+    def _fill_addr_desc(self, a, address, info):
+        pass
+
+    def _segment_presence(self, enc, force=False):
+        """int32[S]: the observation layers always take part; a proposal layer iff its address is in the minibatch."""
+        names = self._seg['names'] if self._seg is not None else self._segment_names()
+        present = np.ones(len(names), dtype=np.int32)
+        if (not self._skip_absent_gradients and not force) or enc is None:
+            return present
+        cur = set(int(i) for i in np.unique(enc.arrays['step_addr']))
+        for k, name in enumerate(names):
+            if name.startswith('_layers_proposal.'):
+                a = name[len('_layers_proposal.'):name.index('._ff._layers.')]
+                present[k] = int(self._addresses[a]['id'] in cur)
+        return present
+
+    def _infer_step_lanes(self, address, prior0, prior1, m):
+        """Proposal parameters at `address` for m particles (_infer_step, :53-66): the head runs once on the shared
+        observation embedding; only the priors differ per particle.  [m, 3K] (means|stddevs|probs), [m, C] or [m, 1]."""
+        info = self._addresses[address]
+        width = info['head_out'] if info['family'] != FAMILY_CATEGORICAL else info['num_categories']
+        params = torch.empty(m, width, dtype=torch.float32, device='cuda')
+        need = self._infer_workspace(m)
+
+        def par(x):
+            if x is None:
+                return None, 0
+            t = ops._f32(x, 'cuda').reshape(-1)      # python scalars: cached device constants (no host->device copy)
+            return t, (0 if t.numel() == 1 else 1)
+        p0, s0 = par(prior0)
+        p1, s1 = par(prior1)
+        call('ppb_ic_infer_step', self._handle, ptr(self._arena.data), ptr(self._infer_observe_embedding), 0, -1, None,
+             info['id'], ptr(p0), s0, ptr(p1), s1, None, None, ptr(params), m, ptr(self._infer_ws), need,
+             self._precision, stream())
+        return params
+
+    def _infer_step_batched(self, address, prev_address, prev_value, prior0, prior1, n):
+        """As InferenceNetworkLSTM._infer_step_batched; the previous site plays no part.  None if the address is unknown
+        (the caller then falls back to the prior)."""
+        if address not in self._addresses:
+            warnings.warn('Address unknown by inference network: {}'.format(address))
+            return None
+        return self._infer_step_lanes(address, prior0, prior1, n)

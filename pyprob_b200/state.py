@@ -15,6 +15,7 @@ import torch
 
 from . import util
 from .distributions import Bernoulli, Categorical, Distribution, Mixture, Normal, Poisson, Uniform
+from .network import InferenceNetworkFeedForward
 from .trace import BatchedTrace, Site
 from .util import InferenceEngine, PriorInflation, TraceMode
 
@@ -214,7 +215,10 @@ def _sample_from_proposal(trace, distribution, addr, n):
     own previous site (address id + value): lanes that reached this statement from different sites are stepped in
     separate groups, like the per-trace `_current_trace_previous_variable` of the reference (state.py:212)."""
     net = _network
-    H, K = net._lstm_dim, net._proposal_mixture_components
+    K = net._proposal_mixture_components
+    if isinstance(net, InferenceNetworkFeedForward):
+        return _propose_and_weigh(trace, distribution, n, *_feedforward_params(net, distribution, addr, n, K))
+    H = net._lstm_dim
     st = trace.ic_state
     if st is None:
         st = trace.ic_state = {'h': torch.zeros(n, H, device='cuda'), 'c': torch.zeros(n, H, device='cuda'),
@@ -268,6 +272,56 @@ def _sample_from_proposal(trace, distribution, addr, n):
             if params is None:
                 params = _default_params(distribution, n, K, width)
             params.index_copy_(0, lanes, out)
+    has = None
+    if not covered:   # lanes whose previous / current address the network does not know fall back to the prior
+        has = torch.zeros(n, dtype=torch.bool, device='cuda')
+        for pid, sel in groups:
+            if known and pid != -2 and (pid < 0 or pid in by_id):
+                lanes = idx if sel is None else (torch.nonzero(sel).view(-1) if idx is None else idx[sel])
+                if lanes is None:
+                    has.fill_(True)
+                else:
+                    has[lanes] = True
+    value = _propose_and_weigh(trace, distribution, n, params, has)
+    # this site becomes the previous site of the lanes that executed it
+    new_id = net._addresses[addr]['id'] if known else -2
+    if idx is None:
+        st['prev_id'].fill_(new_id)
+        st['prev_value'] = value.to(torch.float32).clone()
+        st['uniform_prev'] = new_id
+    else:
+        st['prev_id'].index_fill_(0, idx, new_id)
+        st['prev_value'].index_copy_(0, idx, value.to(torch.float32)[idx])
+        st['uniform_prev'] = None
+    st['last_mask'], st['last_id'] = _mask, new_id
+    return value
+
+
+def _feedforward_params(net, distribution, addr, n, K):
+    """Feed-forward network (inference_network_feedforward.py:53-66): no LSTM state and no previous site, so the lanes
+    that execute this statement are proposed for in ONE call.  -> (params [n, width] or None, None)."""
+    idx = None if _mask is None else (_mask_idx if _mask_idx is not None else torch.nonzero(_mask).view(-1))
+    if addr not in net._addresses:
+        warnings.warn('Address unknown by inference network: {}'.format(addr))
+        return None, None
+    if idx is not None and idx.numel() == 0:
+        return None, None
+    p0, p1 = _prior_params(distribution)
+    out = net._infer_step_lanes(addr, _lanes(p0, idx), _lanes(p1, idx), n if idx is None else idx.numel())
+    if idx is None:
+        return out, None
+    is_cat = isinstance(distribution, Categorical)
+    width = distribution.num_categories if is_cat else 1 if isinstance(distribution, Bernoulli) else 3 * K
+    params = _default_params(distribution, n, K, width)
+    params.index_copy_(0, idx, out)
+    return params, None
+
+
+def _propose_and_weigh(trace, distribution, n, params, has):
+    """value ~ proposal(params) where `has` (None: every lane) marks the lanes the network proposed for, the prior
+    elsewhere; the weight term log p(value) - log q(value) joins the trace's accumulator."""
+    K = _network._proposal_mixture_components
+    is_cat = isinstance(distribution, Categorical)
     if params is None:   # nobody could be proposed for: prior proposal, weight term exactly zero (reference warning path)
         value = distribution.sample(n)
     else:
@@ -285,15 +339,7 @@ def _sample_from_proposal(trace, distribution, addr, n):
         else:
             raise RuntimeError('Distribution currently unsupported: {}'.format(distribution.name))
         value, q_lp = proposal.sample(n, with_log_prob=True)
-        if not covered:   # lanes whose previous / current address the network does not know fall back to the prior
-            has = torch.zeros(n, dtype=torch.bool, device='cuda')
-            for pid, sel in groups:
-                if known and pid != -2 and (pid < 0 or pid in by_id):
-                    lanes = idx if sel is None else (torch.nonzero(sel).view(-1) if idx is None else idx[sel])
-                    if lanes is None:
-                        has.fill_(True)
-                    else:
-                        has[lanes] = True
+        if has is not None:
             prior_value, prior_lp = distribution.sample(n, with_log_prob=True)
             value = torch.where(has, value, prior_value)
             q_lp = torch.where(has, q_lp, prior_lp)
@@ -302,17 +348,6 @@ def _sample_from_proposal(trace, distribution, addr, n):
             distribution.score_into(value, acc, 1.0)
             acc.sub_(q_lp.double())
         _accumulate(trace, fn)
-    # this site becomes the previous site of the lanes that executed it
-    new_id = net._addresses[addr]['id'] if known else -2
-    if idx is None:
-        st['prev_id'].fill_(new_id)
-        st['prev_value'] = value.to(torch.float32).clone()
-        st['uniform_prev'] = new_id
-    else:
-        st['prev_id'].index_fill_(0, idx, new_id)
-        st['prev_value'].index_copy_(0, idx, value.to(torch.float32)[idx])
-        st['uniform_prev'] = None
-    st['last_mask'], st['last_id'] = _mask, new_id
     return value
 
 

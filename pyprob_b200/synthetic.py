@@ -7,7 +7,8 @@ import numpy as np
 import torch
 
 from .encoding import EncodedBatch, SubBatch
-from .network import InferenceNetworkLSTM
+from .network import InferenceNetworkFeedForward, InferenceNetworkLSTM
+from .util import InferenceNetwork
 
 
 class _ExampleTrace:
@@ -22,11 +23,15 @@ class _ExampleTrace:
 
 
 def build_network(observe_embeddings, observe_in_dims, addresses, lstm_dim=512, mixture_components=10, precision=0,
-                  seed=0):
+                  seed=0, inference_network=InferenceNetwork.LSTM):
     """addresses: list of (address, distribution name, num_categories) in address-id order."""
     torch.manual_seed(seed)
-    net = InferenceNetworkLSTM(model=None, observe_embeddings=observe_embeddings, lstm_dim=lstm_dim,
-                               proposal_mixture_components=mixture_components, precision=precision)
+    if inference_network == InferenceNetwork.FEEDFORWARD:
+        net = InferenceNetworkFeedForward(model=None, observe_embeddings=observe_embeddings,
+                                          proposal_mixture_components=mixture_components, precision=precision)
+    else:
+        net = InferenceNetworkLSTM(model=None, observe_embeddings=observe_embeddings, lstm_dim=lstm_dim,
+                                   proposal_mixture_components=mixture_components, precision=precision)
     shapes = {name: (d,) if d > 1 else () for name, d in zip(observe_embeddings.keys(), observe_in_dims)}
     net._ensure_initialized(_ExampleTrace(shapes))
     for address, dist_name, C in addresses:
@@ -97,11 +102,11 @@ def random_sub_batch(rng, addresses, B, obs_dim):
 
 
 # ---- BASELINE.json workloads ---------------------------------------------------------------------------------
-def gum_network(lstm_dim=512, precision=0, seed=0):
+def gum_network(lstm_dim=512, precision=0, seed=0, inference_network=InferenceNetwork.LSTM):
     """Config 2: GaussianUnknownMean, observe embeddings 32+32 (examples/gaussian_unknown_mean.ipynb)."""
     return build_network({'obs0': {'dim': 32}, 'obs1': {'dim': 32}}, [1, 1],
                          [('98__forward__mu__Normal__1', 'Normal', 0)], lstm_dim=lstm_dim, precision=precision,
-                         seed=seed)
+                         seed=seed, inference_network=inference_network)
 
 
 def gum_batch(rng, B):
@@ -117,10 +122,10 @@ def synthetic50_addresses(T=50, C=4):
              'Normal' if t % 2 == 0 else 'Categorical', 0 if t % 2 == 0 else C) for t in range(T)]
 
 
-def synthetic50_network(lstm_dim=512, obs_dim=256, precision=0, seed=0, T=50):
+def synthetic50_network(lstm_dim=512, obs_dim=256, precision=0, seed=0, T=50, inference_network=InferenceNetwork.LSTM):
     """Config 4: 50 addresses alternating Normal(0,1) / Categorical(4), one observable, FF dim 256 depth 2."""
     return build_network({'obs': {'dim': obs_dim}}, [1], synthetic50_addresses(T), lstm_dim=lstm_dim,
-                         precision=precision, seed=seed)
+                         precision=precision, seed=seed, inference_network=inference_network)
 
 
 def synthetic50_batch(rng, B, T=50):
