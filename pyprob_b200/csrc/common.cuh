@@ -52,12 +52,13 @@ extern unsigned long long g_ppb_launches;  // kernels launched by this library (
 __device__ __forceinline__ void ppb_pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void ppb_pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
-bool ppb_pdl_enabled();   // default on; PPB_PDL=0 disables (lib.cu)
-int ppb_pdl_level();      // `pdl` argument of ppb_launch: the attribute is set when pdl != 0 and pdl <= ppb_pdl_level()
+bool ppb_pdl_enabled();          // default on; PPB_PDL=0 disables (lib.cu)
+bool ppb_persistent_enabled();   // default on; PPB_PERSISTENT=0 disables the persistent grouped GEMM (lib.cu)
 
-// <<<grid, block, smem, st>>> with optional PDL attribute and optional (cluster, 1, 1) thread-block cluster
+// <<<grid, block, smem, st>>> with optional PDL attribute (pdl, unless PPB_PDL=0) and optional (cluster, 1, 1)
+// thread-block cluster
 template <typename... KArgs, typename... Args>
-inline cudaError_t ppb_launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, int pdl,
+inline cudaError_t ppb_launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl,
                               int cluster, Args... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
@@ -73,7 +74,7 @@ inline cudaError_t ppb_launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
     attr[n].val.clusterDim.z = 1;
     ++n;
   }
-  if (pdl && pdl <= ppb_pdl_level()) {
+  if (pdl && ppb_pdl_enabled()) {
     attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[n].val.programmaticStreamSerializationAllowed = 1;
     ++n;

@@ -15,14 +15,18 @@ void ppb_set_error(const char* fmt, ...) {
   va_end(ap);
 }
 
-// read at every launch (a getenv per eager launch; graph replays do not come here) so that tests can flip it in-process.
-// PPB_PDL = 0: off; 1 (default): tensor-core kernels and the element-wise kernels between them (cell, pack, NLL); 2: also the
-// observe-MLP backward kernels; 3: also Adam (early-resident blocks of levels 2 and 3 take SMs from the side-stream branches)
-int ppb_pdl_level() {
+// Both switches are read at every call (a getenv per eager launch; graph replays do not come here) so that tests can flip
+// them in-process.
+// PPB_PDL=0 turns programmatic dependent launch off (plain stream order, the reference the PDL chains are tested against)
+bool ppb_pdl_enabled() {
   const char* e = getenv("PPB_PDL");
-  return (e && e[0] >= '0' && e[0] <= '9') ? e[0] - '0' : 1;
+  return !(e && e[0] == '0');
 }
-bool ppb_pdl_enabled() { return ppb_pdl_level() > 0; }
+// PPB_PERSISTENT=0 launches the grouped tensor-core GEMM with one CTA per tile even when a phase has more tiles than SMs
+bool ppb_persistent_enabled() {
+  const char* e = getenv("PPB_PERSISTENT");
+  return !(e && e[0] == '0');
+}
 
 extern "C" {
 

@@ -85,7 +85,6 @@ struct ppb_net {
   cudaEvent_t fork_ev[16] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
                              nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   int fork_next = 0;
-  int single_stream = 0;            // PPB_SINGLE_STREAM=1: everything on the caller's stream (A/B, debugging)
   int pack_tiles_no_hh = 0;         // weight-image tiles without W_hh (a T = 1 step never reads it)
   // ppb_ic_train_step_host: the whole step cached as an instantiated CUDA graph per batch structure
   int host_graph = 1;               // PPB_HOST_STEP_GRAPH=0 disables
@@ -302,14 +301,6 @@ int stream_after(ppb_net* net, cudaStream_t from, cudaStream_t to) {
   PPB_CUDA(cudaStreamWaitEvent(to, ev, 0));
   return PPB_OK;
 }
-// side stream k (or the main stream itself in single-stream mode)
-int side_stream(ppb_net* net, int k, cudaStream_t main_st, cudaStream_t* out) {
-  if (net->single_stream) { *out = main_st; return PPB_OK; }
-  if (!net->side[k]) PPB_CUDA(cudaStreamCreateWithFlags(&net->side[k], cudaStreamNonBlocking));
-  *out = net->side[k];
-  return PPB_OK;
-}
-
 // ---- optional kernel-level profiling of the LSTM gate GEMM class (bench.py roofline) ---------------
 struct Prof {
   bool on = false;
@@ -318,28 +309,40 @@ struct Prof {
   int64_t launches = 0;
 } g_prof;
 
+// One profiled launch: prof_begin records the start event when profiling is on and the caller asks for it (`want`), else
+// leaves e0 null; prof_end records the end event after a non-null e0 and counts one launch of `flops` FLOPs.
+int prof_begin(bool want, cudaStream_t st, cudaEvent_t& e0) {
+  e0 = nullptr;
+  if (!want || !g_prof.on) return PPB_OK;
+  PPB_CUDA(cudaEventCreate(&e0));
+  PPB_CUDA(cudaEventRecord(e0, st));
+  return PPB_OK;
+}
+int prof_end(cudaEvent_t e0, cudaStream_t st, double flops) {
+  if (!e0) return PPB_OK;
+  cudaEvent_t e1;
+  PPB_CUDA(cudaEventCreate(&e1));
+  PPB_CUDA(cudaEventRecord(e1, st));
+  g_prof.spans.push_back({e0, e1});
+  g_prof.launches += 1;
+  g_prof.flops += flops;
+  return PPB_OK;
+}
+template <typename P>
+double phase_flops(const std::vector<P>& probs, const gemm::Phase& ph) {
+  double f = 0.0;
+  for (int i = 0; i < ph.count; ++i) { const P& p = probs[ph.first + i]; f += 2.0 * p.M * p.N * p.K; }
+  return f;
+}
+
 int run_phase(const gemm::Phase& ph, const Problem* dev, cudaStream_t st, const Builder* bl_for_prof = nullptr) {
   if (ph.count == 0) return PPB_OK;
   int grid = ph.tiles < 8 * PPB_NUM_SMS ? ph.tiles : 8 * PPB_NUM_SMS;
-  cudaEvent_t e0 = nullptr, e1 = nullptr;
-  const bool prof = g_prof.on && bl_for_prof;
-  if (prof) {
-    PPB_CUDA(cudaEventCreate(&e0));
-    PPB_CUDA(cudaEventCreate(&e1));
-    PPB_CUDA(cudaEventRecord(e0, st));
-  }
+  cudaEvent_t e0;
+  int rc = prof_begin(bl_for_prof != nullptr, st, e0); if (rc) return rc;
   gemm::k_grouped<<<grid, gemm::kThreads, 0, st>>>(dev + ph.first, ph.count, ph.tiles);
   PPB_LAUNCH_CHECK();
-  if (prof) {
-    PPB_CUDA(cudaEventRecord(e1, st));
-    g_prof.spans.push_back({e0, e1});
-    g_prof.launches += 1;
-    for (int i = 0; i < ph.count; ++i) {
-      const Problem& p = bl_for_prof->probs[ph.first + i];
-      g_prof.flops += 2.0 * p.M * p.N * p.K;
-    }
-  }
-  return PPB_OK;
+  return e0 ? prof_end(e0, st, phase_flops(bl_for_prof->probs, ph)) : PPB_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -455,8 +458,8 @@ __global__ void __launch_bounds__(256) k_cell_fwd(float* __restrict__ gates, con
 // heads: family transform + log q(value) + d(-log q)/d out, loss reduction (:199-218).
 // One WARP per row: lane k owns mixture component k (or categories k, k+32, ...), reductions are shuffles;
 // the formulas are those of heads.cuh (mixture_nll / categorical_nll), restated lane-parallel.
-// nll_row is the per-row routine (x = the row's raw head outputs, global or shared memory); two kernels call it:
-// k_head_nll (x read from the output of the h2 GEMM) and k_head_out_nll (x computed in the kernel, below).
+// nll_row is the per-row routine (x = the row's raw head outputs, global or shared memory); two callers:
+// k_head_nll (x read from the output of the h2 GEMM) and NllRowEpi (x parked in shared memory by the h2 cluster GEMM, below).
 struct NllArgs {
   const ppb_addr_desc* addrs;
   const int* row_step; const int* step_addr;
@@ -697,93 +700,6 @@ __global__ void __launch_bounds__(256) k_head_nll(const float* __restrict__ out_
   int bad = 0;
   for (int row = warp; row < R; row += nwarps) nll_row(A, out_raw + (int64_t)row * A.out_pad, row, lane, local, bad);
   nll_finish(local, bad, lane, A.inv_batch, gridDim.x, loss_acc, loss_out, status_out);
-}
-
-// The output layer of the proposal heads and the NLL in ONE kernel, on the CUDA cores.  The layer is tiny (hidden <= ~300,
-// out = 3K or C <= 128: 8 k MACs per row at configs[1]) but as a tensor-core launch it is a padded 128-wide tile in 3xTF32 plus
-// a kernel boundary: 9.3 us + 7.4 us + a 2 us gap on the configs[1] chain, 62 us at T = 50.  Here blockIdx.y = segment
-// (rows that share an address, hence W2), a block stages that address's W2 and b2 in shared memory once — BEFORE the PDL
-// wait: the weights are not written inside a training step — and each warp walks its rows: hidden activations = hi + lo of the
-// K-format tile image the h1 GEMM wrote (the same two words the tensor-core path multiplies), 4-way split dot products,
-// then nll_row on the outputs in shared memory.
-// Four blocks per SM: without the bound, the Bernoulli branch of nll_row lets ptxas take 103 registers (two blocks per SM);
-// with it the kernel keeps the 64 registers and no spills it had with four families.
-__global__ void __launch_bounds__(256, 4) k_head_out_nll(const float* __restrict__ arena, const float* __restrict__ hid_hi,
-                                                       const float* __restrict__ hid_lo, int64_t hid_kb,
-                                                       const int* __restrict__ step_row0, const int* __restrict__ step_nrows,
-                                                       int rows_per_block, NllArgs A, float* __restrict__ out_raw,
-                                                       float* __restrict__ loss_acc, float* __restrict__ loss_out,
-                                                       int* __restrict__ status_out) {
-  ppb_pdl_trigger();
-  extern __shared__ float sm_head[];
-  const int seg = blockIdx.y, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const ppb_addr_desc a = A.addrs[A.step_addr[seg]];
-  // rows of W2 at a pitch of 4 x (odd) floats: 16-byte shared-memory loads whose quarter-warps hit eight different bank groups
-  const int Hh = a.head_hidden, O = a.head_out, Hh4 = (Hh + 3) & ~3;
-  const int pitch = ((Hh4 >> 2) & 1) ? Hh4 : Hh4 + 4;
-  float* w2s = sm_head;                       // [O][pitch], columns >= Hh zero
-  float* b2s = w2s + (size_t)O * pitch;       // [O]
-  float* hrow = b2s + ((O + 3) & ~3) + (size_t)warp * (Hh4 + 128);   // per warp: hidden row (zero-padded to Hh4), 128 outputs
-  float* xout = hrow + Hh4;
-  const int r0 = step_row0[seg] + blockIdx.x * rows_per_block;
-  int r1 = r0 + rows_per_block;
-  // the padding rows of the segment (up to the next multiple of 128) are walked too: nll_row zero-fills their gradient rows
-  // and images, which the weight-gradient reductions read
-  const int seg_end = step_row0[seg] + step_nrows[seg];
-  const int seg_end_pad = step_row0[seg] + ((step_nrows[seg] + 127) & ~127);
-  if (r1 > seg_end_pad) r1 = seg_end_pad;
-  const bool any = r0 < r1 && r0 < seg_end;
-  if (any) {
-    const float* w2 = arena + a.w2_off;
-    for (int i = threadIdx.x; i < O * pitch; i += blockDim.x) {
-      const int o = i / pitch, k = i - o * pitch;
-      w2s[i] = (k < Hh) ? __ldg(w2 + (int64_t)o * Hh + k) : 0.0f;
-    }
-    for (int o = threadIdx.x; o < O; o += blockDim.x) b2s[o] = __ldg(arena + a.b2_off + o);
-  }
-  ppb_pdl_wait();
-  __syncthreads();
-  float local = 0.0f;
-  int bad = 0;
-  for (int row = r0 + warp; row < r1; row += 8) {
-    if (row >= seg_end) {   // warp-uniform: padding row
-      nll_row(A, xout, row, lane, local, bad);
-      continue;
-    }
-    // hidden activations of the row: hi + lo of the K-format image (32 consecutive k = one swizzled 128-byte span)
-    for (int k = lane; k < Hh4; k += 32) {
-      float v = 0.0f;
-      if (k < Hh) {
-        const int64_t off = tc::packed_offset(row, k, hid_kb);
-        v = __ldg(hid_hi + off) + (hid_lo ? __ldg(hid_lo + off) : 0.0f);
-      }
-      hrow[k] = v;
-    }
-    __syncwarp();
-    for (int o0 = 0; o0 < O; o0 += 32) {
-      const int o = o0 + lane;
-      const float4* wr = reinterpret_cast<const float4*>(w2s + (size_t)(o < O ? o : 0) * pitch);
-      const float4* hr = reinterpret_cast<const float4*>(hrow);
-      float acc[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll 4
-      for (int k4 = 0; k4 < (Hh4 >> 2); ++k4) {
-        const float4 h4 = hr[k4], w4 = wr[k4];
-        acc[0] = fmaf(h4.x, w4.x, acc[0]);
-        acc[1] = fmaf(h4.y, w4.y, acc[1]);
-        acc[2] = fmaf(h4.z, w4.z, acc[2]);
-        acc[3] = fmaf(h4.w, w4.w, acc[3]);
-      }
-      if (o < O) {
-        const float y = ((acc[0] + acc[1]) + (acc[2] + acc[3])) + b2s[o];
-        xout[o] = y;
-        if (out_raw) out_raw[(int64_t)row * A.out_pad + o] = y;
-      }
-    }
-    __syncwarp();
-    nll_row(A, xout, row, lane, local, bad);
-    __syncwarp();
-  }
-  nll_finish(local, bad, lane, A.inv_batch, gridDim.x * gridDim.y, loss_acc, loss_out, status_out);
 }
 
 // LSTM cell backward of one (row, unit) (torch.nn.LSTM gate order i, f, g, o): dht = dL/dh_t, dc_next = dL/dc_t carried back
@@ -1352,12 +1268,9 @@ int ppb_net_create(ppb_net** out, const ppb_net_desc* d) {
   n->fused_cell = !(fc && fc[0] == '0');
   const char* hg = getenv("PPB_HOST_STEP_GRAPH");
   n->host_graph = (hg && hg[0] == '0') ? 0 : 1;   // on by default (PPB_HOST_STEP_GRAPH=0: always launch eagerly)
-  const char* ss = getenv("PPB_SINGLE_STREAM");
-  n->single_stream = (ss && ss[0] == '1') ? 1 : 0;
   // created up front: a training step must be capturable in a CUDA graph right after its first eager run
   for (int i = 0; i < 16; ++i) PPB_CUDA(cudaEventCreateWithFlags(&n->fork_ev[i], cudaEventDisableTiming));
-  if (!n->single_stream)
-    for (int i = 0; i < 2; ++i) PPB_CUDA(cudaStreamCreateWithFlags(&n->side[i], cudaStreamNonBlocking));
+  for (int i = 0; i < 2; ++i) PPB_CUDA(cudaStreamCreateWithFlags(&n->side[i], cudaStreamNonBlocking));
   *out = n;
   return PPB_OK;
 }
@@ -1921,7 +1834,7 @@ int ppb_adam_step(float* arena, const float* grad, float* exp_avg, float* exp_av
                   float beta2, float eps, float weight_decay, int64_t step, float grad_scale, void* stream) {
   PPB_CHECK_ARG(arena && grad && exp_avg && exp_avg_sq && n > 0 && step >= 1, "bad arguments");
   double bc1 = 1.0 - pow((double)beta1, (double)step), bc2 = 1.0 - pow((double)beta2, (double)step);
-  PPB_CUDA(ppb_launch(k_adam, dim3(ppb_grid_for(n, 256, 4)), dim3(256), 0, (cudaStream_t)stream, 3, 0, arena, grad, exp_avg,
+  PPB_CUDA(ppb_launch(k_adam, dim3(ppb_grid_for(n, 256, 4)), dim3(256), 0, (cudaStream_t)stream, 0, 0, arena, grad, exp_avg,
                       exp_avg_sq, n, lr, beta1, beta2, eps, weight_decay, (float)bc1, (float)sqrt(bc2), grad_scale));
   PPB_LAUNCH_CHECK();
   return PPB_OK;
@@ -1935,7 +1848,7 @@ int ppb_adam_step_dev(float* arena, const float* grad, float* exp_avg, float* ex
                       const float* hyper_dev, void* state_dev, void* stream) {
   PPB_CHECK_ARG(arena && grad && exp_avg && exp_avg_sq && hyper_dev && state_dev && n > 0, "bad arguments");
   const int vec = ((((uintptr_t)arena | (uintptr_t)grad | (uintptr_t)exp_avg | (uintptr_t)exp_avg_sq) & 15) == 0) ? 1 : 0;
-  PPB_CUDA(ppb_launch(k_adam_dev, dim3(ppb_grid_for(n, 256, 4)), dim3(256), 0, (cudaStream_t)stream, 3, 0, arena, grad,
+  PPB_CUDA(ppb_launch(k_adam_dev, dim3(ppb_grid_for(n, 256, 4)), dim3(256), 0, (cudaStream_t)stream, 0, 0, arena, grad,
                       exp_avg, exp_avg_sq, n, vec, hyper_dev, (long long*)state_dev, (float*)((char*)state_dev + 8),
                       (unsigned int*)((char*)state_dev + 12)));
   PPB_LAUNCH_CHECK();

@@ -2,8 +2,6 @@
 // Replaces pyprob/distributions/distribution.py:38-43 as driven per particle by pyprob/state.py.
 // Algorithmic bytes per element (SURVEY §8d): Normal/Uniform 16 B, Poisson/Bernoulli 12 B, Categorical 4C+12 B,
 // Mixture-Normal (3K+2)*4 B, Mixture-TruncatedNormal (3K+4)*4 B.
-#include <stdlib.h>
-
 #include "common.cuh"
 
 namespace {
@@ -18,12 +16,6 @@ __device__ __forceinline__ float4 ldg_stream4(const float* p) {
   asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0,%1,%2,%3}, [%4];"
                : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w)
                : "l"(p));
-  return r;
-}
-
-__device__ __forceinline__ float ldg_stream(const float* p) {
-  float r;
-  asm("ld.global.nc.L1::no_allocate.f32 %0, [%1];" : "=f"(r) : "l"(p));
   return r;
 }
 
@@ -258,87 +250,12 @@ __global__ void __launch_bounds__(kThreads) k_mixture(const float* __restrict__ 
   }
 }
 
-// Same arithmetic, parameters staged through shared memory.  A thread of k_mixture reads its own [K] rows with 3K strided
-// 4-byte loads: one warp-level load touches K different 128-byte lines, i.e. 3K * K load wavefronts per 32 particles (300 at
-// K = 10) — the load/store unit, not HBM, bounds that kernel.  Here a WARP owns 32 consecutive particles: it copies their
-// contiguous 32 x K parameter block with fully coalesced 4-byte loads (one wavefront each) into shared memory at an odd row
-// pitch, then every lane reads its own row conflict-free.  Only __syncwarp, no CTA barrier.  Requires densely packed rows
-// (row_stride == K).  Opt-in (PPB_MIXTURE_STAGED=1): results must equal k_mixture's to rounding
-// (tests/test_scoring_staged_gpu.py).
-template <int KMAX, bool TRUNC>
-__global__ void __launch_bounds__(kThreads) k_mixture_staged(const float* __restrict__ value,
-                                                              const float* __restrict__ means,
-                                                              const float* __restrict__ stddevs,
-                                                              const float* __restrict__ probs, int K, Param low,
-                                                              Param high, Sink out, int64_t n) {
-  extern __shared__ __align__(16) float sm[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int pitch = K | 1;
-  float* wm = sm + (size_t)warp * 3 * 32 * pitch;
-  float* ws = wm + 32 * pitch;
-  float* wp = ws + 32 * pitch;
-  const int dr = 32 / K, dk = 32 % K;       // (row, component) of flat element idx + 32
-  const int64_t stride = (int64_t)gridDim.x * (kThreads / 32) * 32;
-  for (int64_t w0 = ((int64_t)blockIdx.x * (kThreads / 32) + warp) * 32; w0 < n; w0 += stride) {
-    const int rows = (int)((n - w0 < 32) ? (n - w0) : 32);
-    const int cnt = rows * K;
-    const float* gm = means + w0 * K;
-    const float* gs = stddevs + w0 * K;
-    const float* gp = probs + w0 * K;
-    // one array at a time: its K loads are issued together (independent requests in flight), then scattered into shared memory
-    const int r0 = lane / K, k0 = lane % K;
-    auto stage = [&](const float* __restrict__ g, float* __restrict__ w) {
-      float v[KMAX];
-#pragma unroll
-      for (int j = 0; j < KMAX; ++j) {
-        const int idx = lane + 32 * j;
-        v[j] = (j < K && idx < cnt) ? ldg_stream(g + idx) : 0.0f;
-      }
-      int r = r0, k = k0;
-#pragma unroll
-      for (int j = 0; j < KMAX; ++j) {
-        if (j < K && lane + 32 * j < cnt) w[r * pitch + k] = v[j];
-        r += dr; k += dk;
-        if (k >= K) { k -= K; ++r; }
-      }
-    };
-    stage(gm, wm);
-    stage(gs, ws);
-    stage(gp, wp);
-    __syncwarp();
-    if (lane < rows) {
-      const int64_t i = w0 + lane;
-      float lo = 0.f, hi = 0.f;
-      if (TRUNC) { lo = low.at(i); hi = high.at(i); }
-      out.put(i, mixture_row<KMAX, TRUNC>(__ldg(value + i), wm + lane * pitch, ws + lane * pitch, wp + lane * pitch, K, lo, hi));
-    }
-    __syncwarp();
-  }
-}
-
-inline bool mixture_staged_enabled() {
-  static const bool on = [] {
-    const char* e = getenv("PPB_MIXTURE_STAGED");
-    return e && e[0] == '1';
-  }();
-  return on;
-}
-
 template <bool TRUNC>
 int launch_mixture(const float* value, const float* means, const float* stddevs, const float* probs,
                    int64_t row_stride, int K, Param low, Param high, Sink out, int64_t n, void* stream) {
   if (n == 0) return PPB_OK;
   cudaStream_t st = (cudaStream_t)stream;
   int grid = ppb_grid_for(n, kThreads, 1);
-  if (mixture_staged_enabled() && row_stride == K && K <= 10) {
-    size_t smem = (size_t)3 * kThreads * (K | 1) * sizeof(float);
-    if (K <= 4)
-      k_mixture_staged<4, TRUNC><<<grid, kThreads, smem, st>>>(value, means, stddevs, probs, K, low, high, out, n);
-    else
-      k_mixture_staged<10, TRUNC><<<grid, kThreads, smem, st>>>(value, means, stddevs, probs, K, low, high, out, n);
-    PPB_LAUNCH_CHECK();
-    return PPB_OK;
-  }
   if (K <= 4)
     k_mixture<4, TRUNC><<<grid, kThreads, 0, st>>>(value, means, stddevs, probs, row_stride, K, low, high, out, n);
   else if (K == 10)   // the proposal heads' component count (pyprob/nn/proposal_normal_mixture.py: mixture_components = 10)

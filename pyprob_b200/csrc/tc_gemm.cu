@@ -3,7 +3,6 @@
 // (tc_grouped.cuh):  C[M,N] = A[M,K] * B[N,K]^T (+bias) (relu)  and  C[M,N] = X[R,M]^T Y[R,N].
 #include <string.h>
 
-#include <stdlib.h>
 #include "common.cuh"
 #include "tc.cuh"
 #include "tc_grouped.cuh"
@@ -58,8 +57,7 @@ int launch_single(const tcg::Problem& hp, cudaStream_t st) {
   if (!g_dev_problem) PPB_CUDA(cudaMalloc((void**)&g_dev_problem, sizeof(tcg::Problem)));
   PPB_CUDA(cudaMemcpyAsync(g_dev_problem, &hp, sizeof(hp), cudaMemcpyHostToDevice, st));
   const int tiles = hp.tiles_m * hp.tiles_n * (hp.k_splits > 1 ? hp.k_splits : 1);
-  const char* pe = getenv("PPB_PERSISTENT");
-  if (!(pe && pe[0] == '0') && tiles > PPB_NUM_SMS) {   // persistent form (tc_persist.cuh); PPB_PERSISTENT=0: one CTA per tile
+  if (ppb_persistent_enabled() && tiles > PPB_NUM_SMS) {   // persistent form (tc_persist.cuh)
     static bool attr_p = false;
     if (!attr_p) {
       PPB_CUDA(cudaFuncSetAttribute(tcp::k_grouped_persistent<X3, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize,

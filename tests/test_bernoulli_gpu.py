@@ -155,12 +155,8 @@ def _oracle(net, subs):
     (3, 32, [([0, 1, 3, 2, 0], 129)]),                              # longer trace, Bernoulli as previous site
     (4, 64, [([0, 2, 3, 1], 40), ([3], 7), ([4, 0, 5, 3, 0, 1], 65)]),   # ragged, three sub-batches, all families
 ])
-@pytest.mark.parametrize('precision,fuse', [(0, False), (0, True), (2, False)])
-def test_loss_and_grads_vs_oracle_random(cuda, monkeypatch, seed, lstm_dim, spec, precision, fuse):
-    if fuse:
-        monkeypatch.setenv('PPB_FUSE_HEAD_OUT', '1')
-    else:
-        monkeypatch.delenv('PPB_FUSE_HEAD_OUT', raising=False)
+@pytest.mark.parametrize('precision', [0, 2])
+def test_loss_and_grads_vs_oracle_random(cuda, seed, lstm_dim, spec, precision):
     net, subs = _random_case(seed, lstm_dim, spec, precision)
     want_loss, want_grads, _ = _oracle(net, subs)
     ok, loss = net._loss(synthetic.ArrayBatch(subs))
