@@ -71,6 +71,40 @@ int ppb_poisson_log_prob(const float* value, const float* rate, int rate_stride,
  * a value outside {0, 1} scores NaN (the reference's argument validation raises). */
 int ppb_bernoulli_log_prob(const float* value, const float* probs, int probs_stride, float* lp_out,
                            double* acc, double acc_scale, int64_t n, void* stream);
+/* The remaining scalar families follow torch.distributions' log_prob, which the reference wraps.  A value outside the
+ * support or an invalid parameter scores NaN (the reference's argument validation raises).
+ * pyprob/distributions/exponential.py: log r - r x, x >= 0. */
+int ppb_exponential_log_prob(const float* value, const float* rate, int rate_stride, float* lp_out,
+                             double* acc, double acc_scale, int64_t n, void* stream);
+/* pyprob/distributions/gamma.py: xlogy(c, r) + xlogy(c - 1, x) - r x - lgamma(c), x >= 0. */
+int ppb_gamma_log_prob(const float* value, const float* concentration, int concentration_stride,
+                       const float* rate, int rate_stride, float* lp_out, double* acc, double acc_scale,
+                       int64_t n, void* stream);
+/* pyprob/distributions/log_normal.py: Normal(loc, scale).log_prob(log x) - log x, x > 0. */
+int ppb_lognormal_log_prob(const float* value, const float* loc, int loc_stride, const float* scale,
+                           int scale_stride, float* lp_out, double* acc, double acc_scale, int64_t n,
+                           void* stream);
+/* pyprob/distributions/weibull.py: torch's Exponential(1) through PowerTransform(1/k) and AffineTransform(0, scale),
+ * x > 0. */
+int ppb_weibull_log_prob(const float* value, const float* scale, int scale_stride, const float* concentration,
+                         int concentration_stride, float* lp_out, double* acc, double acc_scale, int64_t n,
+                         void* stream);
+/* pyprob/distributions/beta.py:38-40: torch Beta(c1, c0).log_prob((x - low) / (high - low)), with no -log(high - low)
+ * term, as the reference; (x - low) / (high - low) in [0, 1]. */
+int ppb_beta_log_prob(const float* value, const float* concentration1, int concentration1_stride,
+                      const float* concentration0, int concentration0_stride, const float* low, int low_stride,
+                      const float* high, int high_stride, float* lp_out, double* acc, double acc_scale,
+                      int64_t n, void* stream);
+/* pyprob/distributions/binomial.py (torch Binomial(total_count, probs=)): torch's logits form with
+ * logits = log(pc) - log1p(-pc), pc = clamp_probs(p); x an integer in [0, total_count]. */
+int ppb_binomial_log_prob(const float* value, const float* total_count, int total_count_stride,
+                          const float* probs, int probs_stride, float* lp_out, double* acc, double acc_scale,
+                          int64_t n, void* stream);
+/* pyprob/distributions/von_mises.py: kappa cos(x - loc) - log(2 pi) - log I0(kappa), log I0 as torch's
+ * _log_modified_bessel_fn computes it (finite at any kappa). */
+int ppb_von_mises_log_prob(const float* value, const float* loc, int loc_stride, const float* concentration,
+                           int concentration_stride, float* lp_out, double* acc, double acc_scale, int64_t n,
+                           void* stream);
 /* probs: [n, C] (probs_row_stride = C) or [C] shared (probs_row_stride = 0); unnormalised, as given to
  * pyprob/distributions/categorical.py:8-21.  value holds category indices stored as fp32. */
 int ppb_categorical_log_prob(const float* value, const float* probs, int64_t probs_row_stride,
@@ -110,6 +144,38 @@ int ppb_poisson_sample(const float* rate, int rate_stride, float* value_out, flo
 /* value = 1 if u < p else 0, u uniform in [0, 1) from Philox word 0 */
 int ppb_bernoulli_sample(const float* probs, int probs_stride, float* value_out, float* lp_out, int64_t n,
                          uint64_t seed, uint64_t offset, int64_t first_index, void* stream);
+/* The samplers of the families in section 1 (pyprob/distributions/{exponential,gamma,log_normal,weibull,beta,binomial,
+ * von_mises}.py).  Invalid parameters draw NaN.  The rejection samplers draw each round from the counter
+ * (i, offset + (round << 40)) and stop after a fixed number of rounds (failure probability below 1e-12 per draw),
+ * so every draw takes bounded time.
+ *   exponential: -log(u) / rate (inversion)
+ *   gamma:       Marsaglia-Tsang for c >= 1; G(c + 1) u^(1/c) for c < 1; clamped below at FLT_MIN, as torch
+ *   lognormal:   exp of the Box-Muller normal
+ *   weibull:     scale (-log u)^(1/k)
+ *   beta:        low + (high - low) Ga / (Ga + Gb), the ratio clamped to [FLT_MIN, 1 - eps] as torch's Dirichlet
+ *   binomial:    inversion for n min(p, 1 - p) < 10, BTRS (Hoermann 1993) otherwise; total_count per particle or shared
+ *   von_mises:   Best-Fisher rejection in double precision, wrapped into [-pi, pi) as torch */
+int ppb_exponential_sample(const float* rate, int rate_stride, float* value_out, float* lp_out, int64_t n,
+                           uint64_t seed, uint64_t offset, int64_t first_index, void* stream);
+int ppb_gamma_sample(const float* concentration, int concentration_stride, const float* rate, int rate_stride,
+                     float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset,
+                     int64_t first_index, void* stream);
+int ppb_lognormal_sample(const float* loc, int loc_stride, const float* scale, int scale_stride,
+                         float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset,
+                         int64_t first_index, void* stream);
+int ppb_weibull_sample(const float* scale, int scale_stride, const float* concentration, int concentration_stride,
+                       float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset,
+                       int64_t first_index, void* stream);
+int ppb_beta_sample(const float* concentration1, int concentration1_stride, const float* concentration0,
+                    int concentration0_stride, const float* low, int low_stride, const float* high,
+                    int high_stride, float* value_out, float* lp_out, int64_t n, uint64_t seed,
+                    uint64_t offset, int64_t first_index, void* stream);
+int ppb_binomial_sample(const float* total_count, int total_count_stride, const float* probs, int probs_stride,
+                        float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset,
+                        int64_t first_index, void* stream);
+int ppb_von_mises_sample(const float* loc, int loc_stride, const float* concentration, int concentration_stride,
+                         float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset,
+                         int64_t first_index, void* stream);
 int ppb_categorical_sample(const float* probs, int64_t probs_row_stride, int num_categories,
                            float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset,
                            int64_t first_index, void* stream);

@@ -32,6 +32,13 @@ _SIGNATURES = {
     'ppb_uniform_log_prob': [c_f, c_f, c_int, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
     'ppb_poisson_log_prob': [c_f, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
     'ppb_bernoulli_log_prob': [c_f, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
+    'ppb_exponential_log_prob': [c_f, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
+    'ppb_gamma_log_prob': [c_f, c_f, c_int, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
+    'ppb_lognormal_log_prob': [c_f, c_f, c_int, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
+    'ppb_weibull_log_prob': [c_f, c_f, c_int, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
+    'ppb_beta_log_prob': [c_f, c_f, c_int, c_f, c_int, c_f, c_int, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
+    'ppb_binomial_log_prob': [c_f, c_f, c_int, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
+    'ppb_von_mises_log_prob': [c_f, c_f, c_int, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
     'ppb_categorical_log_prob': [c_f, c_f, c_i64, c_int, c_f, c_f, c_dbl, c_i64, c_f],
     'ppb_mixture_normal_log_prob': [c_f, c_f, c_f, c_f, c_i64, c_int, c_f, c_f, c_dbl, c_i64, c_f],
     'ppb_mixture_truncated_normal_log_prob': [c_f, c_f, c_f, c_f, c_i64, c_int, c_f, c_int, c_f, c_int, c_f, c_f,
@@ -40,6 +47,13 @@ _SIGNATURES = {
     'ppb_uniform_sample': [c_f, c_int, c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
     'ppb_poisson_sample': [c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
     'ppb_bernoulli_sample': [c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
+    'ppb_exponential_sample': [c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
+    'ppb_gamma_sample': [c_f, c_int, c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
+    'ppb_lognormal_sample': [c_f, c_int, c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
+    'ppb_weibull_sample': [c_f, c_int, c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
+    'ppb_beta_sample': [c_f, c_int, c_f, c_int, c_f, c_int, c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
+    'ppb_binomial_sample': [c_f, c_int, c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
+    'ppb_von_mises_sample': [c_f, c_int, c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
     'ppb_categorical_sample': [c_f, c_i64, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
     'ppb_mixture_normal_sample': [c_f, c_f, c_f, c_i64, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
     'ppb_mixture_truncated_normal_sample': [c_f, c_f, c_f, c_i64, c_int, c_f, c_int, c_f, c_int, c_f, c_f, c_i64,

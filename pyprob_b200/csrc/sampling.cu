@@ -2,6 +2,7 @@
 // Replaces pyprob/distributions/distribution.py:31-36, mixture.py:47-63, truncated_normal.py:94-112.
 // Fused sample+score: lp_out (nullable) gets log_prob of the drawn value (pyprob/state.py:196-197).
 #include "common.cuh"
+#include "families.cuh"
 
 namespace {
 
@@ -102,6 +103,222 @@ __global__ void __launch_bounds__(kThreads) k_bernoulli(P probs, float* __restri
       const float pc = ppb_clamp_prob(p);
       lp[i] = one ? logf(pc) : log1pf(-pc);
     }
+  }
+}
+
+// ---- Exponential .. VonMises: lp_out through the log_prob functions of families.cuh ------------------------------------
+// uniform in (0, 1), open at both ends: the inversions below take logs of u and of 1 - u
+__device__ __forceinline__ float u01_open(uint32_t x) { return ((float)(x >> 8) + 0.5f) * (1.0f / 16777216.0f); }
+// uniform in [0, 1) with 53 random bits from two words
+__device__ __forceinline__ double u01_double(uint32_t a, uint32_t b) {
+  return (double)((((uint64_t)a << 32) | b) >> 11) * (1.0 / 9007199254740992.0);
+}
+__device__ __forceinline__ ppb_philox philox_sub(uint64_t seed, uint64_t idx, uint64_t offset, uint64_t sub) {
+  return ppb_philox4x32_10(seed, idx, offset + (sub << 40));   // fresh words for rejection rounds, as poisson_draw
+}
+
+#define PPB_GRID_LOOP(i) \
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+
+// Exponential: inversion, -log(u) / rate
+__global__ void __launch_bounds__(kThreads) k_exponential(P rate, float* __restrict__ out, float* __restrict__ lp,
+                                                           int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
+  PPB_GRID_LOOP(i) {
+    ppb_philox r = ppb_philox4x32_10(seed, (uint64_t)(first + i), offset);
+    const float lam = rate.at(i);
+    const float v = (lam > 0.0f) ? -logf(u01_open(r.c[0])) / lam : NAN;
+    out[i] = v;
+    if (lp) lp[i] = fam::exponential_lp(v, lam);
+  }
+}
+
+// log of a standard Gamma(c) draw.  Marsaglia & Tsang (2000) for c >= 1; c < 1 as G(c + 1) U^(1/c), with the power
+// taken in log space.  Sub-counters sub0 .. sub0 + kGammaCalls - 1 feed the rounds, sub0 + kGammaCalls the boost uniform.
+// Each Philox call gives two attempts (Box-Muller's cosine and sine normals, two uniforms).  The acceptance rate is
+// lowest at c = 1, 0.952, so all 2 * kGammaCalls = 16 attempts fail with probability below 0.048^16 < 1e-20 per draw;
+// the draw then falls back to log(d), deterministically.
+constexpr uint64_t kGammaCalls = 8;
+__device__ float std_gamma_log(float c, uint64_t seed, uint64_t idx, uint64_t offset, uint64_t sub0) {
+  const bool boost = c < 1.0f;
+  const float d = (boost ? c + 1.0f : c) - 1.0f / 3.0f;
+  const float cc = 1.0f / sqrtf(9.0f * d);
+  float lg = logf(d);
+  bool done = false;
+  for (uint64_t k = 0; k < kGammaCalls && !done; ++k) {
+    const ppb_philox r = philox_sub(seed, idx, offset, sub0 + k);
+    const float rad = sqrtf(-2.0f * logf(ppb_u01_open0(r.c[0])));
+    float sn, cs;
+    sincospif(2.0f * ppb_u01(r.c[1]), &sn, &cs);
+    const float z[2] = {rad * cs, rad * sn};
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const float t = 1.0f + cc * z[j];
+      if (done || t <= 0.0f) continue;
+      const float v = t * t * t, x2 = z[j] * z[j], u = ppb_u01_open0(r.c[2 + j]);
+      if (u < 1.0f - 0.0331f * x2 * x2 || logf(u) < 0.5f * x2 + d * (1.0f - v + logf(v))) {
+        lg = logf(d * v);
+        done = true;
+      }
+    }
+  }
+  if (boost) lg += logf(ppb_u01_open0(philox_sub(seed, idx, offset, sub0 + kGammaCalls).c[0])) / c;
+  return lg;
+}
+
+// Gamma: standard draw / rate, clamped below at the smallest normal float as torch's Gamma.rsample does (no draw is 0)
+__global__ void __launch_bounds__(kThreads) k_gamma(P conc, P rate, float* __restrict__ out, float* __restrict__ lp,
+                                                     int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
+  PPB_GRID_LOOP(i) {
+    const float c = conc.at(i), rt = rate.at(i);
+    float v = NAN;
+    if (c > 0.0f && rt > 0.0f)
+      v = fmaxf(expf(std_gamma_log(c, seed, (uint64_t)(first + i), offset, 0) - logf(rt)), PPB_FLT_TINY);
+    out[i] = v;
+    if (lp) lp[i] = fam::gamma_lp(v, c, rt, fam::gamma_const(c, rt));
+  }
+}
+
+// LogNormal: exp of the Box-Muller normal that k_normal draws
+__global__ void __launch_bounds__(kThreads) k_lognormal(P loc, P scale, float* __restrict__ out, float* __restrict__ lp,
+                                                         int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
+  PPB_GRID_LOOP(i) {
+    ppb_philox r = ppb_philox4x32_10(seed, (uint64_t)(first + i), offset);
+    const float mu = loc.at(i), s = scale.at(i);
+    const float v = (s > 0.0f) ? expf(mu + s * ppb_std_normal_from(r.c[0], r.c[1])) : NAN;
+    out[i] = v;
+    if (lp) lp[i] = fam::lognormal_lp(v, mu, s);
+  }
+}
+
+// Weibull: scale (-log u)^(1/k), kept above 0 (the support) where the power underflows
+__global__ void __launch_bounds__(kThreads) k_weibull(P scale, P conc, float* __restrict__ out, float* __restrict__ lp,
+                                                       int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
+  PPB_GRID_LOOP(i) {
+    ppb_philox r = ppb_philox4x32_10(seed, (uint64_t)(first + i), offset);
+    const float lam = scale.at(i), k = conc.at(i);
+    const float v = (lam > 0.0f && k > 0.0f) ? fmaxf(lam * powf(-logf(u01_open(r.c[0])), 1.0f / k), PPB_FLT_TINY) : NAN;
+    out[i] = v;
+    if (lp) lp[i] = fam::weibull_lp(v, lam, k);
+  }
+}
+
+// Beta: Ga / (Ga + Gb) from two standard Gamma draws on disjoint sub-counters, as 1 / (1 + exp(log Gb - log Ga)) so that
+// neither draw underflows; clamped to [tiny, 1 - eps] as torch's Dirichlet sampler clamps; then low + u (high - low)
+__global__ void __launch_bounds__(kThreads) k_beta(P c1, P c0, P low, P high, float* __restrict__ out,
+                                                    float* __restrict__ lp, int64_t n, uint64_t seed, uint64_t offset,
+                                                    int64_t first) {
+  PPB_GRID_LOOP(i) {
+    const uint64_t idx = (uint64_t)(first + i);
+    const float a = c1.at(i), b = c0.at(i), lo = low.at(i), hi = high.at(i);
+    float v = NAN;
+    if (a > 0.0f && b > 0.0f) {
+      const float la = std_gamma_log(a, seed, idx, offset, 0);
+      const float lb = std_gamma_log(b, seed, idx, offset, kGammaCalls + 1);
+      const float u = fminf(fmaxf(1.0f / (1.0f + expf(lb - la)), PPB_FLT_TINY), 1.0f - PPB_EPS32);
+      v = lo + u * (hi - lo);
+    }
+    out[i] = v;
+    if (lp) lp[i] = fam::beta_lp(v, a, b, lo, hi, fam::beta_const(a, b));
+  }
+}
+
+// Binomial, drawn for q = min(p, 1 - p) and mirrored (n - k) for p > 1/2.
+//  * n q < 10: inversion by sequential search from k = 0 with one 53-bit uniform.  The mean is below 10, so
+//    P(X > 110) < 1e-60: the search stops there (and at n).
+//  * n q >= 10: BTRS, transformed rejection with squeeze (W. Hoermann 1993, "The generation of binomial random variates"),
+//    the acceptance test on exact log-factorials in double precision.  Two attempts per Philox call.  The acceptance
+//    rate is lowest at n q = 10, q = 1/2: 0.71, so all 2 * kBtrsCalls = 32 attempts fail with probability below
+//    0.29^32 < 1e-17 per draw; the draw then falls back to the mode, deterministically.
+constexpr uint64_t kBtrsCalls = 16;
+__device__ float binomial_draw(float nf, float p, uint64_t seed, uint64_t idx, uint64_t offset) {
+  if (!fam::binomial_args_ok(nf, p)) return NAN;
+  if (nf == 0.0f || p == 0.0f) return 0.0f;
+  if (p == 1.0f) return nf;
+  const bool flip = p > 0.5f;
+  const double n = nf, q = flip ? 1.0 - (double)p : (double)p;
+  double k;
+  if (n * q < 10.0) {
+    const ppb_philox r = ppb_philox4x32_10(seed, idx, offset);
+    double u = u01_double(r.c[0], r.c[1]);
+    double f = exp(n * log1p(-q));    // P(X = 0)
+    const double s = q / (1.0 - q), kmax = fmin(n, 110.0);
+    k = 0.0;
+    while (u >= f && k < kmax) {
+      u -= f;
+      f *= (n - k) / (k + 1.0) * s;
+      k += 1.0;
+    }
+  } else {
+    const double spq = sqrt(n * q * (1.0 - q));
+    const double b = 1.15 + 2.53 * spq, a = -0.0873 + 0.0248 * b + 0.01 * q, c = n * q + 0.5;
+    const double alpha = (2.83 + 5.1 / b) * spq, vr = 0.92 - 4.2 / b;
+    const double m = floor((n + 1.0) * q), lpq = log(q / (1.0 - q));
+    const double h = lgamma(m + 1.0) + lgamma(n - m + 1.0);
+    k = m;
+    bool done = false;
+    for (uint64_t call = 0; call < kBtrsCalls && !done; ++call) {
+      const ppb_philox r = philox_sub(seed, idx, offset, call);
+#pragma unroll
+      for (int j = 0; j < 4; j += 2) {
+        if (done) continue;
+        const double U = (double)ppb_u01(r.c[j]) - 0.5, V = ppb_u01(r.c[j + 1]);
+        const double us = 0.5 - fabs(U);
+        const double kk = floor((2.0 * a / us + b) * U + c);
+        if (!(kk >= 0.0 && kk <= n)) continue;
+        if ((us >= 0.07 && V <= vr) ||
+            log(V * alpha / (a / (us * us) + b)) <= h - lgamma(kk + 1.0) - lgamma(n - kk + 1.0) + (kk - m) * lpq) {
+          k = kk;
+          done = true;
+        }
+      }
+    }
+  }
+  return (float)(flip ? n - k : k);
+}
+
+__global__ void __launch_bounds__(kThreads) k_binomial(P count, P probs, float* __restrict__ out, float* __restrict__ lp,
+                                                        int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
+  PPB_GRID_LOOP(i) {
+    const float nt = count.at(i), p = probs.at(i);
+    const float v = binomial_draw(nt, p, seed, (uint64_t)(first + i), offset);
+    out[i] = v;
+    if (lp) lp[i] = fam::binomial_lp(v, nt, p, fam::binomial_const(nt, p));
+  }
+}
+
+// VonMises: Best & Fisher (1979) rejection, in double precision as torch's VonMises.sample runs it (kappa (r - f)
+// cancels in fp32 at large kappa), then wrapped as torch does: (x + pi + loc) mod 2 pi - pi.  One round per Philox call.
+// The acceptance rate falls with kappa towards 0.658, so all kVonMisesCalls = 32 rounds fail with probability below
+// 0.343^32 < 1e-14 per draw; the draw then falls back to loc, deterministically.
+constexpr uint64_t kVonMisesCalls = 32;
+__global__ void __launch_bounds__(kThreads) k_von_mises(P loc, P conc, float* __restrict__ out, float* __restrict__ lp,
+                                                         int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
+  const double kPi = 3.14159265358979323846;
+  PPB_GRID_LOOP(i) {
+    const float locf = loc.at(i), kf = conc.at(i);
+    float v = NAN;
+    if (kf > 0.0f) {
+      const double kappa = kf;
+      const double tau = 1.0 + sqrt(1.0 + 4.0 * kappa * kappa);
+      const double rho = (tau - sqrt(2.0 * tau)) / (2.0 * kappa);
+      const double pr = (kappa < 1e-5) ? 1.0 / kappa + kappa : (1.0 + rho * rho) / (2.0 * rho);
+      double x = 0.0;
+      for (uint64_t call = 0; call < kVonMisesCalls; ++call) {
+        const ppb_philox r = philox_sub(seed, (uint64_t)(first + i), offset, call);
+        const double u1 = ppb_u01(r.c[0]), u2 = ppb_u01(r.c[1]), u3 = ppb_u01(r.c[2]);
+        const double z = cospi(u1);
+        const double f = fmin(fmax((1.0 + pr * z) / (pr + z), -1.0), 1.0);
+        const double c = kappa * (pr - f);
+        if (c * (2.0 - c) - u2 > 0.0 || log(c / u2) + 1.0 - c >= 0.0) {
+          x = (u3 > 0.5 ? 1.0 : u3 < 0.5 ? -1.0 : 0.0) * acos(f);
+          break;
+        }
+      }
+      const double y = x + kPi + (double)locf, two_pi = 2.0 * kPi;
+      v = (float)(y - two_pi * floor(y / two_pi) - kPi);
+    }
+    out[i] = v;
+    if (lp) lp[i] = fam::von_mises_lp(v, locf, kf, fam::von_mises_const(kf));
   }
 }
 
@@ -229,6 +446,73 @@ int ppb_bernoulli_sample(const float* probs, int probs_stride, float* value_out,
                                                                                    lp_out, n, seed, offset, first_index);
   PPB_LAUNCH_CHECK();
   return PPB_OK;
+}
+
+#define PPB_LAUNCH_SAMPLER(kernel, ...)                                                                              \
+  do {                                                                                                               \
+    if (n == 0) return PPB_OK;                                                                                       \
+    kernel<<<ppb_grid_for(n, kThreads, 1), kThreads, 0, (cudaStream_t)stream>>>(__VA_ARGS__, value_out, lp_out, n,   \
+                                                                                 seed, offset, first_index);         \
+    PPB_LAUNCH_CHECK();                                                                                              \
+    return PPB_OK;                                                                                                   \
+  } while (0)
+
+int ppb_exponential_sample(const float* rate, int rate_stride, float* value_out, float* lp_out, int64_t n,
+                           uint64_t seed, uint64_t offset, int64_t first_index, void* stream) {
+  PPB_CHECK_ARG(n >= 0 && rate && value_out, "bad arguments");
+  PPB_CHECK_ARG((rate_stride | 1) == 1, "strides must be 0 or 1");
+  PPB_LAUNCH_SAMPLER(k_exponential, P{rate, rate_stride});
+}
+
+int ppb_gamma_sample(const float* concentration, int concentration_stride, const float* rate, int rate_stride,
+                     float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset, int64_t first_index,
+                     void* stream) {
+  PPB_CHECK_ARG(n >= 0 && concentration && rate && value_out, "bad arguments");
+  PPB_CHECK_ARG((concentration_stride | 1) == 1 && (rate_stride | 1) == 1, "strides must be 0 or 1");
+  PPB_LAUNCH_SAMPLER(k_gamma, P{concentration, concentration_stride}, P{rate, rate_stride});
+}
+
+int ppb_lognormal_sample(const float* loc, int loc_stride, const float* scale, int scale_stride, float* value_out,
+                         float* lp_out, int64_t n, uint64_t seed, uint64_t offset, int64_t first_index, void* stream) {
+  PPB_CHECK_ARG(n >= 0 && loc && scale && value_out, "bad arguments");
+  PPB_CHECK_ARG((loc_stride | 1) == 1 && (scale_stride | 1) == 1, "strides must be 0 or 1");
+  PPB_LAUNCH_SAMPLER(k_lognormal, P{loc, loc_stride}, P{scale, scale_stride});
+}
+
+int ppb_weibull_sample(const float* scale, int scale_stride, const float* concentration, int concentration_stride,
+                       float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset, int64_t first_index,
+                       void* stream) {
+  PPB_CHECK_ARG(n >= 0 && scale && concentration && value_out, "bad arguments");
+  PPB_CHECK_ARG((scale_stride | 1) == 1 && (concentration_stride | 1) == 1, "strides must be 0 or 1");
+  PPB_LAUNCH_SAMPLER(k_weibull, P{scale, scale_stride}, P{concentration, concentration_stride});
+}
+
+int ppb_beta_sample(const float* concentration1, int concentration1_stride, const float* concentration0,
+                    int concentration0_stride, const float* low, int low_stride, const float* high, int high_stride,
+                    float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset, int64_t first_index,
+                    void* stream) {
+  PPB_CHECK_ARG(n >= 0 && concentration1 && concentration0 && low && high && value_out, "bad arguments");
+  PPB_CHECK_ARG((concentration1_stride | 1) == 1 && (concentration0_stride | 1) == 1 && (low_stride | 1) == 1 &&
+                    (high_stride | 1) == 1,
+                "strides must be 0 or 1");
+  PPB_LAUNCH_SAMPLER(k_beta, P{concentration1, concentration1_stride}, P{concentration0, concentration0_stride},
+                     P{low, low_stride}, P{high, high_stride});
+}
+
+int ppb_binomial_sample(const float* total_count, int total_count_stride, const float* probs, int probs_stride,
+                        float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset,
+                        int64_t first_index, void* stream) {
+  PPB_CHECK_ARG(n >= 0 && total_count && probs && value_out, "bad arguments");
+  PPB_CHECK_ARG((total_count_stride | 1) == 1 && (probs_stride | 1) == 1, "strides must be 0 or 1");
+  PPB_LAUNCH_SAMPLER(k_binomial, P{total_count, total_count_stride}, P{probs, probs_stride});
+}
+
+int ppb_von_mises_sample(const float* loc, int loc_stride, const float* concentration, int concentration_stride,
+                         float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset,
+                         int64_t first_index, void* stream) {
+  PPB_CHECK_ARG(n >= 0 && loc && concentration && value_out, "bad arguments");
+  PPB_CHECK_ARG((loc_stride | 1) == 1 && (concentration_stride | 1) == 1, "strides must be 0 or 1");
+  PPB_LAUNCH_SAMPLER(k_von_mises, P{loc, loc_stride}, P{concentration, concentration_stride});
 }
 
 int ppb_categorical_sample(const float* probs, int64_t probs_row_stride, int num_categories, float* value_out,

@@ -1,8 +1,10 @@
 // Per-family log_prob over the particle axis — warp-coalesced, 128-bit vectorised, HBM-bound.
 // Replaces pyprob/distributions/distribution.py:38-43 as driven per particle by pyprob/state.py.
 // Algorithmic bytes per element (SURVEY §8d): Normal/Uniform 16 B, Poisson/Bernoulli 12 B, Categorical 4C+12 B,
-// Mixture-Normal (3K+2)*4 B, Mixture-TruncatedNormal (3K+4)*4 B.
+// Mixture-Normal (3K+2)*4 B, Mixture-TruncatedNormal (3K+4)*4 B; Exponential 12 B, Gamma/LogNormal/Weibull/Binomial/
+// VonMises 16 B, Beta 24 B with per-particle parameters (value + lp_out + 4 B per per-particle parameter).
 #include "common.cuh"
+#include "families.cuh"
 
 namespace {
 
@@ -105,6 +107,53 @@ struct BernoulliOp {
   }
 };
 
+// Exponential .. VonMises (families.cuh).  An Op whose log_prob has a term that depends on the parameters only keeps it
+// in the thread together with the parameters it was computed for, and recomputes it only when they change: with shared
+// (stride-0) parameters that is once per thread instead of once per particle (lgammaf alone is ~40 instructions).
+struct ExponentialOp {
+  static constexpr bool kTable = false;
+  __device__ __forceinline__ float operator()(float v, float rate, float, const float*) const {
+    return fam::exponential_lp(v, rate);
+  }
+};
+struct GammaOp {
+  static constexpr bool kTable = false;
+  float c_ = NAN, r_ = NAN, k_ = NAN;
+  __device__ __forceinline__ float operator()(float v, float c, float r, const float*) {
+    if (!(c == c_ && r == r_)) { c_ = c; r_ = r; k_ = fam::gamma_const(c, r); }
+    return fam::gamma_lp(v, c, r, k_);
+  }
+};
+struct LogNormalOp {
+  static constexpr bool kTable = false;
+  __device__ __forceinline__ float operator()(float v, float mu, float s, const float*) const {
+    return fam::lognormal_lp(v, mu, s);
+  }
+};
+struct WeibullOp {
+  static constexpr bool kTable = false;
+  __device__ __forceinline__ float operator()(float v, float scale, float k, const float*) const {
+    return fam::weibull_lp(v, scale, k);
+  }
+};
+struct BinomialOp {
+  static constexpr bool kTable = false;
+  float n_ = NAN, p_ = NAN;
+  fam::BinomialConst k_{NAN, NAN};
+  __device__ __forceinline__ float operator()(float v, float n, float p, const float*) {
+    if (!(n == n_ && p == p_)) { n_ = n; p_ = p; k_ = fam::binomial_const(n, p); }
+    return fam::binomial_lp(v, n, p, k_);
+  }
+};
+struct VonMisesOp {
+  static constexpr bool kTable = false;
+  float kappa_ = NAN, k_ = NAN;
+  __device__ __forceinline__ float operator()(float v, float loc, float kappa, const float*) {
+    if (!(kappa == kappa_)) { kappa_ = kappa; k_ = fam::von_mises_const(kappa); }
+    return fam::von_mises_lp(v, loc, kappa, k_);
+  }
+};
+
 template <class Op, bool VEC>
 __global__ void __launch_bounds__(kThreads) k_score2(const float* __restrict__ value, Param a, Param b, Sink out,
                                                       int64_t n, Op op) {
@@ -146,6 +195,39 @@ int launch_score2(const float* value, Param a, Param b, Sink out, int64_t n, voi
     k_score2<Op, false><<<grid, kThreads, 0, st>>>(value, a, b, out, n, op);
   PPB_LAUNCH_CHECK();
   return PPB_OK;
+}
+
+// ---- beta (four parameters) ----------------------------------------------------------------------------------------------
+// lbeta(c1, c0) is kept per thread while (c1, c0) repeat, as in the Ops above
+template <bool VEC>
+__global__ void __launch_bounds__(kThreads) k_beta(const float* __restrict__ value, Param c1, Param c0, Param low,
+                                                    Param high, Sink out, int64_t n) {
+  int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  int64_t nth = (int64_t)gridDim.x * blockDim.x;
+  float a_ = NAN, b_ = NAN, k_ = NAN;
+  auto lp = [&](float v, float a, float b, float lo, float hi) {
+    if (!(a == a_ && b == b_)) { a_ = a; b_ = b; k_ = fam::beta_const(a, b); }
+    return fam::beta_lp(v, a, b, lo, hi, k_);
+  };
+  int64_t i0 = 0;
+  if (VEC) {
+    int64_t n4 = n >> 2;
+    for (int64_t q = tid; q < n4; q += nth) {
+      int64_t i = q << 2;
+      float4 vv = ldg_stream4(value + i);
+      float v[4] = {vv.x, vv.y, vv.z, vv.w};
+      float pa[4], pb[4], pl[4], ph[4], r[4];
+      c1.load4(i, pa);
+      c0.load4(i, pb);
+      low.load4(i, pl);
+      high.load4(i, ph);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) r[j] = lp(v[j], pa[j], pb[j], pl[j], ph[j]);
+      out.put4(i, r);
+    }
+    i0 = n4 << 2;
+  }
+  for (int64_t i = i0 + tid; i < n; i += nth) out.put(i, lp(__ldg(value + i), c1.at(i), c0.at(i), low.at(i), high.at(i)));
 }
 
 // ---- categorical --------------------------------------------------------------------------------
@@ -317,6 +399,84 @@ int ppb_bernoulli_log_prob(const float* value, const float* probs, int probs_str
   PPB_CHECK_ARG((probs_stride | 1) == 1, "strides must be 0 or 1");
   return launch_score2(value, Param{probs, probs_stride}, Param{probs, 0}, Sink{lp_out, acc, acc_scale}, n, stream,
                        BernoulliOp{});
+}
+
+int ppb_exponential_log_prob(const float* value, const float* rate, int rate_stride, float* lp_out, double* acc,
+                             double acc_scale, int64_t n, void* stream) {
+  if (n == 0) return PPB_OK;
+  PPB_CHECK_ARG(n >= 0 && value && rate, "null pointer or negative n");
+  PPB_CHECK_ARG((rate_stride | 1) == 1, "strides must be 0 or 1");
+  return launch_score2(value, Param{rate, rate_stride}, Param{rate, 0}, Sink{lp_out, acc, acc_scale}, n, stream,
+                       ExponentialOp{});
+}
+
+int ppb_gamma_log_prob(const float* value, const float* concentration, int concentration_stride, const float* rate,
+                       int rate_stride, float* lp_out, double* acc, double acc_scale, int64_t n, void* stream) {
+  if (n == 0) return PPB_OK;
+  PPB_CHECK_ARG(n >= 0 && value && concentration && rate, "null pointer or negative n");
+  PPB_CHECK_ARG((concentration_stride | 1) == 1 && (rate_stride | 1) == 1, "strides must be 0 or 1");
+  return launch_score2(value, Param{concentration, concentration_stride}, Param{rate, rate_stride},
+                       Sink{lp_out, acc, acc_scale}, n, stream, GammaOp{});
+}
+
+int ppb_lognormal_log_prob(const float* value, const float* loc, int loc_stride, const float* scale, int scale_stride,
+                           float* lp_out, double* acc, double acc_scale, int64_t n, void* stream) {
+  if (n == 0) return PPB_OK;
+  PPB_CHECK_ARG(n >= 0 && value && loc && scale, "null pointer or negative n");
+  PPB_CHECK_ARG((loc_stride | 1) == 1 && (scale_stride | 1) == 1, "strides must be 0 or 1");
+  return launch_score2(value, Param{loc, loc_stride}, Param{scale, scale_stride}, Sink{lp_out, acc, acc_scale}, n,
+                       stream, LogNormalOp{});
+}
+
+int ppb_weibull_log_prob(const float* value, const float* scale, int scale_stride, const float* concentration,
+                         int concentration_stride, float* lp_out, double* acc, double acc_scale, int64_t n,
+                         void* stream) {
+  if (n == 0) return PPB_OK;
+  PPB_CHECK_ARG(n >= 0 && value && scale && concentration, "null pointer or negative n");
+  PPB_CHECK_ARG((scale_stride | 1) == 1 && (concentration_stride | 1) == 1, "strides must be 0 or 1");
+  return launch_score2(value, Param{scale, scale_stride}, Param{concentration, concentration_stride},
+                       Sink{lp_out, acc, acc_scale}, n, stream, WeibullOp{});
+}
+
+int ppb_beta_log_prob(const float* value, const float* concentration1, int concentration1_stride,
+                      const float* concentration0, int concentration0_stride, const float* low, int low_stride,
+                      const float* high, int high_stride, float* lp_out, double* acc, double acc_scale, int64_t n,
+                      void* stream) {
+  if (n == 0) return PPB_OK;
+  PPB_CHECK_ARG(n >= 0 && value && concentration1 && concentration0 && low && high, "null pointer or negative n");
+  PPB_CHECK_ARG((concentration1_stride | 1) == 1 && (concentration0_stride | 1) == 1 && (low_stride | 1) == 1 &&
+                    (high_stride | 1) == 1,
+                "strides must be 0 or 1");
+  Param a{concentration1, concentration1_stride}, b{concentration0, concentration0_stride}, lo{low, low_stride},
+      hi{high, high_stride};
+  Sink out{lp_out, acc, acc_scale};
+  const bool vec = aligned16(value) && a.vec_ok() && b.vec_ok() && lo.vec_ok() && hi.vec_ok() && out.vec_ok();
+  const int grid = ppb_grid_for(n, kThreads, 4);
+  if (vec)
+    k_beta<true><<<grid, kThreads, 0, (cudaStream_t)stream>>>(value, a, b, lo, hi, out, n);
+  else
+    k_beta<false><<<grid, kThreads, 0, (cudaStream_t)stream>>>(value, a, b, lo, hi, out, n);
+  PPB_LAUNCH_CHECK();
+  return PPB_OK;
+}
+
+int ppb_binomial_log_prob(const float* value, const float* total_count, int total_count_stride, const float* probs,
+                          int probs_stride, float* lp_out, double* acc, double acc_scale, int64_t n, void* stream) {
+  if (n == 0) return PPB_OK;
+  PPB_CHECK_ARG(n >= 0 && value && total_count && probs, "null pointer or negative n");
+  PPB_CHECK_ARG((total_count_stride | 1) == 1 && (probs_stride | 1) == 1, "strides must be 0 or 1");
+  return launch_score2(value, Param{total_count, total_count_stride}, Param{probs, probs_stride},
+                       Sink{lp_out, acc, acc_scale}, n, stream, BinomialOp{});
+}
+
+int ppb_von_mises_log_prob(const float* value, const float* loc, int loc_stride, const float* concentration,
+                           int concentration_stride, float* lp_out, double* acc, double acc_scale, int64_t n,
+                           void* stream) {
+  if (n == 0) return PPB_OK;
+  PPB_CHECK_ARG(n >= 0 && value && loc && concentration, "null pointer or negative n");
+  PPB_CHECK_ARG((loc_stride | 1) == 1 && (concentration_stride | 1) == 1, "strides must be 0 or 1");
+  return launch_score2(value, Param{loc, loc_stride}, Param{concentration, concentration_stride},
+                       Sink{lp_out, acc, acc_scale}, n, stream, VonMisesOp{});
 }
 
 int ppb_categorical_log_prob(const float* value, const float* probs, int64_t probs_row_stride, int num_categories,

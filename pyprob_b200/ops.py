@@ -85,6 +85,45 @@ def bernoulli_log_prob(value, probs, lp_out=None, acc=None, acc_scale=1.0):
     return lp_out
 
 
+def _score(name, value, params, lp_out, acc, acc_scale):
+    """log_prob entry points of the form (value, (param, stride)..., lp_out, acc, acc_scale, n, stream)."""
+    value = _f32(value, value.device).reshape(-1)
+    n = value.numel()
+    held = [_param(p, n, value.device) for p in params]
+    lp_out, acc = _sink(n, value.device, lp_out, acc)
+    args = [a for _, pp, ps in held for a in (pp, ps)]
+    call(name, ptr(value), *args, ptr(lp_out), ptr(acc), float(acc_scale), n, stream())
+    return lp_out
+
+
+def exponential_log_prob(value, rate, lp_out=None, acc=None, acc_scale=1.0):
+    return _score('ppb_exponential_log_prob', value, (rate,), lp_out, acc, acc_scale)
+
+
+def gamma_log_prob(value, concentration, rate, lp_out=None, acc=None, acc_scale=1.0):
+    return _score('ppb_gamma_log_prob', value, (concentration, rate), lp_out, acc, acc_scale)
+
+
+def lognormal_log_prob(value, loc, scale, lp_out=None, acc=None, acc_scale=1.0):
+    return _score('ppb_lognormal_log_prob', value, (loc, scale), lp_out, acc, acc_scale)
+
+
+def weibull_log_prob(value, scale, concentration, lp_out=None, acc=None, acc_scale=1.0):
+    return _score('ppb_weibull_log_prob', value, (scale, concentration), lp_out, acc, acc_scale)
+
+
+def beta_log_prob(value, concentration1, concentration0, low=0.0, high=1.0, lp_out=None, acc=None, acc_scale=1.0):
+    return _score('ppb_beta_log_prob', value, (concentration1, concentration0, low, high), lp_out, acc, acc_scale)
+
+
+def binomial_log_prob(value, total_count, probs, lp_out=None, acc=None, acc_scale=1.0):
+    return _score('ppb_binomial_log_prob', value, (total_count, probs), lp_out, acc, acc_scale)
+
+
+def von_mises_log_prob(value, loc, concentration, lp_out=None, acc=None, acc_scale=1.0):
+    return _score('ppb_von_mises_log_prob', value, (loc, concentration), lp_out, acc, acc_scale)
+
+
 def _rows(t, n, device):
     """[C] shared or [n, C] per particle -> (tensor, row_stride, C)"""
     if torch.is_tensor(t) and t.is_cuda and t.dtype == torch.float32 and t.dim() == 2 and t.stride(1) == 1 \
@@ -177,6 +216,45 @@ def bernoulli_sample(probs, n, seed, offset, first_index=0, with_log_prob=False,
     v, lp = _out(n, device, with_log_prob)
     call('ppb_bernoulli_sample', pp, ps, ptr(v), ptr(lp), n, seed, offset, first_index, stream())
     return (v, lp) if with_log_prob else v
+
+
+def _sample(name, params, n, seed, offset, first_index, with_log_prob, device):
+    """sampler entry points of the form ((param, stride)..., value_out, lp_out, n, seed, offset, first_index, stream)."""
+    held = [_param(p, n, device) for p in params]
+    v, lp = _out(n, device, with_log_prob)
+    args = [a for _, pp, ps in held for a in (pp, ps)]
+    call(name, *args, ptr(v), ptr(lp), n, seed, offset, first_index, stream())
+    return (v, lp) if with_log_prob else v
+
+
+def exponential_sample(rate, n, seed, offset, first_index=0, with_log_prob=False, device='cuda'):
+    return _sample('ppb_exponential_sample', (rate,), n, seed, offset, first_index, with_log_prob, device)
+
+
+def gamma_sample(concentration, rate, n, seed, offset, first_index=0, with_log_prob=False, device='cuda'):
+    return _sample('ppb_gamma_sample', (concentration, rate), n, seed, offset, first_index, with_log_prob, device)
+
+
+def lognormal_sample(loc, scale, n, seed, offset, first_index=0, with_log_prob=False, device='cuda'):
+    return _sample('ppb_lognormal_sample', (loc, scale), n, seed, offset, first_index, with_log_prob, device)
+
+
+def weibull_sample(scale, concentration, n, seed, offset, first_index=0, with_log_prob=False, device='cuda'):
+    return _sample('ppb_weibull_sample', (scale, concentration), n, seed, offset, first_index, with_log_prob, device)
+
+
+def beta_sample(concentration1, concentration0, low, high, n, seed, offset, first_index=0, with_log_prob=False,
+                device='cuda'):
+    return _sample('ppb_beta_sample', (concentration1, concentration0, low, high), n, seed, offset, first_index,
+                   with_log_prob, device)
+
+
+def binomial_sample(total_count, probs, n, seed, offset, first_index=0, with_log_prob=False, device='cuda'):
+    return _sample('ppb_binomial_sample', (total_count, probs), n, seed, offset, first_index, with_log_prob, device)
+
+
+def von_mises_sample(loc, concentration, n, seed, offset, first_index=0, with_log_prob=False, device='cuda'):
+    return _sample('ppb_von_mises_sample', (loc, concentration), n, seed, offset, first_index, with_log_prob, device)
 
 
 def categorical_sample(probs, n, seed, offset, first_index=0, with_log_prob=False, device='cuda'):
