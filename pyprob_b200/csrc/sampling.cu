@@ -34,6 +34,9 @@ __global__ void __launch_bounds__(kThreads) k_uniform(P low, P high, float* __re
     ppb_philox r = ppb_philox4x32_10(seed, (uint64_t)(first + i), offset);
     float lo = low.at(i), hi = high.at(i);
     float v = lo + ppb_u01(r.c[0]) * (hi - lo);
+    // u < 1, but the fp32 sum can round up onto hi (Uniform(1000, 1001): every u above 1 - 3.05e-5), which log_prob
+    // scores -inf: step such a draw to the largest float below hi
+    if (v >= hi) v = nextafterf(hi, lo);
     out[i] = v;
     if (lp) lp[i] = ((lo <= v && hi > v) ? 0.0f : -INFINITY) - logf(hi - lo);
   }
@@ -41,6 +44,10 @@ __global__ void __launch_bounds__(kThreads) k_uniform(P low, P high, float* __re
 
 // Poisson: inversion by sequential search for rate < 10 (Devroye), PTRS transformed rejection
 // (W. Hoermann 1993) for rate >= 10; the rejection loop draws fresh Philox words with a bumped counter.
+// PTRS runs in double, as torch's CPU sampler does: its log acceptance ratio -rate + k log(rate) - lgamma(k + 1) is a
+// difference of terms near rate log(rate), and in fp32 (spacing 0.125 at 1e6) it is off by tenths from rate 1e5 up, which
+// skews the distribution (variance 1.05 rate at 1e6).  The draw is returned as a float: exact integers up to 2^24, so rates
+// much above 1e7 are not supported.
 __device__ float poisson_draw(float rate, uint64_t seed, uint64_t idx, uint64_t offset) {
   if (!(rate > 0.0f)) return 0.0f;
   if (rate < 10.0f) {
@@ -59,21 +66,21 @@ __device__ float poisson_draw(float rate, uint64_t seed, uint64_t idx, uint64_t 
       if (sub > 64) return k;
     }
   }
-  float slam = sqrtf(rate), loglam = logf(rate);
-  float b = 0.931f + 2.53f * slam;
-  float a = -0.059f + 0.02483f * b;
-  float invalpha = 1.1239f + 1.1328f / (b - 3.4f);
-  float vr = 0.9277f - 3.6224f / (b - 2.0f);
+  const double lam = rate, slam = sqrt(lam), loglam = log(lam);
+  const double b = 0.931 + 2.53 * slam;
+  const double a = -0.059 + 0.02483 * b;
+  const double invalpha = 1.1239 + 1.1328 / (b - 3.4);
+  const double vr = 0.9277 - 3.6224 / (b - 2.0);
   for (uint64_t sub = 0; sub < 64; ++sub) {
     ppb_philox r = ppb_philox4x32_10(seed, idx, offset + (sub << 40));
     for (int j = 0; j < 4; j += 2) {
-      float U = ppb_u01(r.c[j]) - 0.5f;
-      float V = ppb_u01_open0(r.c[j + 1]);
-      float us = 0.5f - fabsf(U);
-      float k = floorf((2.0f * a / us + b) * U + rate + 0.43f);
-      if (us >= 0.07f && V <= vr) return k;
-      if (k < 0.0f || (us < 0.013f && V > us)) continue;
-      if (logf(V) + logf(invalpha) - logf(a / (us * us) + b) <= -rate + k * loglam - lgammaf(k + 1.0f)) return k;
+      const double U = (double)ppb_u01(r.c[j]) - 0.5;
+      const double V = ppb_u01_open0(r.c[j + 1]);
+      const double us = 0.5 - fabs(U);
+      const double k = floor((2.0 * a / us + b) * U + lam + 0.43);
+      if (us >= 0.07 && V <= vr) return (float)k;
+      if (k < 0.0 || (us < 0.013 && V > us)) continue;
+      if (log(V * invalpha / (a / (us * us) + b)) <= -lam + k * loglam - lgamma(k + 1.0)) return (float)k;
     }
   }
   return floorf(rate);
@@ -357,8 +364,9 @@ __device__ __forceinline__ float truncnormal_draw(float mu, float sg, float lo, 
   float q = ca + u * (cb - ca);
   q = fminf(fmaxf(q, 1e-7f), 1.0f - 6e-8f);
   float v = normcdfinvf(q) * sg + mu;
-  // keep the draw inside the truncation domain (the reference retries until it is)
-  return fminf(fmaxf(v, lo), hi);
+  // keep the draw inside [lo, hi): the reference retries until lo <= v < hi, and a Uniform prior that this mixture proposes
+  // for scores v = hi as -inf
+  return fminf(fmaxf(v, lo), nextafterf(hi, lo));
 }
 
 template <bool TRUNC>
