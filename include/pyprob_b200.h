@@ -502,6 +502,51 @@ int ppb_gemm_packed_tn(const float* X_hi, const float* X_lo, const float* Y_hi, 
                        float* C, int64_t M, int64_t N, int64_t R, int64_t ldc, int precision,
                        void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * 7. Metropolis-Hastings chains (LMH / RMH), csrc/mcmc.cu.  C chains run as the C lanes of one lock-step execution.
+ *    Trace tables, column = address (assigned in order of first appearance, pyprob_b200/mcmc.py), row = (buffer, chain):
+ *      val[2, C, lda] fp32, lp[2, C, lda] fp32 prior log-prob, stamp[2, C, lda] int32, reused[2, C, lda] uint8.
+ *    buf[c] (0 / 1) is the buffer of chain c's current trace, 1 - buf[c] its candidate's; accepting flips buf[c].  A cell
+ *    belongs to the current trace iff its stamp equals cur_stamp[c] (the step that made the trace), to the candidate iff
+ *    it equals the running step: nothing is ever cleared.
+ *    Philox key = seed, counter = (chain index c, offset):
+ *      site choice (ppb_mh_select): m present columns of the current row, u = (w0 >> 8) 2^-24 from word 0,
+ *        k = min(floor(u m), m - 1) in fp32, the chosen column is the k-th present one in increasing column order.
+ *      accept (ppb_mh_accept): u = ((w0 >> 8) + 1) 2^-24 from word 0; accept iff log(u) < log alpha (fp64), where
+ *        log alpha = log cur_n - log cand_n + cand_lpo - cur_lpo + reuse + trans, and -inf when cand_n = 0.
+ *      RMH kernel at the chosen site (ppb_mh_site, kind 1 / 2): the kernel draws iff (w0 >> 8) 2^-24 < 0.5, from
+ *        words 1, 2 (Normal: Box-Muller, as the Normal sampler) or word 1 (Uniform: inverse-CDF truncated normal).
+ * ---------------------------------------------------------------------------------------------- */
+#define PPB_MH_KERNEL_PRIOR 0
+#define PPB_MH_KERNEL_NORMAL 1
+#define PPB_MH_KERNEL_UNIFORM 2
+/* Start a step: reset the candidate accumulators (cand_n, cand_lpo, reuse, trans) and, unless initial, write each chain's
+ * chosen column into choice (-1 when its current trace has no site, and always for the initial step). */
+int ppb_mh_select(const int32_t* stamp, const int32_t* buf, const int32_t* cur_stamp, int64_t C, int64_t lda, int ncols,
+                  int32_t* choice, int32_t* cand_n, double* cand_lpo, double* reuse, double* trans, int initial,
+                  uint64_t seed, uint64_t offset, void* stream);
+/* Rows first .. first + n - 1: the current trace's value and log-prob at column col (has = 0 where it has none or the
+ * lane is masked out). */
+int ppb_mh_fetch(const float* val, const float* lp, const int32_t* stamp, const int32_t* buf, const int32_t* cur_stamp,
+                 int64_t C, int64_t lda, int col, const uint8_t* mask, int64_t n, int64_t first, float* old_v,
+                 float* old_lp, uint8_t* has, void* stream);
+/* One executed sample statement: per executing lane, the chosen site takes the fresh prior draw (kind 0) or the RMH
+ * kernel mixture (writing trans); otherwise the current value is reused where has and rescored > -inf (reuse +=
+ * rescored - old_lp), else the fresh draw is taken.  Writes the candidate cell, cand_n += 1 and value_out. */
+int ppb_mh_site(int kind, int col, const uint8_t* mask, int64_t n, int64_t first, const float* fresh_v,
+                const float* fresh_lp, const float* old_v, const float* old_lp, const uint8_t* has,
+                const float* rescored, const float* p0, int p0_stride, const float* p1, int p1_stride, float* val,
+                float* lp, int32_t* stamp, uint8_t* reused_flag, const int32_t* buf, const int32_t* choice,
+                int32_t step, int64_t C, int64_t lda, int32_t* cand_n, double* reuse, double* trans,
+                int64_t* reused_cnt, float* value_out, uint64_t seed, uint64_t offset, void* stream);
+/* End a step: log alpha and the accept draw per chain (initial: accept always), flip and count, then copy the current
+ * map_func row (map_words 32-bit words) into out[slot] when slot >= 0. */
+int ppb_mh_accept(int64_t C, int initial, int32_t step, int32_t* buf, int32_t* cur_stamp, int32_t* cur_n,
+                  double* cur_lpo, const int32_t* cand_n, const double* cand_lpo, const double* reuse,
+                  const double* trans, double* log_alpha, int64_t* accepted, int64_t* sites_all,
+                  const int32_t* cand_map, int32_t* cur_map, int map_words, int32_t* out, int64_t slot, uint64_t seed,
+                  uint64_t offset, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

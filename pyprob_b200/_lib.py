@@ -94,6 +94,12 @@ _SIGNATURES = {
     'ppb_gemm_packed_tn': [c_f, c_f, c_f, c_f, c_f, c_i64, c_i64, c_i64, c_i64, c_int, c_f],
     'ppb_gemm_packed': [c_f, c_f, c_f, c_f, c_f, c_i64, c_i64, c_i64, c_i64, c_f, c_int, c_int, c_f],
     'ppb_gemm_packed_cluster': [c_f, c_f, c_f, c_f, c_f, c_i64, c_i64, c_i64, c_i64, c_f, c_int, c_int, c_int, c_f],
+    'ppb_mh_select': [c_f, c_f, c_f, c_i64, c_i64, c_int, c_f, c_f, c_f, c_f, c_f, c_int, c_u64, c_u64, c_f],
+    'ppb_mh_fetch': [c_f, c_f, c_f, c_f, c_f, c_i64, c_i64, c_int, c_f, c_i64, c_i64, c_f, c_f, c_f, c_f],
+    'ppb_mh_site': [c_int, c_int, c_f, c_i64, c_i64, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_int, c_f, c_int, c_f, c_f,
+                    c_f, c_f, c_f, c_f, c_i32, c_i64, c_i64, c_f, c_f, c_f, c_f, c_f, c_u64, c_u64, c_f],
+    'ppb_mh_accept': [c_i64, c_int, c_i32, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_int, c_f,
+                      c_i64, c_u64, c_u64, c_f],
 }
 _RESTYPES = {
     'ppb_ic_workspace_bytes': c_i64,

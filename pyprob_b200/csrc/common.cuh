@@ -166,6 +166,18 @@ __device__ __forceinline__ float ppb_truncnormal_lp(float v, float mu, float sig
   return inside + (-(z * z) / 2.0f - PPB_LOG_SQRT_2PI) - log_sz;
 }
 
+// inverse-CDF draw (truncated_normal.py:104): icdf(Phi(alpha) + u (Phi(beta)-Phi(alpha))) * sigma + mu; shared by the
+// truncated mixture sampler (sampling.cu) and the RMH Uniform kernel (mcmc.cu)
+__device__ __forceinline__ float ppb_truncnormal_draw(float mu, float sg, float lo, float hi, float u) {
+  float ca = ppb_std_normal_cdf((lo - mu) / sg), cb = ppb_std_normal_cdf((hi - mu) / sg);
+  float q = ca + u * (cb - ca);
+  q = fminf(fmaxf(q, 1e-7f), 1.0f - 6e-8f);
+  float v = normcdfinvf(q) * sg + mu;
+  // keep the draw inside [lo, hi): the reference retries until lo <= v < hi, and a Uniform prior that this mixture proposes
+  // for scores v = hi as -inf
+  return fminf(fmaxf(v, lo), nextafterf(hi, lo));
+}
+
 __device__ __forceinline__ float ppb_warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -358,17 +358,6 @@ __global__ void __launch_bounds__(kThreads) k_categorical(const float* __restric
   }
 }
 
-__device__ __forceinline__ float truncnormal_draw(float mu, float sg, float lo, float hi, float u) {
-  // inverse-CDF draw (truncated_normal.py:104): icdf(Phi(alpha) + u (Phi(beta)-Phi(alpha))) * sigma + mu
-  float ca = ppb_std_normal_cdf((lo - mu) / sg), cb = ppb_std_normal_cdf((hi - mu) / sg);
-  float q = ca + u * (cb - ca);
-  q = fminf(fmaxf(q, 1e-7f), 1.0f - 6e-8f);
-  float v = normcdfinvf(q) * sg + mu;
-  // keep the draw inside [lo, hi): the reference retries until lo <= v < hi, and a Uniform prior that this mixture proposes
-  // for scores v = hi as -inf
-  return fminf(fmaxf(v, lo), nextafterf(hi, lo));
-}
-
 template <bool TRUNC>
 __global__ void __launch_bounds__(kThreads) k_mixture(const float* __restrict__ means,
                                                        const float* __restrict__ stddevs,
@@ -388,7 +377,7 @@ __global__ void __launch_bounds__(kThreads) k_mixture(const float* __restrict__ 
     float lo = 0.f, hi = 0.f, v;
     if (TRUNC) {
       lo = low.at(i); hi = high.at(i);
-      v = truncnormal_draw(mu, sg, lo, hi, ppb_u01(r.c[1]));
+      v = ppb_truncnormal_draw(mu, sg, lo, hi, ppb_u01(r.c[1]));
     } else {
       v = mu + sg * ppb_std_normal_from(r.c[1], r.c[2]);
     }

@@ -5,6 +5,8 @@ Keeps the reference's ``Empirical`` semantics for the part of it that is on the 
 (log-sum-exp), ESS = 1/sum p^2, expectations in fp64 — with the normalisation done by the CUDA reduce
 kernels (ppb_weights_partials / ppb_weights_finalize).  Disk-backed modes, plotting, copying are out of scope.
 """
+import copy
+
 import torch
 
 from . import ops
@@ -48,6 +50,17 @@ class Empirical:
     @property
     def values(self):
         return self._values
+
+    def __getitem__(self, index):
+        """An int gives the value; a slice gives a new Empirical of those values and weights with the metadata copied
+        (reference empirical.py:415-422), e.g. ``posterior[burn_in:]``."""
+        if isinstance(index, slice):
+            values = self._values[index]
+            ret = Empirical(values, self.log_weights[index], name=self.name)
+            ret._metadata = copy.deepcopy(self._metadata)
+            ret.add_metadata(op='slice', index='{}'.format(index))
+            return ret
+        return self._values[index]
 
     def values_numpy(self):
         return self._values.detach().cpu().numpy() if torch.is_tensor(self._values) else self._values

@@ -1,13 +1,13 @@
 """``Model`` — the public entry point, same call signatures as the reference for the importance-sampling
 path (pyprob/model.py:23-225): ``prior[_results]``, ``posterior[_results]``, ``learn_inference_network``,
-``save/load_inference_network``.  MCMC engines, RemoteModel, ParallelModel and on-disk datasets are out of
-scope (SURVEY.md section 8) and raise NotImplementedError.
+``save/load_inference_network``; the MCMC engines (LMH, RMH) run as lock-step chains (mcmc.py).  RemoteModel,
+ParallelModel and on-disk datasets are out of scope (SURVEY.md section 8) and raise NotImplementedError.
 """
 import warnings
 
 import torch
 
-from . import ops, state, util
+from . import mcmc, ops, state, util
 from .dataset import OnlineDataset
 from .distributions import set_shard_first_index
 from .empirical import Empirical
@@ -116,9 +116,19 @@ class Model:
 
     def posterior(self, num_traces=10, inference_engine=InferenceEngine.IMPORTANCE_SAMPLING, initial_trace=None,
                   map_func=None, observe=None, file_name=None, thinning_steps=None, likelihood_importance=1.,
-                  *args, **kwargs):
+                  num_chains=1, *args, **kwargs):
+        """num_chains (LMH / RMH only): independent chains run in lock-step; num_traces is the number of MH steps of each
+        chain and the result holds num_chains * ceil(num_traces / thinning_steps) states in step-major order."""
         if file_name is not None:
             raise NotImplementedError('disk-backed Empiricals are out of scope for pyprob_b200')
+        if inference_engine in (InferenceEngine.LIGHTWEIGHT_METROPOLIS_HASTINGS,
+                                InferenceEngine.RANDOM_WALK_METROPOLIS_HASTINGS):
+            if initial_trace is not None:
+                raise NotImplementedError('pyprob_b200 starts every MH chain from a prior trace; continuing a chain from '
+                                          'initial_trace is out of scope (use the reference for that)')
+            post, _ = mcmc.posterior(self, num_traces, inference_engine, trace_result if map_func is None else map_func,
+                                     observe, thinning_steps, likelihood_importance, num_chains, args, kwargs)
+            return post
         if inference_engine == InferenceEngine.IMPORTANCE_SAMPLING:
             post = self._traces(num_traces, trace_mode=TraceMode.POSTERIOR, inference_engine=inference_engine,
                                 map_func=map_func, observe=observe, likelihood_importance=likelihood_importance,
@@ -136,8 +146,7 @@ class Model:
             post.rename('Posterior, IC, traces: {:,}, train. traces: {:,}, ESS: {:,.2f}'.format(
                 post.length, self._inference_network._total_train_traces, post.effective_sample_size))
         else:
-            raise NotImplementedError('pyprob_b200 implements IMPORTANCE_SAMPLING and '
-                                      'IMPORTANCE_SAMPLING_WITH_INFERENCE_NETWORK; MCMC engines are out of scope')
+            raise NotImplementedError('Unknown inference engine: {}'.format(inference_engine))
         post.add_metadata(op='posterior', num_traces=num_traces, inference_engine=str(inference_engine),
                           effective_sample_size=post.effective_sample_size)
         return post

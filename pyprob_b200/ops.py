@@ -313,3 +313,37 @@ def weights_finalize(log_w, partials=None, want_logits=True):
     call('ppb_weights_finalize', ptr(log_w), n, ptr(partials), partials.numel() // 3, ptr(stats), ptr(logits),
          stream())
     return stats, logits
+
+
+# ---- Metropolis-Hastings chains (C-ABI section 7); `t` is a pyprob_b200.mcmc.Chains ---------------------------------
+
+def mh_select(t, initial, seed, offset):
+    call('ppb_mh_select', ptr(t.stamp), ptr(t.buf), ptr(t.cur_stamp), t.C, t.lda, t.ncols, ptr(t.choice), ptr(t.cand_n),
+         ptr(t.cand_lpo), ptr(t.reuse), ptr(t.trans), int(initial), seed, offset, stream())
+
+
+def mh_fetch(t, col, mask, n, first):
+    old_v = torch.empty(n, dtype=torch.float32, device='cuda')
+    old_lp = torch.empty(n, dtype=torch.float32, device='cuda')
+    has = torch.empty(n, dtype=torch.uint8, device='cuda')
+    call('ppb_mh_fetch', ptr(t.val), ptr(t.lp), ptr(t.stamp), ptr(t.buf), ptr(t.cur_stamp), t.C, t.lda, col, ptr(mask),
+         n, first, ptr(old_v), ptr(old_lp), ptr(has), stream())
+    return old_v, old_lp, has
+
+
+def mh_site(t, kind, col, mask, n, first, fresh_v, fresh_lp, old_v, old_lp, has, rescored, p0, p1, seed, offset):
+    """-> the value the program sees at this statement, [n] fp32"""
+    out = torch.empty(n, dtype=torch.float32, device='cuda')
+    a, ap, as_ = _param(p0 if p0 is not None else 0.0, n, 'cuda')
+    b, bp, bs = _param(p1 if p1 is not None else 0.0, n, 'cuda')
+    call('ppb_mh_site', kind, col, ptr(mask), n, first, ptr(fresh_v), ptr(fresh_lp), ptr(old_v), ptr(old_lp), ptr(has),
+         ptr(rescored), ap, as_, bp, bs, ptr(t.val), ptr(t.lp), ptr(t.stamp), ptr(t.reused), ptr(t.buf), ptr(t.choice),
+         t.step, t.C, t.lda, ptr(t.cand_n), ptr(t.reuse), ptr(t.trans), ptr(t.reused_count), ptr(out), seed, offset,
+         stream())
+    return out
+
+
+def mh_accept(t, initial, slot, seed, offset):
+    call('ppb_mh_accept', t.C, int(initial), t.step, ptr(t.buf), ptr(t.cur_stamp), ptr(t.cur_n), ptr(t.cur_lpo),
+         ptr(t.cand_n), ptr(t.cand_lpo), ptr(t.reuse), ptr(t.trans), ptr(t.log_alpha), ptr(t.accepted),
+         ptr(t.sites_all), ptr(t.cand_map), ptr(t.cur_map), t.map_words, ptr(t.out), slot, seed, offset, stream())

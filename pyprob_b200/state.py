@@ -34,6 +34,7 @@ _mask_parent = None     # the mask this one was narrowed from (while_loop: the p
 _trace_start = None
 _target_cache = {}
 _NO_MASK_YET = object()
+_mcmc = None            # the mcmc.Chains whose candidate traces this execution writes (LMH / RMH), or None
 
 
 # ---- addressing (same information content as the reference's bytecode addresses, state.py:31-84) --------
@@ -178,6 +179,11 @@ def sample(distribution, name=None, address=None, control=True):
         if _trace_mode == TraceMode.POSTERIOR:
             _accumulate(trace, lambda acc: distribution.score_into(value, acc, _likelihood_importance))
         trace.add(Site(distribution, value, base, addr, instance, name=name, observed=True, mask=_mask))
+        return value
+
+    if _mcmc is not None:   # MH: every non-observed sample is controlled (reference state.py:165-166)
+        value = _mcmc.site(distribution, addr, n, _mask)
+        trace.add(Site(distribution, value, base, addr, instance, control=True, name=name, mask=_mask))
         return value
 
     use_network = (_trace_mode == TraceMode.POSTERIOR and control and
@@ -408,10 +414,6 @@ def _init_traces(func, trace_mode=TraceMode.PRIOR, prior_inflation=PriorInflatio
                  likelihood_importance=1.0):
     global _trace_mode, _inference_engine, _prior_inflation, _likelihood_importance
     global _root_function_name, _network, _observed
-    if inference_engine in (InferenceEngine.LIGHTWEIGHT_METROPOLIS_HASTINGS,
-                            InferenceEngine.RANDOM_WALK_METROPOLIS_HASTINGS):
-        raise NotImplementedError('pyprob_b200 implements the importance-sampling engines only (MCMC is sequential '
-                                  'and out of scope; use the reference for LMH/RMH)')
     _trace_mode, _inference_engine = trace_mode, inference_engine
     _prior_inflation, _likelihood_importance = prior_inflation, float(likelihood_importance)
     _root_function_name = func.__code__.co_name
@@ -435,6 +437,8 @@ def _begin_trace(n):
     global _current_trace, _previous_site, _trace_start, _mask
     _trace_start = time.time()
     _current_trace = BatchedTrace(n)
+    if _mcmc is not None:     # the candidate's log_prob_observed accumulates in the chain tables
+        _current_trace.log_w = _mcmc.log_w_view(n)
     _previous_site = None
     _mask = None
     if _network is not None:
