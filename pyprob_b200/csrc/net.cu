@@ -457,7 +457,8 @@ __global__ void __launch_bounds__(256) k_cell_fwd(float* __restrict__ gates, con
 
 // heads: family transform + log q(value) + d(-log q)/d out, loss reduction (:199-218).
 // One WARP per row: lane k owns mixture component k (or categories k, k+32, ...), reductions are shuffles;
-// the formulas are those of heads.cuh (mixture_nll / categorical_nll), restated lane-parallel.
+// the transforms are those of heads.cuh and the log q those of the reference's Mixture / TruncatedNormal / Categorical /
+// Bernoulli, with d(-log q)/d out derived by hand (tests/heads_fp64.py states the same formulas in fp64 with autograd).
 // nll_row is the per-row routine (x = the row's raw head outputs, global or shared memory); two callers:
 // k_head_nll (x read from the output of the h2 GEMM) and NllRowEpi (x parked in shared memory by the h2 cluster GEMM, below).
 struct NllArgs {
@@ -529,8 +530,15 @@ __device__ __forceinline__ void nll_row(const NllArgs& A, const NllRowIn& in, co
       for (int i = 0; i < 4; ++i) { q[i] = (lane + 32 * i < C) ? expf(xs[i] - mx) : 0.0f; s += q[i]; }
       s = ppb_warp_sum(s);
       float S = 0.0f;
+      // sm = the softmax, q = sm + 1e-8 (the probs the reference's Categorical receives); the gradient goes through sm
+      // itself, not q - 1e-8, which loses the digits of a softmax entry far below 1e-8
+      float sm[4];
 #pragma unroll
-      for (int i = 0; i < 4; ++i) { q[i] = (lane + 32 * i < C) ? q[i] / s + PPB_UTIL_EPSILON : 0.0f; S += q[i]; }
+      for (int i = 0; i < 4; ++i) {
+        sm[i] = (lane + 32 * i < C) ? q[i] / s : 0.0f;
+        q[i] = (lane + 32 * i < C) ? sm[i] + PPB_UTIL_EPSILON : 0.0f;
+        S += q[i];
+      }
       S = ppb_warp_sum(S);
       const int iv = (int)v;
       if (iv < 0 || iv >= C) {
@@ -549,13 +557,13 @@ __device__ __forceinline__ void nll_row(const NllArgs& A, const NllRowIn& in, co
           for (int i = 0; i < 4; ++i) {
             int c = lane + 32 * i;
             g[i] = c < C ? ((c == iv) ? 1.0f / qv : 0.0f) - 1.0f / S : 0.0f;
-            dot += c < C ? (q[i] - PPB_UTIL_EPSILON) * g[i] : 0.0f;
+            dot += c < C ? sm[i] * g[i] : 0.0f;
           }
           dot = ppb_warp_sum(dot);
-          g0 = -((q[0] - PPB_UTIL_EPSILON) * (g[0] - dot));
-          g1 = (lane + 32 < C) ? -((q[1] - PPB_UTIL_EPSILON) * (g[1] - dot)) : 0.f;
-          g2 = (lane + 64 < C) ? -((q[2] - PPB_UTIL_EPSILON) * (g[2] - dot)) : 0.f;
-          g3 = (lane + 96 < C) ? -((q[3] - PPB_UTIL_EPSILON) * (g[3] - dot)) : 0.f;
+          g0 = -(sm[0] * (g[0] - dot));
+          g1 = (lane + 32 < C) ? -(sm[1] * (g[1] - dot)) : 0.f;
+          g2 = (lane + 64 < C) ? -(sm[2] * (g[2] - dot)) : 0.f;
+          g3 = (lane + 96 < C) ? -(sm[3] * (g[3] - dot)) : 0.f;
           if (lane >= C) g0 = 0.f;
         }
       }
@@ -595,28 +603,35 @@ __device__ __forceinline__ void nll_row(const NllArgs& A, const NllRowIn& in, co
         float direct = (on && !clamped) ? r / ph : 0.0f;
         float g_prob = (direct - sum_r_unc) / S;
         float dot = ppb_warp_sum(on ? prob * g_prob : 0.0f);
-        float z = (v - mean) / sd, dmu, dsd;
-        if (!trunc) { dmu = z / sd; dsd = (z * z - 1.0f) / sd; }
+        // dmu = sd d lp_k / d mean and dls = sd d lp_k / d sd, then the transform's factor over sd: nothing overflows where
+        // the exact gradient fits fp32 (z / sd and (z^2 - 1) / sd alone do from sd ~ 1e-13 on)
+        float z = (v - mean) / sd, dmu, dls;
+        if (!trunc) { dmu = z; dls = z * z - 1.0f; }
         else {
           float alpha = (lo - mean) / sd, beta = (hi - mean) / sd;
           float Z = ppb_std_normal_cdf(beta) - ppb_std_normal_cdf(alpha);
           float pa = heads::std_normal_pdf(alpha), pb = heads::std_normal_pdf(beta);
-          dmu = z / sd - (pa - pb) / (sd * Z);
-          dsd = (z * z - 1.0f) / sd - (alpha * pa - beta * pb) / (sd * Z);
+          dmu = z - (pa - pb) / Z;
+          dls = z * z - 1.0f - (alpha * pa - beta * pb) / Z;
         }
-        dmu *= r; dsd *= r;
         float dxm, dxs;
-        if (fam == PPB_FAMILY_NORMAL) { dxm = dmu * p1; dxs = dsd * sd; }
+        if (fam == PPB_FAMILY_NORMAL) { dxm = (dmu * p1) / sd; dxs = dls; }
         else if (fam == PPB_FAMILY_UNIFORM) {
           float range = p1 - p0, sm = heads::sigmoidf_(xm), ss = heads::sigmoidf_(xsd);
-          dxm = dmu * sm * (1.0f - sm) * range;
-          dxs = dsd * ss * (1.0f - ss) * range * 10.0f;
-        } else { float sm = heads::sigmoidf_(xm); dxm = dmu * sm * (1.0f - sm) * 40.0f; dxs = dsd * sd; }
+          dxm = (dmu * (sm * (1.0f - sm) * range)) / sd;
+          dxs = (dls * (ss * (1.0f - ss) * range * 10.0f)) / sd;
+        } else { float sm = heads::sigmoidf_(xm); dxm = (dmu * (sm * (1.0f - sm) * 40.0f)) / sd; dxs = dls; }
+        // a component with responsibility 0 contributes nothing: its derivatives may overflow (a tiny sd far from v) and
+        // 0 * inf would put NaN into d_out with the status still 0 (DESIGN.md §8)
+        dxm = r > 0.0f ? dxm * r : 0.0f; dxs = r > 0.0f ? dxs * r : 0.0f;
         if (on) { g0 = -dxm; g1 = -dxs; g2 = -(prob * (g_prob - dot)); }
       }
     }
     if (lp == -INFINITY) { lp = PPB_LOG_EPSILON; g0 = g1 = g2 = g3 = 0.f; }  // util.replace_negative_inf (:213)
-    if (isnan(lp) || isinf(lp)) { if (lane == 0) bad += 1; lp = 0.0f; g0 = g1 = g2 = g3 = 0.f; }
+    // a finite log q whose gradient does not fit fp32 (a component with sd ~ 1e-20 that explains v from 0.3 away:
+    // d(-log q)/d out ~ 1e38 and beyond) fails the batch like a NaN log q, so that no inf reaches the optimiser (DESIGN.md §8)
+    const bool g_bad = __any_sync(0xffffffffu, !(isfinite(g0) && isfinite(g1) && isfinite(g2) && isfinite(g3)));
+    if (isnan(lp) || isinf(lp) || g_bad) { if (lane == 0) bad += 1; lp = 0.0f; g0 = g1 = g2 = g3 = 0.f; }
     if (lane == 0) local += -lp;
   }
   if (row_lp && lane == 0) row_lp[row] = lp;
