@@ -547,6 +547,34 @@ int ppb_mh_accept(int64_t C, int initial, int32_t step, int32_t* buf, int32_t* c
                   const int32_t* cand_map, int32_t* cur_map, int map_words, int32_t* out, int64_t slot, uint64_t seed,
                   uint64_t offset, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * 8. MCMC diagnostics, csrc/diagnostics.cu: Gelman-Rubin R-hat against the prefix length and per-chain autocorrelation
+ *    (replaces pyprob/diagnostics.py:714-873, the reference's python loops over traces, lags and steps).
+ *    x holds S steps of C chains of V variables: x[s, c, v] at element s * stride_s + c * stride_c + v * stride_v, fp32
+ *    (PPB_DIAG_F32) or fp64 (PPB_DIAG_F64).  iters / lags are HOST int64 arrays; out is device fp64.  Every statistic is
+ *    accumulated in fp64 in a fixed order (two calls give the same bits); means and variances are Welford / Chan
+ *    combinations, never sum(x^2) - sum(x)^2 / n.  The caller allocates the device workspace of the size the
+ *    *_workspace_bytes function returns for the same arguments (-1: invalid arguments).  R-hat's workspace is
+ *    at most max(256 MiB, (2^17 + C V) * 16 B) + n_distinct_iters * V * ceil(C / 256) * 32 B, so a per-iteration curve
+ *    (iters = 1 .. S) costs 32 B per (iteration, variable, 256 chains), not per chain; autocorrelation's is at most about 1 GiB of per-chunk
+ *    partials plus 16 B per value column.
+ *    R-hat (diagnostics.py:788-796), for every iters[i] (any order, >= 1; values above S mean S) with n = min(iters[i], S)
+ *    and m = C: b = n var(chain means of x[:n], ddof 1), w = mean(chain variances of x[:n], ddof 1),
+ *    out[v * n_iters + i] = sqrt(((n - 1) / n w + b / n) / w) -- NaN at n = 1, inf / NaN where w = 0, as numpy.  C >= 2.
+ *    Autocorrelation (diagnostics.py:720-736), for every lags[l] in [0, S]: with mu the chain's mean over all S steps,
+ *    out[(v * C + c) * n_lags + l] = sum_{i < S - lag} (x_i - mu)(x_{i+lag} - mu) / (1e-8 + sum_i (x_i - mu)^2).
+ * ---------------------------------------------------------------------------------------------- */
+#define PPB_DIAG_F32 0
+#define PPB_DIAG_F64 1
+int64_t ppb_diag_rhat_workspace_bytes(int64_t S, int64_t C, int64_t V, const int64_t* iters, int n_iters);
+int ppb_diag_rhat(const void* x, int dtype, int64_t S, int64_t C, int64_t V, int64_t stride_s, int64_t stride_c,
+                  int64_t stride_v, const int64_t* iters, int n_iters, double* out, void* workspace,
+                  int64_t workspace_bytes, void* stream);
+int64_t ppb_diag_autocorr_workspace_bytes(int dtype, int64_t S, int64_t C, int64_t V, int n_lags);
+int ppb_diag_autocorr(const void* x, int dtype, int64_t S, int64_t C, int64_t V, int64_t stride_s, int64_t stride_c,
+                      int64_t stride_v, const int64_t* lags, int n_lags, double* out, void* workspace,
+                      int64_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -10,3 +10,4 @@ from .util import (InferenceEngine, InferenceNetwork, LearningRateScheduler, Obs
 from .state import factor, observe, sample, tag, while_loop  # noqa: F401
 from .model import Model  # noqa: F401
 from . import distributions  # noqa: F401
+from . import diagnostics  # noqa: F401

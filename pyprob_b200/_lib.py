@@ -100,8 +100,15 @@ _SIGNATURES = {
                     c_f, c_f, c_f, c_f, c_i32, c_i64, c_i64, c_f, c_f, c_f, c_f, c_f, c_u64, c_u64, c_f],
     'ppb_mh_accept': [c_i64, c_int, c_i32, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_int, c_f,
                       c_i64, c_u64, c_u64, c_f],
+    'ppb_diag_rhat_workspace_bytes': [c_i64, c_i64, c_i64, C.c_void_p, c_int],
+    'ppb_diag_rhat': [c_f, c_int, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, C.c_void_p, c_int, c_f, c_f, c_i64, c_f],
+    'ppb_diag_autocorr_workspace_bytes': [c_int, c_i64, c_i64, c_i64, c_int],
+    'ppb_diag_autocorr': [c_f, c_int, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, C.c_void_p, c_int, c_f, c_f, c_i64,
+                          c_f],
 }
 _RESTYPES = {
+    'ppb_diag_rhat_workspace_bytes': c_i64,
+    'ppb_diag_autocorr_workspace_bytes': c_i64,
     'ppb_ic_workspace_bytes': c_i64,
     'ppb_ic_infer_workspace_bytes': c_i64,
     'ppb_packed_floats': c_i64,
@@ -111,7 +118,8 @@ _RESTYPES = {
 }
 # entry points whose integer return value is data, not a status
 _VALUE_RETURNS = {'ppb_optimizer_scratch_bytes', 'ppb_version', 'ppb_device_arch', 'ppb_weights_num_partials', 'ppb_ic_workspace_bytes',
-                  'ppb_ic_infer_workspace_bytes', 'ppb_packed_floats', 'ppb_sizeof', 'ppb_launch_count'}
+                  'ppb_ic_infer_workspace_bytes', 'ppb_packed_floats', 'ppb_sizeof', 'ppb_launch_count',
+                  'ppb_diag_rhat_workspace_bytes', 'ppb_diag_autocorr_workspace_bytes'}
 
 EXPORTED_SYMBOLS = sorted(list(_SIGNATURES.keys()) + ['ppb_last_error'])
 

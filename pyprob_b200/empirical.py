@@ -87,6 +87,11 @@ class Empirical:
     def effective_sample_size(self):
         return float(self._stats[1])
 
+    @property
+    def metadata(self):
+        """The list of metadata dicts (e.g. ``op='posterior', num_chains=...``), oldest first."""
+        return self._metadata
+
     def add_metadata(self, **kwargs):
         self._metadata.append(kwargs)
 

@@ -3,6 +3,9 @@
 Every function takes CUDA fp32 tensors and launches on the current torch stream.  Parameters may be
 0-d / 1-element tensors (broadcast over particles) or length-n tensors.
 """
+import ctypes
+
+import numpy as np
 import torch
 
 from . import _lib
@@ -347,3 +350,45 @@ def mh_accept(t, initial, slot, seed, offset):
     call('ppb_mh_accept', t.C, int(initial), t.step, ptr(t.buf), ptr(t.cur_stamp), ptr(t.cur_n), ptr(t.cur_lpo),
          ptr(t.cand_n), ptr(t.cand_lpo), ptr(t.reuse), ptr(t.trans), ptr(t.log_alpha), ptr(t.accepted),
          ptr(t.sites_all), ptr(t.cand_map), ptr(t.cur_map), t.map_words, ptr(t.out), slot, seed, offset, stream())
+
+
+# ---- MCMC diagnostics (C-ABI section 8); x is a CUDA tensor [S, C, V], fp32 or fp64, any strides ---------------------
+
+def _diag_args(x):
+    if x.dim() != 3 or x.dtype not in (torch.float32, torch.float64):
+        raise ValueError('diagnostics kernels take a [S, C, V] fp32 or fp64 tensor, got {} {}'.format(
+            tuple(x.shape), x.dtype))
+    dtype = 0 if x.dtype == torch.float32 else 1
+    return (ptr(x), dtype) + tuple(x.shape) + tuple(x.stride())
+
+
+def _host_i64(a):
+    a = np.ascontiguousarray(np.asarray(a, dtype=np.int64).reshape(-1))
+    return a, a.ctypes.data_as(ctypes.c_void_p)
+
+
+def diag_rhat(x, iters):
+    """R-hat of every variable at every prefix length in iters (host ints >= 1) -> fp64 CUDA tensor [V, len(iters)]."""
+    S, Cn, V = x.shape
+    it, it_p = _host_i64(iters)
+    nbytes = _lib.call('ppb_diag_rhat_workspace_bytes', S, Cn, V, it_p, len(it))
+    if nbytes < 0:
+        raise ValueError('ppb_diag_rhat: invalid arguments (S = {}, C = {}, V = {}, iters = {})'.format(S, Cn, V, it))
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+    out = torch.empty(V, len(it), dtype=torch.float64, device=x.device)
+    call('ppb_diag_rhat', *_diag_args(x), it_p, len(it), ptr(out), ptr(ws), nbytes, stream())
+    return out
+
+
+def diag_autocorr(x, lags):
+    """Autocorrelation of every chain of every variable at lags (host ints in [0, S]) -> fp64 CUDA tensor
+    [V, C, len(lags)]."""
+    S, Cn, V = x.shape
+    lg, lg_p = _host_i64(lags)
+    nbytes = _lib.call('ppb_diag_autocorr_workspace_bytes', _diag_args(x)[1], S, Cn, V, len(lg))
+    if nbytes < 0:
+        raise ValueError('ppb_diag_autocorr: invalid arguments (S = {}, C = {}, V = {})'.format(S, Cn, V))
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+    out = torch.empty(V, Cn, len(lg), dtype=torch.float64, device=x.device)
+    call('ppb_diag_autocorr', *_diag_args(x), lg_p, len(lg), ptr(out), ptr(ws), nbytes, stream())
+    return out
