@@ -189,6 +189,51 @@ int ppb_mixture_truncated_normal_sample(const float* means, const float* stddevs
                                         int64_t first_index, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * 2b. Event-shaped observations: sites whose value is a vector or an image
+ *
+ * Replace  pyprob/state.py:118-155 with a tensor value: distribution.log_prob(value, sum=True) as
+ * pyprob/distributions/distribution.py:38-43 computes it (torch broadcasts the value against the parameters and the
+ * element-wise log-densities are summed), and pyprob/state.py:136-137, which draws the observed value from the
+ * likelihood for a training trace.  A site has D = prod(event shape) elements per particle.
+ * Every operand is (pointer, particle stride ps, element stride es): element j of particle i is p[i ps + j es], and
+ * (ps, es) must be one of (0, 0) scalar, (1, 0) one per particle, (0, 1) shared event, (D, 1) event per particle.
+ * Families and their parameters p0 .. p3 (unused slots are ignored):
+ *   NORMAL (loc, scale), UNIFORM (low, high), POISSON (rate), BERNOULLI (probs), EXPONENTIAL (rate),
+ *   GAMMA (concentration, rate), LOGNORMAL (loc, scale), WEIBULL (scale, concentration),
+ *   BETA (concentration1, concentration0, low, high), BINOMIAL (total_count, probs), VON_MISES (loc, concentration);
+ * each element is scored exactly as the family's section-1 entry point scores a particle.
+ * ---------------------------------------------------------------------------------------------- */
+#define PPB_EVENT_NORMAL 0
+#define PPB_EVENT_UNIFORM 1
+#define PPB_EVENT_POISSON 2
+#define PPB_EVENT_BERNOULLI 3
+#define PPB_EVENT_EXPONENTIAL 4
+#define PPB_EVENT_GAMMA 5
+#define PPB_EVENT_LOGNORMAL 6
+#define PPB_EVENT_WEIBULL 7
+#define PPB_EVENT_BETA 8
+#define PPB_EVENT_BINOMIAL 9
+#define PPB_EVENT_VON_MISES 10
+/* acc (nullable) fp64[n]: acc[i] += acc_scale * sum_j lp_ij, summed in fp64 in an order that depends on (n, D) only,
+ * without atomics (repeated calls give identical bits; with D = 1 the update is the section-1 entry point's).
+ * lp_out (nullable) fp32[n, D], row-major: the element-wise log-densities.  PPB_EINVAL for an unknown family, n < 0,
+ * D < 1, a null operand the family needs, or strides not of the four forms. */
+int ppb_event_log_prob(int family, const float* value, int64_t value_ps, int64_t value_es, const float* p0,
+                       int64_t p0_ps, int64_t p0_es, const float* p1, int64_t p1_ps, int64_t p1_es,
+                       const float* p2, int64_t p2_ps, int64_t p2_es, const float* p3, int64_t p3_ps,
+                       int64_t p3_es, int64_t n, int64_t D, float* lp_out, double* acc, double acc_scale,
+                       void* stream);
+/* value_out fp32[n, D] row-major; lp_out (nullable) fp32[n]: the row's event-summed log-density, as
+ * ppb_event_log_prob sums it.  Element j of particle i draws with the family's section-2 draw from the Philox counter
+ * ((first_index + i) | (j << 40), offset + (round << 40)): element 0 is the section-2 draw bit for bit, and a shard of
+ * the particles draws the rows the full run draws.  PPB_EINVAL, besides the cases above, for D > 2^24 or
+ * first_index + n > 2^40 (the counter fields would overlap). */
+int ppb_event_sample(int family, const float* p0, int64_t p0_ps, int64_t p0_es, const float* p1, int64_t p1_ps,
+                     int64_t p1_es, const float* p2, int64_t p2_ps, int64_t p2_es, const float* p3, int64_t p3_ps,
+                     int64_t p3_es, float* value_out, float* lp_out, int64_t n, int64_t D, uint64_t seed,
+                     uint64_t offset, int64_t first_index, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * 3. Importance-weight normalisation (SURVEY §8a rows a14, a15)
  *
  * Replaces  pyprob/distributions/empirical.py:298-302 (Categorical(logits=log_weights.double()))

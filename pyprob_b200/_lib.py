@@ -58,6 +58,10 @@ _SIGNATURES = {
     'ppb_mixture_normal_sample': [c_f, c_f, c_f, c_i64, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
     'ppb_mixture_truncated_normal_sample': [c_f, c_f, c_f, c_i64, c_int, c_f, c_int, c_f, c_int, c_f, c_f, c_i64,
                                             c_u64, c_u64, c_i64, c_f],
+    'ppb_event_log_prob': [c_int, c_f, c_i64, c_i64, c_f, c_i64, c_i64, c_f, c_i64, c_i64, c_f, c_i64, c_i64, c_f,
+                           c_i64, c_i64, c_i64, c_i64, c_f, c_f, c_dbl, c_f],
+    'ppb_event_sample': [c_int, c_f, c_i64, c_i64, c_f, c_i64, c_i64, c_f, c_i64, c_i64, c_f, c_i64, c_i64, c_f, c_f,
+                         c_i64, c_i64, c_u64, c_u64, c_i64, c_f],
     'ppb_weights_cast': [c_f, c_f, c_f, c_i64, c_f],
     'ppb_weights_num_partials': [c_i64],
     'ppb_weights_partials': [c_f, c_i64, c_f, c_f],

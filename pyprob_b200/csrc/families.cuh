@@ -116,3 +116,10 @@ __device__ __forceinline__ float von_mises_lp(float v, float loc, float kappa, f
 }
 
 }  // namespace fam
+
+// Event-summed log_prob (scoring.cu), shared with the event samplers (sampling.cu), whose lp_out is this kernel's fp32
+// row sum of the drawn rows.  params / params_ps / params_es hold ppb_event_num_params(family) operands.
+int ppb_event_num_params(int family);
+int ppb_event_score(int family, const float* value, int64_t value_ps, int64_t value_es, const float* const* params,
+                    const int64_t* params_ps, const int64_t* params_es, int64_t n, int64_t D, float* lp_out,
+                    float* row_lp, double* acc, double acc_scale, void* stream);

@@ -1,6 +1,9 @@
 // Samplers over the particle axis (Philox4x32-10, counter = (global particle index, offset)).
 // Replaces pyprob/distributions/distribution.py:31-36, mixture.py:47-63, truncated_normal.py:94-112.
 // Fused sample+score: lp_out (nullable) gets log_prob of the drawn value (pyprob/state.py:196-197).
+// Event draws (k_event_sample, [n, D]): element j of particle i uses Philox index (first + i) | (j << 40) and the usual
+// offset + (round << 40) for rejection rounds, so particle indices must stay below 2^40 and D at most 2^24 (checked
+// before launch); element 0 is the per-particle draw, and a shard of the particles draws the full run's rows.
 #include "common.cuh"
 #include "families.cuh"
 
@@ -14,10 +17,21 @@ struct P {
   __device__ __forceinline__ float at(int64_t i) const { return stride ? __ldg(p + i) : __ldg(p); }
 };
 
+// The draw of each family from Philox counter (idx, offset [+ (round << 40)]), shared by the per-particle samplers and the
+// event sampler (k_event_sample), so that element 0 of an event row is the per-particle draw bit for bit.
+// The single-counter families take the Philox words of (idx, offset).  k_normal and k_von_mises spell their draw out in
+// the kernel: with the draw behind a function their SASS changes (instruction order and registers), and the test that
+// element 0 of an event row is the per-particle draw bit for bit ties the two forms together.
+__device__ __forceinline__ float normal_draw(const ppb_philox& r, float mu, float s) {
+  float z = ppb_std_normal_from(r.c[0], r.c[1]);
+  return mu + s * z;
+}
+
 __global__ void __launch_bounds__(kThreads) k_normal(P mean, P sd, float* __restrict__ out, float* __restrict__ lp,
                                                       int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
   int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, nth = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i = tid; i < n; i += nth) {
+    // the draw of normal_draw (the event sampler's), spelled out: change both together
     ppb_philox r = ppb_philox4x32_10(seed, (uint64_t)(first + i), offset);
     float z = ppb_std_normal_from(r.c[0], r.c[1]);
     float mu = mean.at(i), s = sd.at(i);
@@ -27,16 +41,21 @@ __global__ void __launch_bounds__(kThreads) k_normal(P mean, P sd, float* __rest
   }
 }
 
+__device__ __forceinline__ float uniform_draw(const ppb_philox& r, float lo, float hi) {
+  float v = lo + ppb_u01(r.c[0]) * (hi - lo);
+  // u < 1, but the fp32 sum can round up onto hi (Uniform(1000, 1001): every u above 1 - 3.05e-5), which log_prob
+  // scores -inf: step such a draw to the largest float below hi
+  if (v >= hi) v = nextafterf(hi, lo);
+  return v;
+}
+
 __global__ void __launch_bounds__(kThreads) k_uniform(P low, P high, float* __restrict__ out, float* __restrict__ lp,
                                                        int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
   int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, nth = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i = tid; i < n; i += nth) {
     ppb_philox r = ppb_philox4x32_10(seed, (uint64_t)(first + i), offset);
     float lo = low.at(i), hi = high.at(i);
-    float v = lo + ppb_u01(r.c[0]) * (hi - lo);
-    // u < 1, but the fp32 sum can round up onto hi (Uniform(1000, 1001): every u above 1 - 3.05e-5), which log_prob
-    // scores -inf: step such a draw to the largest float below hi
-    if (v >= hi) v = nextafterf(hi, lo);
+    float v = uniform_draw(r, lo, hi);
     out[i] = v;
     if (lp) lp[i] = ((lo <= v && hi > v) ? 0.0f : -INFINITY) - logf(hi - lo);
   }
@@ -98,13 +117,17 @@ __global__ void __launch_bounds__(kThreads) k_poisson(P rate, float* __restrict_
 }
 
 // Bernoulli: 1 if u < p (u uniform in [0, 1) from word 0), so p = 0 never and p = 1 always draws 1
+__device__ __forceinline__ bool bernoulli_one(const ppb_philox& r, float p) {
+  return ppb_u01(r.c[0]) < p;
+}
+
 __global__ void __launch_bounds__(kThreads) k_bernoulli(P probs, float* __restrict__ out, float* __restrict__ lp,
                                                          int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
   int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, nth = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i = tid; i < n; i += nth) {
     ppb_philox r = ppb_philox4x32_10(seed, (uint64_t)(first + i), offset);
     const float p = probs.at(i);
-    const bool one = ppb_u01(r.c[0]) < p;
+    const bool one = bernoulli_one(r, p);
     out[i] = one ? 1.0f : 0.0f;
     if (lp) {
       const float pc = ppb_clamp_prob(p);
@@ -128,12 +151,16 @@ __device__ __forceinline__ ppb_philox philox_sub(uint64_t seed, uint64_t idx, ui
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
 
 // Exponential: inversion, -log(u) / rate
+__device__ __forceinline__ float exponential_draw(const ppb_philox& r, float lam) {
+  return (lam > 0.0f) ? -logf(u01_open(r.c[0])) / lam : NAN;
+}
+
 __global__ void __launch_bounds__(kThreads) k_exponential(P rate, float* __restrict__ out, float* __restrict__ lp,
                                                            int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
   PPB_GRID_LOOP(i) {
     ppb_philox r = ppb_philox4x32_10(seed, (uint64_t)(first + i), offset);
     const float lam = rate.at(i);
-    const float v = (lam > 0.0f) ? -logf(u01_open(r.c[0])) / lam : NAN;
+    const float v = exponential_draw(r, lam);
     out[i] = v;
     if (lp) lp[i] = fam::exponential_lp(v, lam);
   }
@@ -173,37 +200,50 @@ __device__ float std_gamma_log(float c, uint64_t seed, uint64_t idx, uint64_t of
 }
 
 // Gamma: standard draw / rate, clamped below at the smallest normal float as torch's Gamma.rsample does (no draw is 0)
+__device__ __forceinline__ float gamma_draw(float c, float rt, uint64_t seed, uint64_t idx, uint64_t offset) {
+  float v = NAN;
+  if (c > 0.0f && rt > 0.0f)
+    v = fmaxf(expf(std_gamma_log(c, seed, idx, offset, 0) - logf(rt)), PPB_FLT_TINY);
+  return v;
+}
+
 __global__ void __launch_bounds__(kThreads) k_gamma(P conc, P rate, float* __restrict__ out, float* __restrict__ lp,
                                                      int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
   PPB_GRID_LOOP(i) {
     const float c = conc.at(i), rt = rate.at(i);
-    float v = NAN;
-    if (c > 0.0f && rt > 0.0f)
-      v = fmaxf(expf(std_gamma_log(c, seed, (uint64_t)(first + i), offset, 0) - logf(rt)), PPB_FLT_TINY);
+    const float v = gamma_draw(c, rt, seed, (uint64_t)(first + i), offset);
     out[i] = v;
     if (lp) lp[i] = fam::gamma_lp(v, c, rt, fam::gamma_const(c, rt));
   }
 }
 
 // LogNormal: exp of the Box-Muller normal that k_normal draws
+__device__ __forceinline__ float lognormal_draw(const ppb_philox& r, float mu, float s) {
+  return (s > 0.0f) ? expf(mu + s * ppb_std_normal_from(r.c[0], r.c[1])) : NAN;
+}
+
 __global__ void __launch_bounds__(kThreads) k_lognormal(P loc, P scale, float* __restrict__ out, float* __restrict__ lp,
                                                          int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
   PPB_GRID_LOOP(i) {
     ppb_philox r = ppb_philox4x32_10(seed, (uint64_t)(first + i), offset);
     const float mu = loc.at(i), s = scale.at(i);
-    const float v = (s > 0.0f) ? expf(mu + s * ppb_std_normal_from(r.c[0], r.c[1])) : NAN;
+    const float v = lognormal_draw(r, mu, s);
     out[i] = v;
     if (lp) lp[i] = fam::lognormal_lp(v, mu, s);
   }
 }
 
 // Weibull: scale (-log u)^(1/k), kept above 0 (the support) where the power underflows
+__device__ __forceinline__ float weibull_draw(const ppb_philox& r, float lam, float k) {
+  return (lam > 0.0f && k > 0.0f) ? fmaxf(lam * powf(-logf(u01_open(r.c[0])), 1.0f / k), PPB_FLT_TINY) : NAN;
+}
+
 __global__ void __launch_bounds__(kThreads) k_weibull(P scale, P conc, float* __restrict__ out, float* __restrict__ lp,
                                                        int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
   PPB_GRID_LOOP(i) {
     ppb_philox r = ppb_philox4x32_10(seed, (uint64_t)(first + i), offset);
     const float lam = scale.at(i), k = conc.at(i);
-    const float v = (lam > 0.0f && k > 0.0f) ? fmaxf(lam * powf(-logf(u01_open(r.c[0])), 1.0f / k), PPB_FLT_TINY) : NAN;
+    const float v = weibull_draw(r, lam, k);
     out[i] = v;
     if (lp) lp[i] = fam::weibull_lp(v, lam, k);
   }
@@ -211,19 +251,24 @@ __global__ void __launch_bounds__(kThreads) k_weibull(P scale, P conc, float* __
 
 // Beta: Ga / (Ga + Gb) from two standard Gamma draws on disjoint sub-counters, as 1 / (1 + exp(log Gb - log Ga)) so that
 // neither draw underflows; clamped to [tiny, 1 - eps] as torch's Dirichlet sampler clamps; then low + u (high - low)
+__device__ __forceinline__ float beta_draw(float a, float b, float lo, float hi, uint64_t seed, uint64_t idx,
+                                           uint64_t offset) {
+  float v = NAN;
+  if (a > 0.0f && b > 0.0f) {
+    const float la = std_gamma_log(a, seed, idx, offset, 0);
+    const float lb = std_gamma_log(b, seed, idx, offset, kGammaCalls + 1);
+    const float u = fminf(fmaxf(1.0f / (1.0f + expf(lb - la)), PPB_FLT_TINY), 1.0f - PPB_EPS32);
+    v = lo + u * (hi - lo);
+  }
+  return v;
+}
+
 __global__ void __launch_bounds__(kThreads) k_beta(P c1, P c0, P low, P high, float* __restrict__ out,
                                                     float* __restrict__ lp, int64_t n, uint64_t seed, uint64_t offset,
                                                     int64_t first) {
   PPB_GRID_LOOP(i) {
-    const uint64_t idx = (uint64_t)(first + i);
     const float a = c1.at(i), b = c0.at(i), lo = low.at(i), hi = high.at(i);
-    float v = NAN;
-    if (a > 0.0f && b > 0.0f) {
-      const float la = std_gamma_log(a, seed, idx, offset, 0);
-      const float lb = std_gamma_log(b, seed, idx, offset, kGammaCalls + 1);
-      const float u = fminf(fmaxf(1.0f / (1.0f + expf(lb - la)), PPB_FLT_TINY), 1.0f - PPB_EPS32);
-      v = lo + u * (hi - lo);
-    }
+    const float v = beta_draw(a, b, lo, hi, seed, (uint64_t)(first + i), offset);
     out[i] = v;
     if (lp) lp[i] = fam::beta_lp(v, a, b, lo, hi, fam::beta_const(a, b));
   }
@@ -298,6 +343,36 @@ __global__ void __launch_bounds__(kThreads) k_binomial(P count, P probs, float* 
 // The acceptance rate falls with kappa towards 0.658, so all kVonMisesCalls = 32 rounds fail with probability below
 // 0.343^32 < 1e-14 per draw; the draw then falls back to loc, deterministically.
 constexpr uint64_t kVonMisesCalls = 32;
+// k_von_mises's draw (see normal_draw)
+__device__ __forceinline__ float von_mises_draw(float locf, float kf, uint64_t seed, uint64_t idx, uint64_t offset) {
+  const double kPi = 3.14159265358979323846;
+  float v = NAN;
+  if (kf > 0.0f) {
+    const double kappa = kf;
+    const double tau = 1.0 + sqrt(1.0 + 4.0 * kappa * kappa);
+    const double rho = (tau - sqrt(2.0 * tau)) / (2.0 * kappa);
+    const double pr = (kappa < 1e-5) ? 1.0 / kappa + kappa : (1.0 + rho * rho) / (2.0 * rho);
+    double x = 0.0;
+    for (uint64_t call = 0; call < kVonMisesCalls; ++call) {
+      const ppb_philox r = philox_sub(seed, idx, offset, call);
+      const double u1 = ppb_u01(r.c[0]), u2 = ppb_u01(r.c[1]), u3 = ppb_u01(r.c[2]);
+      const double z = cospi(u1);
+      const double f = fmin(fmax((1.0 + pr * z) / (pr + z), -1.0), 1.0);
+      const double c = kappa * (pr - f);
+      if (c * (2.0 - c) - u2 > 0.0 || log(c / u2) + 1.0 - c >= 0.0) {
+        x = (u3 > 0.5 ? 1.0 : u3 < 0.5 ? -1.0 : 0.0) * acos(f);
+        break;
+      }
+    }
+    const double y = x + kPi + (double)locf, two_pi = 2.0 * kPi;
+    v = (float)(y - two_pi * floor(y / two_pi) - kPi);
+  }
+  return v;
+}
+
+// The draw below is repeated in von_mises_draw (the event sampler's): change both together.  It stays spelled out here so
+// that this kernel's SASS is what it was before the event sampler existed; the test that element 0 of an event row is
+// this kernel's draw bit for bit ties the two.
 __global__ void __launch_bounds__(kThreads) k_von_mises(P loc, P conc, float* __restrict__ out, float* __restrict__ lp,
                                                          int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
   const double kPi = 3.14159265358979323846;
@@ -394,6 +469,47 @@ __global__ void __launch_bounds__(kThreads) k_mixture(const float* __restrict__ 
       for (int j = 0; j < K; ++j) acc += expf(t[j] - mx);
       lp[i] = (mx == -INFINITY) ? -INFINITY : mx + logf(acc);
     }
+  }
+}
+
+// ---- event sampler: [n, D] draws ------------------------------------------------------------------------------------------
+// Philox counter layout.  Element j of particle i (global index g = first + i) draws from idx = g | (j << 40), with the
+// family's rejection rounds in offset + (round << 40) as above:
+//   * idx bits 0 .. 39 hold the particle (g < 2^40) and bits 40 .. 63 the element (j < 2^24), so no (particle, element)
+//     pair shares idx, and the rounds of one pair differ in offset: no (particle, element, round) triple shares a counter;
+//   * element 0 has idx = g, the per-particle samplers' counter, so it is their draw bit for bit;
+//   * the counter depends on the global index only, so a shard [a, b) of the particles draws the full run's rows.
+// ppb_event_sample rejects D > 2^24 and first_index + n > 2^40 before launch.
+struct EvP {
+  const float* p;
+  int64_t ps, es;
+  __device__ __forceinline__ float at(int64_t i, int64_t j) const { return p ? __ldg(p + i * ps + j * es) : 0.0f; }
+};
+
+template <int FAMILY>
+__global__ void __launch_bounds__(kThreads) k_event_sample(EvP p0, EvP p1, EvP p2, EvP p3, float* __restrict__ out,
+                                                            int64_t n, int64_t D, uint64_t seed, uint64_t offset,
+                                                            int64_t first) {
+  const int64_t total = n * D;
+  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t i = e / D, j = e - i * D;
+    const uint64_t idx = (uint64_t)(first + i) | ((uint64_t)j << 40);
+    const float a = p0.at(i, j), b = p1.at(i, j);
+    float v;
+    switch (FAMILY) {
+      case PPB_EVENT_NORMAL: v = normal_draw(ppb_philox4x32_10(seed, idx, offset), a, b); break;
+      case PPB_EVENT_UNIFORM: v = uniform_draw(ppb_philox4x32_10(seed, idx, offset), a, b); break;
+      case PPB_EVENT_POISSON: v = poisson_draw(a, seed, idx, offset); break;
+      case PPB_EVENT_BERNOULLI: v = bernoulli_one(ppb_philox4x32_10(seed, idx, offset), a) ? 1.0f : 0.0f; break;
+      case PPB_EVENT_EXPONENTIAL: v = exponential_draw(ppb_philox4x32_10(seed, idx, offset), a); break;
+      case PPB_EVENT_GAMMA: v = gamma_draw(a, b, seed, idx, offset); break;
+      case PPB_EVENT_LOGNORMAL: v = lognormal_draw(ppb_philox4x32_10(seed, idx, offset), a, b); break;
+      case PPB_EVENT_WEIBULL: v = weibull_draw(ppb_philox4x32_10(seed, idx, offset), a, b); break;
+      case PPB_EVENT_BETA: v = beta_draw(a, b, p2.at(i, j), p3.at(i, j), seed, idx, offset); break;
+      case PPB_EVENT_BINOMIAL: v = binomial_draw(a, b, seed, idx, offset); break;
+      default: v = von_mises_draw(a, b, seed, idx, offset); break;
+    }
+    out[e] = v;
   }
 }
 
@@ -550,6 +666,56 @@ int ppb_mixture_truncated_normal_sample(const float* means, const float* stddevs
       offset, first_index);
   PPB_LAUNCH_CHECK();
   return PPB_OK;
+}
+
+int ppb_event_sample(int family, const float* p0, int64_t p0_ps, int64_t p0_es, const float* p1, int64_t p1_ps,
+                     int64_t p1_es, const float* p2, int64_t p2_ps, int64_t p2_es, const float* p3, int64_t p3_ps,
+                     int64_t p3_es, float* value_out, float* lp_out, int64_t n, int64_t D, uint64_t seed,
+                     uint64_t offset, int64_t first_index, void* stream) {
+  const int np = ppb_event_num_params(family);
+  PPB_CHECK_ARG(np > 0, "unknown family id");
+  PPB_CHECK_ARG(n >= 0 && D > 0 && value_out, "n must be >= 0, D > 0 and value_out non-null");
+  PPB_CHECK_ARG(D <= ((int64_t)1 << 24), "D > 2^24: the element index does not fit Philox counter bits 40 .. 63");
+  PPB_CHECK_ARG(first_index >= 0 && first_index + n <= ((int64_t)1 << 40),
+                "first_index + n > 2^40: the particle index does not fit Philox counter bits 0 .. 39");
+  const float* p[4] = {p0, p1, p2, p3};
+  const int64_t ps[4] = {p0_ps, p1_ps, p2_ps, p3_ps}, es[4] = {p0_es, p1_es, p2_es, p3_es};
+  EvP q[4];
+  for (int k = 0; k < 4; ++k) {
+    if (k < np) {
+      PPB_CHECK_ARG(p[k] && ((ps[k] == 0 && es[k] == 0) || (ps[k] == 1 && es[k] == 0) || (ps[k] == 0 && es[k] == 1) ||
+                             (ps[k] == D && es[k] == 1)),
+                    "parameter: null pointer, or strides not one of (0, 0), (1, 0), (0, 1), (D, 1)");
+      q[k] = EvP{p[k], ps[k], es[k]};
+    } else {
+      q[k] = EvP{nullptr, 0, 0};
+    }
+  }
+  if (n == 0) return PPB_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int grid = ppb_grid_for(n * D, kThreads, 1);
+#define PPB_EVENT_CASE(F)                                                                                       \
+  case F:                                                                                                       \
+    k_event_sample<F><<<grid, kThreads, 0, st>>>(q[0], q[1], q[2], q[3], value_out, n, D, seed, offset, first_index); \
+    break;
+  switch (family) {
+    PPB_EVENT_CASE(PPB_EVENT_NORMAL)
+    PPB_EVENT_CASE(PPB_EVENT_UNIFORM)
+    PPB_EVENT_CASE(PPB_EVENT_POISSON)
+    PPB_EVENT_CASE(PPB_EVENT_BERNOULLI)
+    PPB_EVENT_CASE(PPB_EVENT_EXPONENTIAL)
+    PPB_EVENT_CASE(PPB_EVENT_GAMMA)
+    PPB_EVENT_CASE(PPB_EVENT_LOGNORMAL)
+    PPB_EVENT_CASE(PPB_EVENT_WEIBULL)
+    PPB_EVENT_CASE(PPB_EVENT_BETA)
+    PPB_EVENT_CASE(PPB_EVENT_BINOMIAL)
+    default: PPB_EVENT_CASE(PPB_EVENT_VON_MISES)
+  }
+#undef PPB_EVENT_CASE
+  PPB_LAUNCH_CHECK();
+  if (!lp_out) return PPB_OK;
+  // lp_out: the scoring kernel's row sums over the drawn rows (value operand (D, 1))
+  return ppb_event_score(family, value_out, D, 1, p, ps, es, n, D, nullptr, lp_out, nullptr, 0.0, stream);
 }
 
 }  // extern "C"

@@ -3,6 +3,8 @@
 // Algorithmic bytes per element (SURVEY §8d): Normal/Uniform 16 B, Poisson/Bernoulli 12 B, Categorical 4C+12 B,
 // Mixture-Normal (3K+2)*4 B, Mixture-TruncatedNormal (3K+4)*4 B; Exponential 12 B, Gamma/LogNormal/Weibull/Binomial/
 // VonMises 16 B, Beta 24 B with per-particle parameters (value + lp_out + 4 B per per-particle parameter).
+// Event sites (k_event, pyprob/state.py:147 with a tensor value): 4 B per element of each per-particle-event operand, a
+// shared event row once, 16 B per particle for the fp64 accumulator (+ 4 B per element for lp_out).
 #include "common.cuh"
 #include "families.cuh"
 
@@ -354,9 +356,223 @@ int launch_mixture(const float* value, const float* means, const float* stddevs,
   return PPB_OK;
 }
 
+// ---- event-shaped sites: sum_j log p(v_ij) per particle ----------------------------------------------------------------
+// One kernel template over the Ops above for every family with an element-wise log_prob.  An operand is (pointer,
+// particle stride ps, element stride es): element j of particle i is p[i ps + j es], with (ps, es) one of (0, 0) scalar,
+// (1, 0) one per particle, (0, 1) shared event, (D, 1) event per particle.
+// Thread mapping: G lanes (a power of two, 1 .. 32) share a row; lane l of a group owns the 4-element chunks
+// l, l + G, l + 2G, ... of the row, and G is the smallest power of two >= ceil(D / 4) (capped at 32), so small D puts
+// several rows in a warp and large D a warp on each row.  A chunk is one 128-bit load where its address is 16-byte
+// aligned (every chunk of an aligned row; D is generally not a multiple of 4, so which rows are aligned depends on i) and
+// four 32-bit loads elsewhere.  Per-particle rows stream past L1; a shared event row is read through L1 / L2.
+// Each lane sums its elements in fp64 in element order, and the group combines its lanes with a fixed butterfly: the
+// order depends on (n, D) only (G is a function of D; the load width does not change what is summed), so a call is
+// bit-reproducible, and with D = 1 the sum is the single term, exactly k_score2's accumulator update.
+struct EvOperand {
+  const float* p;
+  int64_t ps, es;
+  // elements j0 .. j0 + 3 of row i (elements at or past D read as 0 and are never used)
+  __device__ __forceinline__ void load4(int64_t i, int64_t j0, int64_t D, float (&o)[4]) const {
+    const float* r = p + i * ps;
+    if (es == 0) {
+      const float s = __ldg(r);
+      o[0] = o[1] = o[2] = o[3] = s;
+      return;
+    }
+    r += j0;
+    if (j0 + 4 <= D && aligned16(r)) {
+      const float4 v = ps ? ldg_stream4(r) : __ldg(reinterpret_cast<const float4*>(r));
+      o[0] = v.x; o[1] = v.y; o[2] = v.z; o[3] = v.w;
+    } else {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) o[k] = (j0 + k < D) ? __ldg(r + k) : 0.0f;
+    }
+  }
+};
+
+struct EvArgs {
+  EvOperand v, p[4];
+  float* lp;       // nullable [n, D] element-wise log-densities
+  float* row_lp;   // nullable [n] fp32 row sums (the samplers' lp_out)
+  double* acc;     // nullable [n] acc[i] += scale * row sum
+  double scale;
+  int64_t n, D;
+};
+
+// (value, parameter vector) -> log-density, over the two-parameter Ops (one-parameter families ignore p[1])
+template <class Op>
+struct EvFamily {
+  static constexpr bool kTable = Op::kTable;
+  Op op;
+  __device__ __forceinline__ float operator()(float v, const float (&p)[4], const float* tab) {
+    return op(v, p[0], p[1], tab);
+  }
+};
+struct EvBeta {
+  static constexpr bool kTable = false;
+  float a_ = NAN, b_ = NAN, k_ = NAN;
+  __device__ __forceinline__ float operator()(float v, const float (&p)[4], const float*) {
+    if (!(p[0] == a_ && p[1] == b_)) { a_ = p[0]; b_ = p[1]; k_ = fam::beta_const(p[0], p[1]); }
+    return fam::beta_lp(v, p[0], p[1], p[2], p[3], k_);
+  }
+};
+
+template <class F, int NP, int G>
+__global__ void __launch_bounds__(kThreads) k_event(EvArgs a, F f) {
+  __shared__ float tab[F::kTable ? 64 : 1];
+  if (F::kTable) {
+    if (threadIdx.x < 64) tab[threadIdx.x] = c_log_factorial[threadIdx.x];
+    __syncthreads();
+  }
+  constexpr int kRowsPerWarp = 32 / G;
+  const int lane = threadIdx.x & 31, sub = lane % G;
+  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  const int64_t D = a.D, chunks = (D + 3) >> 2;
+  for (int64_t base = warp * kRowsPerWarp; base < a.n; base += nwarps * kRowsPerWarp) {   // warp-uniform
+    const int64_t i = base + lane / G;
+    double s = 0.0;
+    if (i < a.n) {
+      for (int64_t c = sub; c < chunks; c += G) {
+        const int64_t j0 = c << 2;
+        float v[4], p[NP][4], r[4];
+        a.v.load4(i, j0, D, v);
+#pragma unroll
+        for (int k = 0; k < NP; ++k) a.p[k].load4(i, j0, D, p[k]);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          float pe[4];
+#pragma unroll
+          for (int k = 0; k < 4; ++k) pe[k] = p[k < NP ? k : 0][e];
+          r[e] = f(v[e], pe, tab);
+        }
+        const int m = (D - j0 < 4) ? (int)(D - j0) : 4;
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+          if (e < m) s += (double)r[e];
+        if (a.lp) {
+          float* o = a.lp + i * D + j0;
+          if (m == 4 && aligned16(o)) {
+            *reinterpret_cast<float4*>(o) = make_float4(r[0], r[1], r[2], r[3]);
+          } else {
+#pragma unroll
+            for (int e = 0; e < 4; ++e)
+              if (e < m) o[e] = r[e];
+          }
+        }
+      }
+    }
+#pragma unroll
+    for (int o = G / 2; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (i < a.n && sub == 0) {
+      if (a.acc) a.acc[i] += a.scale * s;
+      if (a.row_lp) a.row_lp[i] = (float)s;
+    }
+  }
+}
+
+template <class F, int NP>
+int launch_event(const EvArgs& a, cudaStream_t st, F f) {
+  const int64_t chunks = (a.D + 3) >> 2;
+  int g = 1;
+  while (g < chunks && g < 32) g <<= 1;
+  const int grid = ppb_grid_for(a.n, kThreads / g, 1);
+  switch (g) {
+    case 1: k_event<F, NP, 1><<<grid, kThreads, 0, st>>>(a, f); break;
+    case 2: k_event<F, NP, 2><<<grid, kThreads, 0, st>>>(a, f); break;
+    case 4: k_event<F, NP, 4><<<grid, kThreads, 0, st>>>(a, f); break;
+    case 8: k_event<F, NP, 8><<<grid, kThreads, 0, st>>>(a, f); break;
+    case 16: k_event<F, NP, 16><<<grid, kThreads, 0, st>>>(a, f); break;
+    default: k_event<F, NP, 32><<<grid, kThreads, 0, st>>>(a, f); break;
+  }
+  PPB_LAUNCH_CHECK();
+  return PPB_OK;
+}
+
+// c_log_factorial, uploaded once per process by the first Poisson log_prob call (per-particle or event)
+int upload_log_factorial() {
+  static bool table_ready = false;
+  if (!table_ready) {
+    float t[64];
+    for (int k = 0; k < 64; ++k) t[k] = (float)lgamma((double)k + 1.0);
+    PPB_CUDA(cudaMemcpyToSymbol(c_log_factorial, t, sizeof(t)));
+    table_ready = true;
+  }
+  return PPB_OK;
+}
+
+bool ev_layout_ok(const void* p, int64_t ps, int64_t es, int64_t D) {
+  return p && ((ps == 0 && es == 0) || (ps == 1 && es == 0) || (ps == 0 && es == 1) || (ps == D && es == 1));
+}
+
 }  // namespace
 
+int ppb_event_num_params(int family) {
+  switch (family) {
+    case PPB_EVENT_POISSON: case PPB_EVENT_BERNOULLI: case PPB_EVENT_EXPONENTIAL: return 1;
+    case PPB_EVENT_BETA: return 4;
+    case PPB_EVENT_NORMAL: case PPB_EVENT_UNIFORM: case PPB_EVENT_GAMMA: case PPB_EVENT_LOGNORMAL:
+    case PPB_EVENT_WEIBULL: case PPB_EVENT_BINOMIAL: case PPB_EVENT_VON_MISES: return 2;
+    default: return -1;
+  }
+}
+
+int ppb_event_score(int family, const float* value, int64_t value_ps, int64_t value_es, const float* const* params,
+                    const int64_t* params_ps, const int64_t* params_es, int64_t n, int64_t D, float* lp_out,
+                    float* row_lp, double* acc, double acc_scale, void* stream) {
+  const int np = ppb_event_num_params(family);
+  PPB_CHECK_ARG(np > 0, "unknown family id");
+  PPB_CHECK_ARG(n >= 0 && D > 0, "n must be >= 0 and D > 0");
+  PPB_CHECK_ARG(ev_layout_ok(value, value_ps, value_es, D),
+                "value: null pointer, or strides not one of (0, 0), (1, 0), (0, 1), (D, 1)");
+  EvArgs a;
+  a.v = EvOperand{value, value_ps, value_es};
+  for (int k = 0; k < 4; ++k) {
+    if (k < np) {
+      PPB_CHECK_ARG(ev_layout_ok(params[k], params_ps[k], params_es[k], D),
+                    "parameter: null pointer, or strides not one of (0, 0), (1, 0), (0, 1), (D, 1)");
+      a.p[k] = EvOperand{params[k], params_ps[k], params_es[k]};
+    } else {
+      a.p[k] = EvOperand{nullptr, 0, 0};
+    }
+  }
+  if (n == 0) return PPB_OK;
+  a.lp = lp_out;
+  a.row_lp = row_lp;
+  a.acc = acc;
+  a.scale = acc_scale;
+  a.n = n;
+  a.D = D;
+  cudaStream_t st = (cudaStream_t)stream;
+  switch (family) {
+    case PPB_EVENT_NORMAL: return launch_event<EvFamily<NormalOp>, 2>(a, st, {});
+    case PPB_EVENT_UNIFORM: return launch_event<EvFamily<UniformOp>, 2>(a, st, {});
+    case PPB_EVENT_POISSON: {
+      const int e = upload_log_factorial();
+      if (e != PPB_OK) return e;
+      return launch_event<EvFamily<PoissonOp>, 1>(a, st, {});
+    }
+    case PPB_EVENT_BERNOULLI: return launch_event<EvFamily<BernoulliOp>, 1>(a, st, {});
+    case PPB_EVENT_EXPONENTIAL: return launch_event<EvFamily<ExponentialOp>, 1>(a, st, {});
+    case PPB_EVENT_GAMMA: return launch_event<EvFamily<GammaOp>, 2>(a, st, {});
+    case PPB_EVENT_LOGNORMAL: return launch_event<EvFamily<LogNormalOp>, 2>(a, st, {});
+    case PPB_EVENT_WEIBULL: return launch_event<EvFamily<WeibullOp>, 2>(a, st, {});
+    case PPB_EVENT_BETA: return launch_event<EvBeta, 4>(a, st, {});
+    case PPB_EVENT_BINOMIAL: return launch_event<EvFamily<BinomialOp>, 2>(a, st, {});
+    default: return launch_event<EvFamily<VonMisesOp>, 2>(a, st, {});
+  }
+}
+
 extern "C" {
+
+int ppb_event_log_prob(int family, const float* value, int64_t value_ps, int64_t value_es, const float* p0,
+                       int64_t p0_ps, int64_t p0_es, const float* p1, int64_t p1_ps, int64_t p1_es, const float* p2,
+                       int64_t p2_ps, int64_t p2_es, const float* p3, int64_t p3_ps, int64_t p3_es, int64_t n,
+                       int64_t D, float* lp_out, double* acc, double acc_scale, void* stream) {
+  const float* p[4] = {p0, p1, p2, p3};
+  const int64_t ps[4] = {p0_ps, p1_ps, p2_ps, p3_ps}, es[4] = {p0_es, p1_es, p2_es, p3_es};
+  return ppb_event_score(family, value, value_ps, value_es, p, ps, es, n, D, lp_out, nullptr, acc, acc_scale, stream);
+}
 
 int ppb_normal_log_prob(const float* value, const float* mean, int mean_stride, const float* stddev,
                         int stddev_stride, float* lp_out, double* acc, double acc_scale, int64_t n, void* stream) {
@@ -381,13 +597,8 @@ int ppb_poisson_log_prob(const float* value, const float* rate, int rate_stride,
   if (n == 0) return PPB_OK;
   PPB_CHECK_ARG(n >= 0 && value && rate, "null pointer or negative n");
   PPB_CHECK_ARG((rate_stride | 1) == 1, "strides must be 0 or 1");
-  static bool table_ready = false;
-  if (!table_ready) {
-    float t[64];
-    for (int k = 0; k < 64; ++k) t[k] = (float)lgamma((double)k + 1.0);
-    PPB_CUDA(cudaMemcpyToSymbol(c_log_factorial, t, sizeof(t)));
-    table_ready = true;
-  }
+  const int e = upload_log_factorial();
+  if (e != PPB_OK) return e;
   return launch_score2(value, Param{rate, rate_stride}, Param{rate, 0}, Sink{lp_out, acc, acc_scale}, n, stream,
                        PoissonOp{});
 }

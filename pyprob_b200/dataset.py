@@ -52,10 +52,9 @@ class TraceBatch:
 
         def param(p):
             return push(p if torch.is_tensor(p) else torch.full((n,), float(p), device='cuda'))
-        obs_cols = []
-        for name in net._observe_names:
-            v = self.trace.named_variables[name].value
-            obs_cols.append(push(v))
+        # observables: D columns each (an event-shaped observable's [n, *E] value, flattened), in _observe_names order
+        obs_mat = torch.cat([self.trace.named_variables[name].value.reshape(n, -1).float()
+                             for name in net._observe_names], dim=1)
         for sites, idx in self.groups:
             ids, vc, p0c, p1c = [], [], [], []
             for s in sites:
@@ -72,7 +71,8 @@ class TraceBatch:
                 else:
                     p0c.append(-1); p1c.append(-1)
             plan.append((ids, vc, p0c, p1c, idx))
-        host = torch.stack(cols, dim=0).cpu().numpy()  # one device->host copy for the whole batch
+        ncols = len(cols)
+        host = torch.cat([torch.stack(cols, dim=0), obs_mat.t()], dim=0).cpu().numpy()  # one device->host copy
         zeros = np.zeros(n, dtype=np.float32)
         subs = []
         for ids, vc, p0c, p1c, idx in plan:
@@ -80,7 +80,7 @@ class TraceBatch:
 
             def rows(cs):
                 return np.stack([(zeros if c < 0 else host[c])[sel] for c in cs], axis=0)
-            obs = np.stack([host[c][sel] for c in obs_cols], axis=1)
+            obs = np.ascontiguousarray(host[ncols:, sel].T)
             subs.append(SubBatch(ids, rows(vc), rows(p0c), rows(p1c), obs))
         self._encoded = EncodedBatch(subs, row_align=net.row_align)
         return self._encoded

@@ -4,6 +4,20 @@ Public protocol follows the reference (pyprob/distributions/distribution.py:9-95
 ``_address_suffix``, ``sample()``, ``log_prob(value, sum=False)``, ``mean/stddev/variance``.  Parameters may
 be Python scalars (shared by all particles) or length-n CUDA tensors (one per particle).  There is no CPU
 path: every sample/log_prob is a kernel launch over the particle axis.
+
+Event shapes (observations only).  A site over n particles has an event shape E (D = prod(E) elements) formed as torch's
+``log_prob`` broadcasts the value against the parameters:
+  * a parameter that is a Python scalar or a 1-D [n] tensor keeps its meaning (shared, one per particle), and so does
+    an [n, 1, ...] tensor of n elements (``w.view(-1, 1)``); a tensor with at least 2 dims and leading size n is one
+    event per particle, [n, *E]; [1, *E] or any other shape (a 1-D tensor of another length included) is one event
+    shared by all particles.  A parameter that only broadcasts to E (a [28, 1] against a [28, 28] value) is expanded;
+  * an observed value is data, the same for every particle: a scalar, or a 1-D [n] tensor under a distribution whose
+    parameters have no event shape, keeps today's per-particle meaning; any other shape is one shared event.  So a
+    shared 1-D event of length n must be passed as [1, n];
+  * parameters and value that do not broadcast raise ValueError.
+The site's weight term is likelihood_importance * sum_j log p(v_j), the reference's log_prob(value, sum=True) for one
+particle (pyprob/state.py:147); ``log_prob(value)`` returns the element-wise [n, *E] values and ``sample(n)`` draws
+[n, *E].  Categorical, Mixture and TruncatedNormal have no event form (NotImplementedError).
 """
 import math
 
@@ -25,6 +39,148 @@ def _as_param(x):
     return float(x)
 
 
+def _params(*xs):
+    """-> (parameters as _as_param gives them, parameters with their shape kept (for event sites))"""
+    shaped = []
+    for x in xs:
+        if torch.is_tensor(x) and x.numel() > 1 and x.dim() >= 2:
+            shaped.append(x.to(device='cuda', dtype=torch.float32))
+        else:
+            shaped.append(_as_param(x))
+    return tuple(p.reshape(-1) if torch.is_tensor(p) else p for p in shaped), tuple(shaped)
+
+
+class EventSite:
+    """A site with an event shape, resolved against n particles: event operands for ops.event_log_prob /
+    ops.event_sample ([n, 1] per particle, [1, D] shared event, [n, D] event per particle, or a scalar)."""
+
+    def __init__(self, family, shape, n, params, value=None):
+        self.family, self.shape, self.n = family, tuple(shape), int(n)
+        self.D = int(math.prod(self.shape))
+        self.params, self.value = params, value
+
+    @property
+    def site_value(self):
+        """The observed value as the trace holds it: an [n, *E] view of the one shared row (row stride 0, no copy)."""
+        v = self.value
+        if not torch.is_tensor(v):
+            v = torch.full((1,), float(v), device='cuda')
+        return (v.reshape(1) if v.numel() == 1 else v.reshape(self.shape)).expand(self.n, *self.shape)
+
+    def score_into(self, acc, scale):
+        ops.event_log_prob(self.family, self.value, self.params, self.n, self.D, acc=acc, acc_scale=scale)
+
+    def log_prob(self):
+        return ops.event_log_prob(self.family, self.value, self.params, self.n, self.D).view(self.n, *self.shape)
+
+    def sample(self, with_log_prob=False):
+        s, o, f = util._seed, util.next_draw_offset(), _shard_first_index
+        out = ops.event_sample(self.family, self.params, self.n, self.D, s, o, f, with_log_prob)
+        if with_log_prob:
+            return out[0].view(self.n, *self.shape), out[1]
+        return out.view(self.n, *self.shape)
+
+
+_NO_VALUE = object()
+_REFERENCE_NOTE = ('(the reference scores and draws such sites with torch, pyprob/state.py:118-219; pyprob_b200 supports '
+                   'tensor-valued observations of the families with an element-wise log_prob)')
+
+
+def _broadcast_events(shapes):
+    try:
+        return tuple(torch.broadcast_shapes(*shapes))
+    except RuntimeError as e:
+        raise ValueError('event shapes do not broadcast: {} ({})'.format(
+            ', '.join(str(tuple(s)) for s in shapes), e)) from None
+
+
+def _param_form(p, n):
+    """(kind, event shape) of a parameter over n particles: a scalar; one per particle (a 1-D [n] tensor, or [n, 1, ...]);
+    one event per particle ([n, *E], at least 2 dims); or one shared event ([1, *E], or any other shape)."""
+    if not torch.is_tensor(p):
+        return 'scalar', ()
+    if p.dim() >= 1 and p.size(0) == n and p.numel() == n:
+        return 'particle', ()
+    if p.dim() <= 1:
+        return 'event', tuple(p.shape)
+    if p.size(0) == n:
+        return 'particle_event', tuple(p.shape[1:])
+    if p.size(0) == 1:
+        return 'event', tuple(p.shape[1:])
+    return 'event', tuple(p.shape)
+
+
+def _event_layout(shaped, n, value=_NO_VALUE, per_particle_value=False):
+    """The shape rules (module docstring), host-side only: -> None when the site is scalar (today's path), else
+    (E, [(kind, event shape)] per parameter, value form, value), kind / form one of 'scalar', 'particle',
+    'particle_event', 'event' (shared)."""
+    param_event = any(_param_form(p, n)[0] == 'event' or _param_form(p, n)[0] == 'particle_event' for p in shaped)
+    if value is _NO_VALUE or value is None:
+        vform = None
+    elif isinstance(value, (int, float)):
+        vform = 'scalar'
+    else:
+        if not torch.is_tensor(value):
+            value = torch.as_tensor(value, dtype=torch.float32)
+        if value.numel() == 1:
+            vform = 'scalar'
+        elif per_particle_value and value.dim() >= 2 and value.size(0) == n:
+            vform = 'particle_event'
+        elif value.dim() <= 1 and value.numel() == n and not param_event:
+            return None
+        else:
+            vform = 'event'
+    if not param_event and vform in (None, 'scalar'):
+        return None
+    forms = [_param_form(p, n) for p in shaped]
+    shapes = [e for _, e in forms]
+    if vform in ('event', 'particle_event'):
+        shapes.append(tuple(value.shape[1:]) if vform == 'particle_event' else tuple(value.shape))
+    E = _broadcast_events(shapes)
+    if math.prod(E) <= 1 and vform in (None, 'scalar'):
+        return None                     # [n, 1, ...] parameters: one value per particle, today's path
+    return E, forms, vform, value
+
+
+def _resolve_event(dist, n, value=_NO_VALUE, per_particle_value=False):
+    """The EventSite of `dist` over n particles observing `value`, or None when the site is scalar (today's path)."""
+    shaped = dist._shaped
+    layout = _event_layout(shaped, n, value, per_particle_value)
+    if layout is None:
+        return None
+    E, forms, vform, value = layout
+    D = math.prod(E)
+    family = ops.EVENT_FAMILIES.get(dist.name)
+    if family is None:
+        raise NotImplementedError('{} has no event-shaped form in pyprob_b200 (event shape {}) {}'.format(
+            dist.name, E, _REFERENCE_NOTE))
+
+    def particle_rows(t, e):
+        t = t.reshape(n, *([1] * (len(E) - len(e))), *e)
+        return t.expand(n, *E).reshape(n, D)
+
+    def shared_row(t, e):
+        return t.reshape(e).expand(E).reshape(1, D)
+    params = []
+    for p, (kind, e) in zip(shaped, forms):
+        if kind == 'scalar':
+            params.append(p)
+        elif kind == 'particle':
+            params.append(p.reshape(n, 1))
+        elif kind == 'particle_event':
+            params.append(particle_rows(p, e))
+        else:
+            params.append(shared_row(p, e))
+    if vform is None:
+        v = None
+    elif vform == 'scalar':
+        v = float(value) if not torch.is_tensor(value) else value.to(device='cuda', dtype=torch.float32).reshape(1)
+    else:
+        t = value.to(device='cuda', dtype=torch.float32)
+        v = particle_rows(t, tuple(t.shape[1:])) if vform == 'particle_event' else shared_row(t, tuple(t.shape))
+    return EventSite(family, E, n, params, v)
+
+
 def _length(*params):
     n = 1
     for p in params:
@@ -43,6 +199,8 @@ def _value(v, n=None):
 
 
 class Distribution:
+    _shaped = ()   # the parameters with their shapes (event sites); empty for the families without an event form
+
     def __init__(self, name, address_suffix):
         self.name = name
         self._address_suffix = address_suffix
@@ -54,12 +212,47 @@ class Distribution:
     def _draw(self, n, with_log_prob):
         raise NotImplementedError()
 
+    def _has_event_param(self):
+        """A parameter of at least 2 dims that is not one column of values ([n, 1, ...])."""
+        return any(torch.is_tensor(p) and p.dim() >= 2 and p.numel() != p.size(0) for p in self._shaped)
+
+    def _standalone_n(self):
+        """Particles of a call outside a trace: the length of the one-per-particle parameters (1-D, or [n, 1, ...]);
+        event parameters do not count."""
+        if self._has_event_param():
+            return max([p.size(0) for p in self._shaped if torch.is_tensor(p) and p.numel() == p.size(0)] + [1])
+        return self.batch_length
+
+    def event_site(self, n, value=_NO_VALUE):
+        """The EventSite of this distribution over n particles observing `value` (a data value, shared by every
+        particle), or None when the site is scalar.  Raises ValueError when the shapes do not broadcast and
+        NotImplementedError for a family without an event form."""
+        if not self._shaped:
+            if value is not _NO_VALUE and value is not None and not isinstance(value, (int, float)):
+                v = value if torch.is_tensor(value) else torch.as_tensor(value)
+                if v.numel() > 1 and not (v.dim() <= 1 and v.numel() == n):
+                    raise NotImplementedError('{} observations with an event shape {} {}'.format(
+                        self.name, tuple(v.shape), _REFERENCE_NOTE))
+            return None
+        return _resolve_event(self, n, value)
+
     def sample(self, n=None, with_log_prob=False):
-        n = self.batch_length if n is None else n
+        n = self._standalone_n() if n is None else n
+        if self._shaped:
+            ev = _resolve_event(self, n)
+            if ev is not None:
+                return ev.sample(with_log_prob)
         return self._draw(n, with_log_prob)
 
     def log_prob(self, value, sum=False):
-        lp = self._log_prob(value)
+        ev = None
+        if self._has_event_param() and torch.is_tensor(value) and value.numel() > 1:
+            # without an event parameter, log_prob is today's element-wise [N] kernel call
+            n = self._standalone_n()
+            if value.dim() >= 2 and n == 1:
+                n = value.size(0)
+            ev = _resolve_event(self, n, value, per_particle_value=True)
+        lp = ev.log_prob() if ev is not None else self._log_prob(value)
         return lp.sum() if sum else lp
 
     def prob(self, value):
@@ -76,7 +269,7 @@ class Distribution:
 class Normal(Distribution):
     def __init__(self, loc, scale):
         super().__init__('Normal', 'Normal')
-        self.loc, self.scale = _as_param(loc), _as_param(scale)
+        (self.loc, self.scale), self._shaped = _params(loc, scale)
 
     @property
     def batch_length(self):
@@ -103,7 +296,7 @@ class Normal(Distribution):
 class Uniform(Distribution):
     def __init__(self, low, high):
         super().__init__('Uniform', 'Uniform')
-        self.low, self.high = _as_param(low), _as_param(high)
+        (self.low, self.high), self._shaped = _params(low, high)
 
     @property
     def batch_length(self):
@@ -129,7 +322,7 @@ class Uniform(Distribution):
 class Poisson(Distribution):
     def __init__(self, rate):
         super().__init__('Poisson', 'Poisson')
-        self.rate = _as_param(rate)
+        (self.rate,), self._shaped = _params(rate)
 
     @property
     def batch_length(self):
@@ -166,7 +359,7 @@ class Bernoulli(Distribution):
             if logits is None:
                 raise ValueError('Either probs or logits must be given.')
             probs = torch.sigmoid(torch.as_tensor(logits, dtype=torch.float32))
-        self.probs = _as_param(probs)
+        (self.probs,), self._shaped = _params(probs)
 
     @property
     def batch_length(self):
@@ -208,7 +401,7 @@ class Exponential(Distribution):
 
     def __init__(self, rate):
         super().__init__('Exponential', 'Exponential')
-        self.rate = _as_param(rate)
+        (self.rate,), self._shaped = _params(rate)
 
     @property
     def batch_length(self):
@@ -237,7 +430,7 @@ class Gamma(Distribution):
 
     def __init__(self, concentration, rate):
         super().__init__('Gamma', 'Gamma')
-        self.concentration, self.rate = _as_param(concentration), _as_param(rate)
+        (self.concentration, self.rate), self._shaped = _params(concentration, rate)
 
     @property
     def batch_length(self):
@@ -265,7 +458,7 @@ class LogNormal(Distribution):
 
     def __init__(self, loc, scale):
         super().__init__('LogNormal', 'LogNormal')
-        self.loc, self.scale = _as_param(loc), _as_param(scale)
+        (self.loc, self.scale), self._shaped = _params(loc, scale)
 
     @property
     def batch_length(self):
@@ -294,7 +487,7 @@ class Weibull(Distribution):
 
     def __init__(self, scale, concentration):
         super().__init__('Weibull', 'Weibull')
-        self.scale, self.concentration = _as_param(scale), _as_param(concentration)
+        (self.scale, self.concentration), self._shaped = _params(scale, concentration)
 
     @property
     def batch_length(self):
@@ -329,8 +522,8 @@ class Beta(Distribution):
 
     def __init__(self, concentration1, concentration0, low=0, high=1):
         super().__init__('Beta', 'Beta')
-        self.concentration1, self.concentration0 = _as_param(concentration1), _as_param(concentration0)
-        self.low, self.high = _as_param(low), _as_param(high)
+        (self.concentration1, self.concentration0, self.low, self.high), self._shaped = _params(
+            concentration1, concentration0, low, high)
 
     @property
     def batch_length(self):
@@ -381,7 +574,7 @@ class Binomial(Distribution):
             if logits is None:
                 raise ValueError('Either probs or logits must be given.')
             probs = torch.sigmoid(torch.as_tensor(logits, dtype=torch.float32))
-        self.total_count, self.probs = _as_param(total_count), _as_param(probs)
+        (self.total_count, self.probs), self._shaped = _params(total_count, probs)
 
     @property
     def batch_length(self):
@@ -415,7 +608,7 @@ class VonMises(Distribution):
 
     def __init__(self, loc, concentration):
         super().__init__('VonMises', 'VonMises')
-        self.loc, self.concentration = _as_param(loc), _as_param(concentration)
+        (self.loc, self.concentration), self._shaped = _params(loc, concentration)
 
     @property
     def batch_length(self):

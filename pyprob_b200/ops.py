@@ -286,6 +286,85 @@ def mixture_truncated_normal_sample(means, stddevs, probs, low, high, n, seed, o
     return (v, lp) if with_log_prob else v
 
 
+# ---- event-shaped sites (C-ABI section 2b): D elements per particle ---------------------------------------------------
+
+EVENT_FAMILIES = {'Normal': 0, 'Uniform': 1, 'Poisson': 2, 'Bernoulli': 3, 'Exponential': 4, 'Gamma': 5,
+                  'LogNormal': 6, 'Weibull': 7, 'Beta': 8, 'Binomial': 9, 'VonMises': 10}
+EVENT_NUM_PARAMS = {0: 2, 1: 2, 2: 1, 3: 1, 4: 1, 5: 2, 6: 2, 7: 2, 8: 4, 9: 2, 10: 2}
+EVENT_MAX_D = 1 << 24          # element index: Philox counter bits 40 .. 63
+EVENT_MAX_PARTICLES = 1 << 40  # particle index: Philox counter bits 0 .. 39
+
+
+def _event_operand(x, n, D, device):
+    """An operand of an event kernel -> (tensor kept alive, pointer, particle stride, element stride).
+
+    x is a python scalar or 1-element tensor (shared scalar: (0, 0)), or a 2-D tensor: [n, 1] one per particle (1, 0),
+    [1, D] or an [n, D] view with row stride 0 one shared event (0, 1), [n, D] one event per particle (D, 1)."""
+    if not torch.is_tensor(x) or x.numel() == 1:
+        t = _f32(x, device)
+        return t, ptr(t), 0, 0
+    t = x if (x.is_cuda and x.dtype == torch.float32) else x.to(device=device, dtype=torch.float32)
+    if t.dim() != 2:
+        raise ValueError('event operand must be a scalar or 2-D, got shape {}'.format(tuple(t.shape)))
+    r, c = t.shape
+    if c == 1 and r == n:
+        t = t.reshape(n).contiguous()
+        return t, ptr(t), 1, 0
+    if c != D or r not in (1, n):
+        raise ValueError('event operand of shape {} for n = {}, D = {}'.format(tuple(t.shape), n, D))
+    if r == 1 or t.stride(0) == 0:
+        row = t[0]
+        if row.stride(0) != 1:
+            row = row.contiguous()
+        return row, ptr(row), 0, 1
+    if t.stride(1) != 1 or t.stride(0) != D:
+        t = t.contiguous()
+    return t, ptr(t), D, 1
+
+
+def _event_params(family, params, n, D, device):
+    np_ = EVENT_NUM_PARAMS[family]
+    if len(params) != np_:
+        raise ValueError('family {} takes {} parameters, got {}'.format(family, np_, len(params)))
+    held = [_event_operand(p, n, D, device) for p in params]
+    args = []
+    for k in range(4):
+        args += [held[k][1], held[k][2], held[k][3]] if k < np_ else [None, 0, 0]
+    return held, args
+
+
+def event_log_prob(family, value, params, n, D, lp_out=None, acc=None, acc_scale=1.0, device='cuda'):
+    """sum_j log p(value_ij) of an event site: acc[i] += acc_scale * row sum (fp64), and / or the element-wise
+    log-densities lp_out [n, D] (allocated and returned when acc is None).  value / params are event operands (see
+    _event_operand)."""
+    n, D = int(n), int(D)
+    v = _event_operand(value, n, D, device)
+    held, args = _event_params(family, params, n, D, device)
+    if lp_out is None and acc is None:
+        lp_out = torch.empty(n, D, dtype=torch.float32, device=device)
+    if lp_out is not None and (lp_out.dtype != torch.float32 or lp_out.numel() != n * D or not lp_out.is_contiguous()):
+        raise ValueError('lp_out must be a contiguous float32 tensor of n * D elements')
+    if acc is not None and (acc.dtype != torch.float64 or acc.numel() != n or not acc.is_contiguous()):
+        raise ValueError('acc must be a contiguous float64 tensor of length n')
+    call('ppb_event_log_prob', family, v[1], v[2], v[3], *args, n, D, ptr(lp_out), ptr(acc), float(acc_scale), stream())
+    return lp_out
+
+
+def event_sample(family, params, n, D, seed, offset, first_index=0, with_log_prob=False, device='cuda'):
+    """[n, D] draws (element j of particle i from Philox index (first_index + i) | (j << 40)) and, with_log_prob, the
+    event-summed log-density of each row [n]."""
+    n, D = int(n), int(D)
+    if not 1 <= D <= EVENT_MAX_D:
+        raise ValueError('event size D = {} outside [1, 2^24]'.format(D))
+    if first_index < 0 or first_index + n > EVENT_MAX_PARTICLES:
+        raise ValueError('particle indices [{}, {}) outside [0, 2^40)'.format(first_index, first_index + n))
+    held, args = _event_params(family, params, n, D, device)
+    v = torch.empty(n, D, dtype=torch.float32, device=device)
+    lp = torch.empty(n, dtype=torch.float32, device=device) if with_log_prob else None
+    call('ppb_event_sample', family, *args, ptr(v), ptr(lp), n, D, seed, offset, first_index, stream())
+    return (v, lp) if with_log_prob else v
+
+
 # ---- importance weights -----------------------------------------------------------------------------
 
 def weights_cast(acc):

@@ -109,6 +109,18 @@ def _broadcast_value(value, n):
     return v
 
 
+def _observation(distribution, raw, n):
+    """An observed value -> (the value the trace holds, fn(acc) adding likelihood_importance * log p(value)).
+
+    A value with an event shape is one shared event (distributions.py): the trace holds an [n, *E] view of it and the
+    weight term is the sum of its element-wise log-densities (reference: log_prob(value, sum=True), state.py:147)."""
+    ev = distribution.event_site(n, raw)
+    if ev is None:
+        value = _broadcast_value(raw, n)
+        return value, lambda acc: distribution.score_into(value, acc, _likelihood_importance)
+    return ev.site_value, lambda acc: ev.score_into(acc, _likelihood_importance)
+
+
 def _accumulate(trace, fn):
     """Run fn(acc) (which adds weight terms into acc) for the lanes of the current mask only."""
     if _mask is None:
@@ -152,17 +164,18 @@ def observe(distribution, value=None, name=None, address=None):
         return
     base, instance, addr = _addresses(distribution, address, 2)
     n = trace.n
+    score = None
     if name in _observed:
-        value = _broadcast_value(_observed[name], n)
+        value, score = _observation(distribution, _observed[name], n)
     elif value is not None:
-        value = _broadcast_value(value, n)
+        value, score = _observation(distribution, value, n)
     elif _trace_mode == TraceMode.PRIOR_FOR_INFERENCE_NETWORK:
-        value = distribution.sample(n)
+        value = distribution.sample(n)      # [n, *E] for an event-shaped likelihood (reference: state.py:136-137)
     if value is None:
         trace.add(Site(distribution, None, base, addr, instance, name=name, observed=False, mask=_mask))
         return None
     if _trace_mode == TraceMode.POSTERIOR:
-        _accumulate(trace, lambda acc: distribution.score_into(value, acc, _likelihood_importance))
+        _accumulate(trace, score)
     trace.add(Site(distribution, value, base, addr, instance, name=name, observed=True, mask=_mask))
     return value
 
@@ -175,11 +188,15 @@ def sample(distribution, name=None, address=None, control=True):
     base, instance, addr = _addresses(distribution, address, 2)
     n = trace.n
     if name in _observed:
-        value = _broadcast_value(_observed[name], n)
+        value, score = _observation(distribution, _observed[name], n)
         if _trace_mode == TraceMode.POSTERIOR:
-            _accumulate(trace, lambda acc: distribution.score_into(value, acc, _likelihood_importance))
+            _accumulate(trace, score)
         trace.add(Site(distribution, value, base, addr, instance, name=name, observed=True, mask=_mask))
         return value
+    if distribution._shaped and distribution.event_site(n) is not None:
+        raise NotImplementedError('tensor-valued latent sample site {} ({}): pyprob_b200 supports event shapes on '
+                                  'observations only; the reference (pyprob/state.py:157-219) samples such sites with '
+                                  'torch'.format(addr, distribution.name))
 
     if _mcmc is not None:   # MH: every non-observed sample is controlled (reference state.py:165-166)
         value = _mcmc.site(distribution, addr, n, _mask)
