@@ -58,53 +58,9 @@ int ppb_prof_read(double* total_ms_out, int64_t* launches_out, double* flops_out
  *   acc      (nullable) fp64[n]   per-particle running log importance weight; acc[i] += acc_scale*lp
  *                                 (Trace.end's double-precision sum of fp32 terms, pyprob/trace.py:123-125;
  *                                  acc_scale = likelihood_importance for observes, -1 for a proposal term)
+ * The eleven families with an element-wise log_prob (Normal .. VonMises) are scored by ppb_event_log_prob_d1
+ * (section 2b); this section holds the families whose parameters are rows.
  * ---------------------------------------------------------------------------------------------- */
-int ppb_normal_log_prob(const float* value, const float* mean, int mean_stride, const float* stddev,
-                        int stddev_stride, float* lp_out, double* acc, double acc_scale, int64_t n,
-                        void* stream);
-int ppb_uniform_log_prob(const float* value, const float* low, int low_stride, const float* high,
-                         int high_stride, float* lp_out, double* acc, double acc_scale, int64_t n,
-                         void* stream);
-int ppb_poisson_log_prob(const float* value, const float* rate, int rate_stride, float* lp_out,
-                         double* acc, double acc_scale, int64_t n, void* stream);
-/* pyprob/distributions/bernoulli.py (torch Bernoulli(probs=)): v log(pc) + (1 - v) log(1 - pc), pc = clamp_probs(p);
- * a value outside {0, 1} scores NaN (the reference's argument validation raises). */
-int ppb_bernoulli_log_prob(const float* value, const float* probs, int probs_stride, float* lp_out,
-                           double* acc, double acc_scale, int64_t n, void* stream);
-/* The remaining scalar families follow torch.distributions' log_prob, which the reference wraps.  A value outside the
- * support or an invalid parameter scores NaN (the reference's argument validation raises).
- * pyprob/distributions/exponential.py: log r - r x, x >= 0. */
-int ppb_exponential_log_prob(const float* value, const float* rate, int rate_stride, float* lp_out,
-                             double* acc, double acc_scale, int64_t n, void* stream);
-/* pyprob/distributions/gamma.py: xlogy(c, r) + xlogy(c - 1, x) - r x - lgamma(c), x >= 0. */
-int ppb_gamma_log_prob(const float* value, const float* concentration, int concentration_stride,
-                       const float* rate, int rate_stride, float* lp_out, double* acc, double acc_scale,
-                       int64_t n, void* stream);
-/* pyprob/distributions/log_normal.py: Normal(loc, scale).log_prob(log x) - log x, x > 0. */
-int ppb_lognormal_log_prob(const float* value, const float* loc, int loc_stride, const float* scale,
-                           int scale_stride, float* lp_out, double* acc, double acc_scale, int64_t n,
-                           void* stream);
-/* pyprob/distributions/weibull.py: torch's Exponential(1) through PowerTransform(1/k) and AffineTransform(0, scale),
- * x > 0. */
-int ppb_weibull_log_prob(const float* value, const float* scale, int scale_stride, const float* concentration,
-                         int concentration_stride, float* lp_out, double* acc, double acc_scale, int64_t n,
-                         void* stream);
-/* pyprob/distributions/beta.py:38-40: torch Beta(c1, c0).log_prob((x - low) / (high - low)), with no -log(high - low)
- * term, as the reference; (x - low) / (high - low) in [0, 1]. */
-int ppb_beta_log_prob(const float* value, const float* concentration1, int concentration1_stride,
-                      const float* concentration0, int concentration0_stride, const float* low, int low_stride,
-                      const float* high, int high_stride, float* lp_out, double* acc, double acc_scale,
-                      int64_t n, void* stream);
-/* pyprob/distributions/binomial.py (torch Binomial(total_count, probs=)): torch's logits form with
- * logits = log(pc) - log1p(-pc), pc = clamp_probs(p); x an integer in [0, total_count]. */
-int ppb_binomial_log_prob(const float* value, const float* total_count, int total_count_stride,
-                          const float* probs, int probs_stride, float* lp_out, double* acc, double acc_scale,
-                          int64_t n, void* stream);
-/* pyprob/distributions/von_mises.py: kappa cos(x - loc) - log(2 pi) - log I0(kappa), log I0 as torch's
- * _log_modified_bessel_fn computes it (finite at any kappa). */
-int ppb_von_mises_log_prob(const float* value, const float* loc, int loc_stride, const float* concentration,
-                           int concentration_stride, float* lp_out, double* acc, double acc_scale, int64_t n,
-                           void* stream);
 /* probs: [n, C] (probs_row_stride = C) or [C] shared (probs_row_stride = 0); unnormalised, as given to
  * pyprob/distributions/categorical.py:8-21.  value holds category indices stored as fp32. */
 int ppb_categorical_log_prob(const float* value, const float* probs, int64_t probs_row_stride,
@@ -132,50 +88,8 @@ int ppb_mixture_truncated_normal_log_prob(const float* value, const float* means
  * are independent of the launch geometry and of the number of GPUs (rank r shards the index range).
  * `first_index` is the global index of element 0 (for sharded particle ranges).
  * lp_out (nullable): log_prob of the drawn value under the sampled distribution (fused sample+score).
+ * The eleven families with an element-wise log_prob are drawn by ppb_event_sample_d1 (section 2b).
  * ---------------------------------------------------------------------------------------------- */
-int ppb_normal_sample(const float* mean, int mean_stride, const float* stddev, int stddev_stride,
-                      float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset,
-                      int64_t first_index, void* stream);
-int ppb_uniform_sample(const float* low, int low_stride, const float* high, int high_stride,
-                       float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset,
-                       int64_t first_index, void* stream);
-int ppb_poisson_sample(const float* rate, int rate_stride, float* value_out, float* lp_out, int64_t n,
-                       uint64_t seed, uint64_t offset, int64_t first_index, void* stream);
-/* value = 1 if u < p else 0, u uniform in [0, 1) from Philox word 0 */
-int ppb_bernoulli_sample(const float* probs, int probs_stride, float* value_out, float* lp_out, int64_t n,
-                         uint64_t seed, uint64_t offset, int64_t first_index, void* stream);
-/* The samplers of the families in section 1 (pyprob/distributions/{exponential,gamma,log_normal,weibull,beta,binomial,
- * von_mises}.py).  Invalid parameters draw NaN.  The rejection samplers draw each round from the counter
- * (i, offset + (round << 40)) and stop after a fixed number of rounds (failure probability below 1e-12 per draw),
- * so every draw takes bounded time.
- *   exponential: -log(u) / rate (inversion)
- *   gamma:       Marsaglia-Tsang for c >= 1; G(c + 1) u^(1/c) for c < 1; clamped below at FLT_MIN, as torch
- *   lognormal:   exp of the Box-Muller normal
- *   weibull:     scale (-log u)^(1/k)
- *   beta:        low + (high - low) Ga / (Ga + Gb), the ratio clamped to [FLT_MIN, 1 - eps] as torch's Dirichlet
- *   binomial:    inversion for n min(p, 1 - p) < 10, BTRS (Hoermann 1993) otherwise; total_count per particle or shared
- *   von_mises:   Best-Fisher rejection in double precision, wrapped into [-pi, pi) as torch */
-int ppb_exponential_sample(const float* rate, int rate_stride, float* value_out, float* lp_out, int64_t n,
-                           uint64_t seed, uint64_t offset, int64_t first_index, void* stream);
-int ppb_gamma_sample(const float* concentration, int concentration_stride, const float* rate, int rate_stride,
-                     float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset,
-                     int64_t first_index, void* stream);
-int ppb_lognormal_sample(const float* loc, int loc_stride, const float* scale, int scale_stride,
-                         float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset,
-                         int64_t first_index, void* stream);
-int ppb_weibull_sample(const float* scale, int scale_stride, const float* concentration, int concentration_stride,
-                       float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset,
-                       int64_t first_index, void* stream);
-int ppb_beta_sample(const float* concentration1, int concentration1_stride, const float* concentration0,
-                    int concentration0_stride, const float* low, int low_stride, const float* high,
-                    int high_stride, float* value_out, float* lp_out, int64_t n, uint64_t seed,
-                    uint64_t offset, int64_t first_index, void* stream);
-int ppb_binomial_sample(const float* total_count, int total_count_stride, const float* probs, int probs_stride,
-                        float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset,
-                        int64_t first_index, void* stream);
-int ppb_von_mises_sample(const float* loc, int loc_stride, const float* concentration, int concentration_stride,
-                         float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset,
-                         int64_t first_index, void* stream);
 int ppb_categorical_sample(const float* probs, int64_t probs_row_stride, int num_categories,
                            float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset,
                            int64_t first_index, void* stream);
@@ -189,19 +103,37 @@ int ppb_mixture_truncated_normal_sample(const float* means, const float* stddevs
                                         int64_t first_index, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * 2b. Event-shaped observations: sites whose value is a vector or an image
+ * 2b. The families with an element-wise log_prob: scalar sites, and sites whose value is a vector or an image
  *
- * Replace  pyprob/state.py:118-155 with a tensor value: distribution.log_prob(value, sum=True) as
- * pyprob/distributions/distribution.py:38-43 computes it (torch broadcasts the value against the parameters and the
- * element-wise log-densities are summed), and pyprob/state.py:136-137, which draws the observed value from the
- * likelihood for a training trace.  A site has D = prod(event shape) elements per particle.
+ * Replace  pyprob/distributions/distribution.py:31-43 for these families as pyprob/state.py drives them, one
+ * particle at a time, and pyprob/state.py:118-155 with a tensor value: distribution.log_prob(value, sum=True)
+ * (torch broadcasts the value against the parameters and the element-wise log-densities are summed), and
+ * pyprob/state.py:136-137, which draws the observed value from the likelihood for a training trace.
+ * A site has D = prod(event shape) elements per particle; D = 1 is the per-particle (scalar) site.
  * Every operand is (pointer, particle stride ps, element stride es): element j of particle i is p[i ps + j es], and
- * (ps, es) must be one of (0, 0) scalar, (1, 0) one per particle, (0, 1) shared event, (D, 1) event per particle.
- * Families and their parameters p0 .. p3 (unused slots are ignored):
- *   NORMAL (loc, scale), UNIFORM (low, high), POISSON (rate), BERNOULLI (probs), EXPONENTIAL (rate),
- *   GAMMA (concentration, rate), LOGNORMAL (loc, scale), WEIBULL (scale, concentration),
- *   BETA (concentration1, concentration0, low, high), BINOMIAL (total_count, probs), VON_MISES (loc, concentration);
- * each element is scored exactly as the family's section-1 entry point scores a particle.
+ * (ps, es) must be one of (0, 0) scalar, (1, 0) one per particle, (0, 1) shared event, (D, 1) event per particle
+ * (at D = 1 all four are a scalar or one per particle).
+ * Families and their parameters p0 .. p3 (unused slots are ignored).  log_prob follows torch.distributions, which the
+ * reference wraps; a value outside the support or an invalid parameter scores NaN (the reference's argument
+ * validation raises) and draws NaN:
+ *   NORMAL (loc, scale), UNIFORM (low, high), POISSON (rate)
+ *   BERNOULLI (probs): v log(pc) + (1 - v) log(1 - pc), pc = clamp_probs(p), v in {0, 1}; draws 1 if u < p
+ *   EXPONENTIAL (rate): log r - r x, x >= 0
+ *   GAMMA (concentration, rate): xlogy(c, r) + xlogy(c - 1, x) - r x - lgamma(c), x >= 0
+ *   LOGNORMAL (loc, scale): Normal(loc, scale).log_prob(log x) - log x, x > 0
+ *   WEIBULL (scale, concentration): torch's Exponential(1) through PowerTransform(1/k), AffineTransform(0, scale)
+ *   BETA (concentration1, concentration0, low, high): torch Beta(c1, c0).log_prob((x - low) / (high - low)), with no
+ *     -log(high - low) term, as pyprob/distributions/beta.py:38-40
+ *   BINOMIAL (total_count, probs): torch's logits form, logits = log(pc) - log1p(-pc); x an integer in [0, total_count]
+ *   VON_MISES (loc, concentration): kappa cos(x - loc) - log(2 pi) - log I0(kappa), log I0 as torch's
+ *     _log_modified_bessel_fn computes it (finite at any kappa)
+ * Draws: Normal and LogNormal by Box-Muller, Uniform, Exponential and Weibull by inversion, Poisson by inversion below
+ * rate 10 and PTRS above; Gamma by Marsaglia-Tsang (c < 1 as G(c + 1) u^(1/c)), clamped below at FLT_MIN as torch;
+ * Beta as low + (high - low) Ga / (Ga + Gb), the ratio clamped to [FLT_MIN, 1 - eps] as torch's Dirichlet; Binomial by
+ * inversion for n min(p, 1 - p) < 10 and BTRS (Hoermann 1993) otherwise; VonMises by Best-Fisher rejection in double
+ * precision, wrapped into [-pi, pi) as torch.  The rejection samplers draw each round from the counter
+ * (index, offset + (round << 40)) and stop after a fixed number of rounds (failure probability below 1e-12 per draw),
+ * so every draw takes bounded time.
  * ---------------------------------------------------------------------------------------------- */
 #define PPB_EVENT_NORMAL 0
 #define PPB_EVENT_UNIFORM 1
@@ -215,23 +147,34 @@ int ppb_mixture_truncated_normal_sample(const float* means, const float* stddevs
 #define PPB_EVENT_BINOMIAL 9
 #define PPB_EVENT_VON_MISES 10
 /* acc (nullable) fp64[n]: acc[i] += acc_scale * sum_j lp_ij, summed in fp64 in an order that depends on (n, D) only,
- * without atomics (repeated calls give identical bits; with D = 1 the update is the section-1 entry point's).
- * lp_out (nullable) fp32[n, D], row-major: the element-wise log-densities.  PPB_EINVAL for an unknown family, n < 0,
- * D < 1, a null operand the family needs, or strides not of the four forms. */
+ * without atomics (repeated calls give identical bits).
+ * lp_out (nullable) fp32[n, D], row-major: the element-wise log-densities.  PPB_EINVAL for an unknown family, n < 0 or
+ * D < 1, and with n > 0 for a null operand the family needs or strides not of the four forms; n = 0 does nothing. */
 int ppb_event_log_prob(int family, const float* value, int64_t value_ps, int64_t value_es, const float* p0,
                        int64_t p0_ps, int64_t p0_es, const float* p1, int64_t p1_ps, int64_t p1_es,
                        const float* p2, int64_t p2_ps, int64_t p2_es, const float* p3, int64_t p3_ps,
                        int64_t p3_es, int64_t n, int64_t D, float* lp_out, double* acc, double acc_scale,
                        void* stream);
 /* value_out fp32[n, D] row-major; lp_out (nullable) fp32[n]: the row's event-summed log-density, as
- * ppb_event_log_prob sums it.  Element j of particle i draws with the family's section-2 draw from the Philox counter
- * ((first_index + i) | (j << 40), offset + (round << 40)): element 0 is the section-2 draw bit for bit, and a shard of
- * the particles draws the rows the full run draws.  PPB_EINVAL, besides the cases above, for D > 2^24 or
- * first_index + n > 2^40 (the counter fields would overlap). */
+ * ppb_event_log_prob sums it.  Element j of particle i draws from the Philox counter
+ * ((first_index + i) | (j << 40), offset + (round << 40)): element 0 is the D = 1 draw bit for bit, and a shard of
+ * the particles draws the rows the full run draws.  PPB_EINVAL, besides the cases above, for D > 2^24, a negative
+ * first_index or first_index + n > 2^40 (the counter fields would overlap), at any D, and for a null value_out with
+ * n > 0. */
 int ppb_event_sample(int family, const float* p0, int64_t p0_ps, int64_t p0_es, const float* p1, int64_t p1_ps,
                      int64_t p1_es, const float* p2, int64_t p2_ps, int64_t p2_es, const float* p3, int64_t p3_ps,
                      int64_t p3_es, float* value_out, float* lp_out, int64_t n, int64_t D, uint64_t seed,
                      uint64_t offset, int64_t first_index, void* stream);
+/* The same two entry points at D = 1, the per-particle site, with a shorter argument list for the calls that score or
+ * draw one scalar site at a time: value is fp32[n]; parameter k is one per particle where bit k of param_strides is set
+ * and a scalar where it is clear (unused slots are ignored).  Results, checks and draws are ppb_event_log_prob's and
+ * ppb_event_sample's with D = 1. */
+int ppb_event_log_prob_d1(int family, const float* value, const float* p0, const float* p1, const float* p2,
+                          const float* p3, int param_strides, float* lp_out, double* acc, double acc_scale, int64_t n,
+                          void* stream);
+int ppb_event_sample_d1(int family, const float* p0, const float* p1, const float* p2, const float* p3,
+                        int param_strides, float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset,
+                        int64_t first_index, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * 3. Importance-weight normalisation (SURVEY §8a rows a14, a15)

@@ -28,32 +28,10 @@ _SIGNATURES = {
     'ppb_launch_count': [],
     'ppb_prof_enable': [c_int],
     'ppb_prof_read': [C.c_void_p, C.c_void_p, C.c_void_p],
-    'ppb_normal_log_prob': [c_f, c_f, c_int, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
-    'ppb_uniform_log_prob': [c_f, c_f, c_int, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
-    'ppb_poisson_log_prob': [c_f, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
-    'ppb_bernoulli_log_prob': [c_f, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
-    'ppb_exponential_log_prob': [c_f, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
-    'ppb_gamma_log_prob': [c_f, c_f, c_int, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
-    'ppb_lognormal_log_prob': [c_f, c_f, c_int, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
-    'ppb_weibull_log_prob': [c_f, c_f, c_int, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
-    'ppb_beta_log_prob': [c_f, c_f, c_int, c_f, c_int, c_f, c_int, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
-    'ppb_binomial_log_prob': [c_f, c_f, c_int, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
-    'ppb_von_mises_log_prob': [c_f, c_f, c_int, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
     'ppb_categorical_log_prob': [c_f, c_f, c_i64, c_int, c_f, c_f, c_dbl, c_i64, c_f],
     'ppb_mixture_normal_log_prob': [c_f, c_f, c_f, c_f, c_i64, c_int, c_f, c_f, c_dbl, c_i64, c_f],
     'ppb_mixture_truncated_normal_log_prob': [c_f, c_f, c_f, c_f, c_i64, c_int, c_f, c_int, c_f, c_int, c_f, c_f,
                                               c_dbl, c_i64, c_f],
-    'ppb_normal_sample': [c_f, c_int, c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
-    'ppb_uniform_sample': [c_f, c_int, c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
-    'ppb_poisson_sample': [c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
-    'ppb_bernoulli_sample': [c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
-    'ppb_exponential_sample': [c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
-    'ppb_gamma_sample': [c_f, c_int, c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
-    'ppb_lognormal_sample': [c_f, c_int, c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
-    'ppb_weibull_sample': [c_f, c_int, c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
-    'ppb_beta_sample': [c_f, c_int, c_f, c_int, c_f, c_int, c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
-    'ppb_binomial_sample': [c_f, c_int, c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
-    'ppb_von_mises_sample': [c_f, c_int, c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
     'ppb_categorical_sample': [c_f, c_i64, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
     'ppb_mixture_normal_sample': [c_f, c_f, c_f, c_i64, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
     'ppb_mixture_truncated_normal_sample': [c_f, c_f, c_f, c_i64, c_int, c_f, c_int, c_f, c_int, c_f, c_f, c_i64,
@@ -62,6 +40,8 @@ _SIGNATURES = {
                            c_i64, c_i64, c_i64, c_i64, c_f, c_f, c_dbl, c_f],
     'ppb_event_sample': [c_int, c_f, c_i64, c_i64, c_f, c_i64, c_i64, c_f, c_i64, c_i64, c_f, c_i64, c_i64, c_f, c_f,
                          c_i64, c_i64, c_u64, c_u64, c_i64, c_f],
+    'ppb_event_log_prob_d1': [c_int, c_f, c_f, c_f, c_f, c_f, c_int, c_f, c_f, c_dbl, c_i64, c_f],
+    'ppb_event_sample_d1': [c_int, c_f, c_f, c_f, c_f, c_int, c_f, c_f, c_i64, c_u64, c_u64, c_i64, c_f],
     'ppb_weights_cast': [c_f, c_f, c_f, c_i64, c_f],
     'ppb_weights_num_partials': [c_i64],
     'ppb_weights_partials': [c_f, c_i64, c_f, c_f],

@@ -1,6 +1,6 @@
-// Log-densities of the Exponential, Gamma, LogNormal, Weibull, Beta, Binomial and VonMises families, shared by the
-// scoring kernels (scoring.cu) and the fused sample+score samplers (sampling.cu), so that a sampler's lp_out is the
-// log_prob kernel's value at the drawn value.
+// Log-densities of the eleven families with an element-wise log_prob (PPB_EVENT_*), shared by the scoring kernels
+// (scoring.cu) and the fused sample+score samplers (sampling.cu), so that a sampler's lp_out is the log_prob kernel's
+// value at the drawn value.
 // The reference wraps torch.distributions (pyprob/distributions/{exponential,gamma,log_normal,weibull,beta,binomial,
 // von_mises}.py); every function below follows torch's log_prob term by term, in fp32.  A value outside the support or
 // an invalid parameter gives NaN: the reference's argument validation raises there, and ppb_weights_cast then marks
@@ -12,6 +12,30 @@
 
 #define PPB_FLT_TINY 1.17549435e-38f     // torch.finfo(torch.float32).tiny
 #define PPB_LOG_2PI 1.8378770664093453f  // math.log(2 * math.pi)
+
+// MUFU approximations (<= 2 ulp): the scoring kernels are bound by instruction issue, not HBM, as soon as they carry an IEEE
+// division or a libm logf/expf; results stay within 1e-6 relative of the libm forms.
+__device__ __forceinline__ float fast_rcp(float x) { float r; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
+__device__ __forceinline__ float fast_ex2(float x) { float r; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
+__device__ __forceinline__ float fast_lg2(float x) { float r; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
+
+// log(k!) for the counts that actually occur (k < 64), correctly rounded from the double-precision lgamma: lgammaf costs
+// ~40 instructions per particle and made the Poisson kernel ALU-bound at 39 % of HBM; other values take lgammaf.
+// A kernel whose Op has kTable copies the table to shared memory in every CTA: the lanes of a warp hold different counts,
+// and a constant-bank read with divergent indices is replayed once per distinct address (63 % of HBM), shared memory
+// serves them in one pass.  The library is built without relocatable device code, so every translation unit has its own
+// copy of the table and uploads it once, on its first launch that needs it.
+static __constant__ float c_log_factorial[64];
+static inline int ppb_upload_log_factorial() {
+  static bool table_ready = false;
+  if (!table_ready) {
+    float t[64];
+    for (int k = 0; k < 64; ++k) t[k] = (float)lgamma((double)k + 1.0);
+    PPB_CUDA(cudaMemcpyToSymbol(c_log_factorial, t, sizeof(t)));
+    table_ready = true;
+  }
+  return PPB_OK;
+}
 
 namespace fam {
 
@@ -117,9 +141,137 @@ __device__ __forceinline__ float von_mises_lp(float v, float loc, float kappa, f
 
 }  // namespace fam
 
-// Event-summed log_prob (scoring.cu), shared with the event samplers (sampling.cu), whose lp_out is this kernel's fp32
-// row sum of the drawn rows.  params / params_ps / params_es hold ppb_event_num_params(family) operands.
-int ppb_event_num_params(int family);
+// ---- one log-density functor per family ---------------------------------------------------------------------------------
+// op(v, p, tab): log p(v) under parameters p[0 .. kParams - 1] (the PPB_EVENT_* order; later slots are unused), with tab
+// the shared-memory copy of c_log_factorial when kTable.  An Op whose log_prob has a term that depends on the parameters
+// only keeps it in the thread together with the parameters it was computed for, and recomputes it only when they change:
+// with shared (stride-0) parameters that is once per thread instead of once per particle (lgammaf alone is ~40
+// instructions).  A kernel keeps one Op per thread for its whole grid-stride loop.
+struct NormalOp {
+  static constexpr int kFamily = PPB_EVENT_NORMAL, kParams = 2;
+  static constexpr bool kTable = false;
+  // torch/distributions/normal.py log_prob: -((v - mu)^2) / (2 var) - log(sigma) - log(sqrt(2 pi))
+  __device__ __forceinline__ float operator()(float v, const float (&p)[4], const float*) const {
+    const float z = (v - p[0]) * fast_rcp(p[1]);
+    return fmaf(-0.5f * z, z, -fast_lg2(p[1]) * PPB_LN2) - PPB_LOG_SQRT_2PI;
+  }
+};
+struct UniformOp {
+  static constexpr int kFamily = PPB_EVENT_UNIFORM, kParams = 2;
+  static constexpr bool kTable = false;
+  // torch/distributions/uniform.py log_prob: log(lb*ub) - log(high-low), lb = low<=v, ub = high>v
+  __device__ __forceinline__ float operator()(float v, const float (&p)[4], const float*) const {
+    float inside = (p[0] <= v && p[1] > v) ? 0.0f : -INFINITY;
+    return inside - logf(p[1] - p[0]);
+  }
+};
+struct PoissonOp {
+  static constexpr int kFamily = PPB_EVENT_POISSON, kParams = 1;
+  static constexpr bool kTable = true;
+  // torch/distributions/poisson.py log_prob: xlogy(v, rate) - rate - lgamma(v+1)
+  __device__ __forceinline__ float operator()(float v, const float (&p)[4], const float* tab) const {
+    float xl = (v == 0.0f) ? 0.0f : v * (fast_lg2(p[0]) * PPB_LN2);
+    const int k = (int)v;
+    const float lg = (v >= 0.0f && v < 64.0f && (float)k == v) ? tab[k] : lgammaf(v + 1.0f);
+    return xl - p[0] - lg;
+  }
+};
+struct BernoulliOp {
+  static constexpr int kFamily = PPB_EVENT_BERNOULLI, kParams = 1;
+  static constexpr bool kTable = false;
+  // torch/distributions/bernoulli.py log_prob: -BCEWithLogits(log pc - log1p(-pc), v) = v log pc + (1 - v) log(1 - pc),
+  // pc = clamp_probs(p); values outside {0, 1} are rejected by the reference's argument validation: NaN here
+  __device__ __forceinline__ float operator()(float v, const float (&p)[4], const float*) const {
+    const float pc = ppb_clamp_prob(p[0]);
+    return (v == 1.0f) ? logf(pc) : (v == 0.0f) ? log1pf(-pc) : NAN;
+  }
+};
+struct ExponentialOp {
+  static constexpr int kFamily = PPB_EVENT_EXPONENTIAL, kParams = 1;
+  static constexpr bool kTable = false;
+  __device__ __forceinline__ float operator()(float v, const float (&p)[4], const float*) const {
+    return fam::exponential_lp(v, p[0]);
+  }
+};
+struct GammaOp {
+  static constexpr int kFamily = PPB_EVENT_GAMMA, kParams = 2;
+  static constexpr bool kTable = false;
+  float c_ = NAN, r_ = NAN, k_ = NAN;
+  __device__ __forceinline__ float operator()(float v, const float (&p)[4], const float*) {
+    if (!(p[0] == c_ && p[1] == r_)) { c_ = p[0]; r_ = p[1]; k_ = fam::gamma_const(p[0], p[1]); }
+    return fam::gamma_lp(v, p[0], p[1], k_);
+  }
+};
+struct LogNormalOp {
+  static constexpr int kFamily = PPB_EVENT_LOGNORMAL, kParams = 2;
+  static constexpr bool kTable = false;
+  __device__ __forceinline__ float operator()(float v, const float (&p)[4], const float*) const {
+    return fam::lognormal_lp(v, p[0], p[1]);
+  }
+};
+struct WeibullOp {
+  static constexpr int kFamily = PPB_EVENT_WEIBULL, kParams = 2;
+  static constexpr bool kTable = false;
+  __device__ __forceinline__ float operator()(float v, const float (&p)[4], const float*) const {
+    return fam::weibull_lp(v, p[0], p[1]);
+  }
+};
+struct BetaOp {
+  static constexpr int kFamily = PPB_EVENT_BETA, kParams = 4;
+  static constexpr bool kTable = false;
+  float a_ = NAN, b_ = NAN, k_ = NAN;
+  __device__ __forceinline__ float operator()(float v, const float (&p)[4], const float*) {
+    if (!(p[0] == a_ && p[1] == b_)) { a_ = p[0]; b_ = p[1]; k_ = fam::beta_const(p[0], p[1]); }
+    return fam::beta_lp(v, p[0], p[1], p[2], p[3], k_);
+  }
+};
+struct BinomialOp {
+  static constexpr int kFamily = PPB_EVENT_BINOMIAL, kParams = 2;
+  static constexpr bool kTable = false;
+  float n_ = NAN, p_ = NAN;
+  fam::BinomialConst k_{NAN, NAN};
+  __device__ __forceinline__ float operator()(float v, const float (&p)[4], const float*) {
+    if (!(p[0] == n_ && p[1] == p_)) { n_ = p[0]; p_ = p[1]; k_ = fam::binomial_const(p[0], p[1]); }
+    return fam::binomial_lp(v, p[0], p[1], k_);
+  }
+};
+struct VonMisesOp {
+  static constexpr int kFamily = PPB_EVENT_VON_MISES, kParams = 2;
+  static constexpr bool kTable = false;
+  float kappa_ = NAN, k_ = NAN;
+  __device__ __forceinline__ float operator()(float v, const float (&p)[4], const float*) {
+    if (!(p[1] == kappa_)) { kappa_ = p[1]; k_ = fam::von_mises_const(p[1]); }
+    return fam::von_mises_lp(v, p[0], p[1], k_);
+  }
+};
+
+// fn(Op{}) for the Op of a PPB_EVENT_* id; -1 for an unknown id
+template <class Fn>
+int ppb_with_family(int family, Fn&& fn) {
+  switch (family) {
+    case PPB_EVENT_NORMAL: return fn(NormalOp{});
+    case PPB_EVENT_UNIFORM: return fn(UniformOp{});
+    case PPB_EVENT_POISSON: return fn(PoissonOp{});
+    case PPB_EVENT_BERNOULLI: return fn(BernoulliOp{});
+    case PPB_EVENT_EXPONENTIAL: return fn(ExponentialOp{});
+    case PPB_EVENT_GAMMA: return fn(GammaOp{});
+    case PPB_EVENT_LOGNORMAL: return fn(LogNormalOp{});
+    case PPB_EVENT_WEIBULL: return fn(WeibullOp{});
+    case PPB_EVENT_BETA: return fn(BetaOp{});
+    case PPB_EVENT_BINOMIAL: return fn(BinomialOp{});
+    case PPB_EVENT_VON_MISES: return fn(VonMisesOp{});
+    default: return -1;
+  }
+}
+
+// number of parameters of a family; -1 for an unknown id
+inline int ppb_event_num_params(int family) {
+  return ppb_with_family(family, [](auto op) { return decltype(op)::kParams; });
+}
+
+// Event-summed log_prob (scoring.cu), shared with the event sampler (sampling.cu), whose lp_out at D > 1 is this
+// kernel's fp32 row sum of the drawn rows (row_lp; at D = 1 a row is its one element, lp_out).  params / params_ps /
+// params_es hold ppb_event_num_params(family) operands.
 int ppb_event_score(int family, const float* value, int64_t value_ps, int64_t value_es, const float* const* params,
                     const int64_t* params_ps, const int64_t* params_es, int64_t n, int64_t D, float* lp_out,
                     float* row_lp, double* acc, double acc_scale, void* stream);

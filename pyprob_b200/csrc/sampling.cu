@@ -1,6 +1,7 @@
 // Samplers over the particle axis (Philox4x32-10, counter = (global particle index, offset)).
 // Replaces pyprob/distributions/distribution.py:31-36, mixture.py:47-63, truncated_normal.py:94-112.
-// Fused sample+score: lp_out (nullable) gets log_prob of the drawn value (pyprob/state.py:196-197).
+// Fused sample+score: lp_out (nullable) gets log_prob of the drawn value (pyprob/state.py:196-197); for the eleven
+// element-wise families that is the scoring kernels' value, through the Ops of families.cuh.
 // Event draws (k_event_sample, [n, D]): element j of particle i uses Philox index (first + i) | (j << 40) and the usual
 // offset + (round << 40) for rejection rounds, so particle indices must stay below 2^40 and D at most 2^24 (checked
 // before launch); element 0 is the per-particle draw, and a shard of the particles draws the full run's rows.
@@ -17,28 +18,12 @@ struct P {
   __device__ __forceinline__ float at(int64_t i) const { return stride ? __ldg(p + i) : __ldg(p); }
 };
 
-// The draw of each family from Philox counter (idx, offset [+ (round << 40)]), shared by the per-particle samplers and the
-// event sampler (k_event_sample), so that element 0 of an event row is the per-particle draw bit for bit.
-// The single-counter families take the Philox words of (idx, offset).  k_normal and k_von_mises spell their draw out in
-// the kernel: with the draw behind a function their SASS changes (instruction order and registers), and the test that
-// element 0 of an event row is the per-particle draw bit for bit ties the two forms together.
+// The draw of each family from Philox counter (idx, offset [+ (round << 40)]), shared by the per-particle sampler (k_sample)
+// and the event sampler (k_event_sample), so that element 0 of an event row is the per-particle draw bit for bit.
+// The single-counter families take the Philox words of (idx, offset).
 __device__ __forceinline__ float normal_draw(const ppb_philox& r, float mu, float s) {
   float z = ppb_std_normal_from(r.c[0], r.c[1]);
   return mu + s * z;
-}
-
-__global__ void __launch_bounds__(kThreads) k_normal(P mean, P sd, float* __restrict__ out, float* __restrict__ lp,
-                                                      int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
-  int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, nth = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = tid; i < n; i += nth) {
-    // the draw of normal_draw (the event sampler's), spelled out: change both together
-    ppb_philox r = ppb_philox4x32_10(seed, (uint64_t)(first + i), offset);
-    float z = ppb_std_normal_from(r.c[0], r.c[1]);
-    float mu = mean.at(i), s = sd.at(i);
-    float v = mu + s * z;
-    out[i] = v;
-    if (lp) lp[i] = ppb_normal_lp(v, mu, s);
-  }
 }
 
 __device__ __forceinline__ float uniform_draw(const ppb_philox& r, float lo, float hi) {
@@ -47,18 +32,6 @@ __device__ __forceinline__ float uniform_draw(const ppb_philox& r, float lo, flo
   // scores -inf: step such a draw to the largest float below hi
   if (v >= hi) v = nextafterf(hi, lo);
   return v;
-}
-
-__global__ void __launch_bounds__(kThreads) k_uniform(P low, P high, float* __restrict__ out, float* __restrict__ lp,
-                                                       int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
-  int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, nth = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = tid; i < n; i += nth) {
-    ppb_philox r = ppb_philox4x32_10(seed, (uint64_t)(first + i), offset);
-    float lo = low.at(i), hi = high.at(i);
-    float v = uniform_draw(r, lo, hi);
-    out[i] = v;
-    if (lp) lp[i] = ((lo <= v && hi > v) ? 0.0f : -INFINITY) - logf(hi - lo);
-  }
 }
 
 // Poisson: inversion by sequential search for rate < 10 (Devroye), PTRS transformed rejection
@@ -105,38 +78,11 @@ __device__ float poisson_draw(float rate, uint64_t seed, uint64_t idx, uint64_t 
   return floorf(rate);
 }
 
-__global__ void __launch_bounds__(kThreads) k_poisson(P rate, float* __restrict__ out, float* __restrict__ lp,
-                                                       int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
-  int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, nth = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = tid; i < n; i += nth) {
-    float lam = rate.at(i);
-    float v = poisson_draw(lam, seed, (uint64_t)(first + i), offset);
-    out[i] = v;
-    if (lp) lp[i] = ((v == 0.0f) ? 0.0f : v * logf(lam)) - lam - lgammaf(v + 1.0f);
-  }
-}
-
 // Bernoulli: 1 if u < p (u uniform in [0, 1) from word 0), so p = 0 never and p = 1 always draws 1
 __device__ __forceinline__ bool bernoulli_one(const ppb_philox& r, float p) {
   return ppb_u01(r.c[0]) < p;
 }
 
-__global__ void __launch_bounds__(kThreads) k_bernoulli(P probs, float* __restrict__ out, float* __restrict__ lp,
-                                                         int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
-  int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, nth = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = tid; i < n; i += nth) {
-    ppb_philox r = ppb_philox4x32_10(seed, (uint64_t)(first + i), offset);
-    const float p = probs.at(i);
-    const bool one = bernoulli_one(r, p);
-    out[i] = one ? 1.0f : 0.0f;
-    if (lp) {
-      const float pc = ppb_clamp_prob(p);
-      lp[i] = one ? logf(pc) : log1pf(-pc);
-    }
-  }
-}
-
-// ---- Exponential .. VonMises: lp_out through the log_prob functions of families.cuh ------------------------------------
 // uniform in (0, 1), open at both ends: the inversions below take logs of u and of 1 - u
 __device__ __forceinline__ float u01_open(uint32_t x) { return ((float)(x >> 8) + 0.5f) * (1.0f / 16777216.0f); }
 // uniform in [0, 1) with 53 random bits from two words
@@ -147,23 +93,9 @@ __device__ __forceinline__ ppb_philox philox_sub(uint64_t seed, uint64_t idx, ui
   return ppb_philox4x32_10(seed, idx, offset + (sub << 40));   // fresh words for rejection rounds, as poisson_draw
 }
 
-#define PPB_GRID_LOOP(i) \
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
-
 // Exponential: inversion, -log(u) / rate
 __device__ __forceinline__ float exponential_draw(const ppb_philox& r, float lam) {
   return (lam > 0.0f) ? -logf(u01_open(r.c[0])) / lam : NAN;
-}
-
-__global__ void __launch_bounds__(kThreads) k_exponential(P rate, float* __restrict__ out, float* __restrict__ lp,
-                                                           int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
-  PPB_GRID_LOOP(i) {
-    ppb_philox r = ppb_philox4x32_10(seed, (uint64_t)(first + i), offset);
-    const float lam = rate.at(i);
-    const float v = exponential_draw(r, lam);
-    out[i] = v;
-    if (lp) lp[i] = fam::exponential_lp(v, lam);
-  }
 }
 
 // log of a standard Gamma(c) draw.  Marsaglia & Tsang (2000) for c >= 1; c < 1 as G(c + 1) U^(1/c), with the power
@@ -207,46 +139,14 @@ __device__ __forceinline__ float gamma_draw(float c, float rt, uint64_t seed, ui
   return v;
 }
 
-__global__ void __launch_bounds__(kThreads) k_gamma(P conc, P rate, float* __restrict__ out, float* __restrict__ lp,
-                                                     int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
-  PPB_GRID_LOOP(i) {
-    const float c = conc.at(i), rt = rate.at(i);
-    const float v = gamma_draw(c, rt, seed, (uint64_t)(first + i), offset);
-    out[i] = v;
-    if (lp) lp[i] = fam::gamma_lp(v, c, rt, fam::gamma_const(c, rt));
-  }
-}
-
-// LogNormal: exp of the Box-Muller normal that k_normal draws
+// LogNormal: exp of the Box-Muller normal that normal_draw draws
 __device__ __forceinline__ float lognormal_draw(const ppb_philox& r, float mu, float s) {
   return (s > 0.0f) ? expf(mu + s * ppb_std_normal_from(r.c[0], r.c[1])) : NAN;
-}
-
-__global__ void __launch_bounds__(kThreads) k_lognormal(P loc, P scale, float* __restrict__ out, float* __restrict__ lp,
-                                                         int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
-  PPB_GRID_LOOP(i) {
-    ppb_philox r = ppb_philox4x32_10(seed, (uint64_t)(first + i), offset);
-    const float mu = loc.at(i), s = scale.at(i);
-    const float v = lognormal_draw(r, mu, s);
-    out[i] = v;
-    if (lp) lp[i] = fam::lognormal_lp(v, mu, s);
-  }
 }
 
 // Weibull: scale (-log u)^(1/k), kept above 0 (the support) where the power underflows
 __device__ __forceinline__ float weibull_draw(const ppb_philox& r, float lam, float k) {
   return (lam > 0.0f && k > 0.0f) ? fmaxf(lam * powf(-logf(u01_open(r.c[0])), 1.0f / k), PPB_FLT_TINY) : NAN;
-}
-
-__global__ void __launch_bounds__(kThreads) k_weibull(P scale, P conc, float* __restrict__ out, float* __restrict__ lp,
-                                                       int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
-  PPB_GRID_LOOP(i) {
-    ppb_philox r = ppb_philox4x32_10(seed, (uint64_t)(first + i), offset);
-    const float lam = scale.at(i), k = conc.at(i);
-    const float v = weibull_draw(r, lam, k);
-    out[i] = v;
-    if (lp) lp[i] = fam::weibull_lp(v, lam, k);
-  }
 }
 
 // Beta: Ga / (Ga + Gb) from two standard Gamma draws on disjoint sub-counters, as 1 / (1 + exp(log Gb - log Ga)) so that
@@ -261,17 +161,6 @@ __device__ __forceinline__ float beta_draw(float a, float b, float lo, float hi,
     v = lo + u * (hi - lo);
   }
   return v;
-}
-
-__global__ void __launch_bounds__(kThreads) k_beta(P c1, P c0, P low, P high, float* __restrict__ out,
-                                                    float* __restrict__ lp, int64_t n, uint64_t seed, uint64_t offset,
-                                                    int64_t first) {
-  PPB_GRID_LOOP(i) {
-    const float a = c1.at(i), b = c0.at(i), lo = low.at(i), hi = high.at(i);
-    const float v = beta_draw(a, b, lo, hi, seed, (uint64_t)(first + i), offset);
-    out[i] = v;
-    if (lp) lp[i] = fam::beta_lp(v, a, b, lo, hi, fam::beta_const(a, b));
-  }
 }
 
 // Binomial, drawn for q = min(p, 1 - p) and mirrored (n - k) for p > 1/2.
@@ -328,22 +217,11 @@ __device__ float binomial_draw(float nf, float p, uint64_t seed, uint64_t idx, u
   return (float)(flip ? n - k : k);
 }
 
-__global__ void __launch_bounds__(kThreads) k_binomial(P count, P probs, float* __restrict__ out, float* __restrict__ lp,
-                                                        int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
-  PPB_GRID_LOOP(i) {
-    const float nt = count.at(i), p = probs.at(i);
-    const float v = binomial_draw(nt, p, seed, (uint64_t)(first + i), offset);
-    out[i] = v;
-    if (lp) lp[i] = fam::binomial_lp(v, nt, p, fam::binomial_const(nt, p));
-  }
-}
-
 // VonMises: Best & Fisher (1979) rejection, in double precision as torch's VonMises.sample runs it (kappa (r - f)
 // cancels in fp32 at large kappa), then wrapped as torch does: (x + pi + loc) mod 2 pi - pi.  One round per Philox call.
 // The acceptance rate falls with kappa towards 0.658, so all kVonMisesCalls = 32 rounds fail with probability below
 // 0.343^32 < 1e-14 per draw; the draw then falls back to loc, deterministically.
 constexpr uint64_t kVonMisesCalls = 32;
-// k_von_mises's draw (see normal_draw)
 __device__ __forceinline__ float von_mises_draw(float locf, float kf, uint64_t seed, uint64_t idx, uint64_t offset) {
   const double kPi = 3.14159265358979323846;
   float v = NAN;
@@ -370,37 +248,45 @@ __device__ __forceinline__ float von_mises_draw(float locf, float kf, uint64_t s
   return v;
 }
 
-// The draw below is repeated in von_mises_draw (the event sampler's): change both together.  It stays spelled out here so
-// that this kernel's SASS is what it was before the event sampler existed; the test that element 0 of an event row is
-// this kernel's draw bit for bit ties the two.
-__global__ void __launch_bounds__(kThreads) k_von_mises(P loc, P conc, float* __restrict__ out, float* __restrict__ lp,
-                                                         int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
-  const double kPi = 3.14159265358979323846;
-  PPB_GRID_LOOP(i) {
-    const float locf = loc.at(i), kf = conc.at(i);
-    float v = NAN;
-    if (kf > 0.0f) {
-      const double kappa = kf;
-      const double tau = 1.0 + sqrt(1.0 + 4.0 * kappa * kappa);
-      const double rho = (tau - sqrt(2.0 * tau)) / (2.0 * kappa);
-      const double pr = (kappa < 1e-5) ? 1.0 / kappa + kappa : (1.0 + rho * rho) / (2.0 * rho);
-      double x = 0.0;
-      for (uint64_t call = 0; call < kVonMisesCalls; ++call) {
-        const ppb_philox r = philox_sub(seed, (uint64_t)(first + i), offset, call);
-        const double u1 = ppb_u01(r.c[0]), u2 = ppb_u01(r.c[1]), u3 = ppb_u01(r.c[2]);
-        const double z = cospi(u1);
-        const double f = fmin(fmax((1.0 + pr * z) / (pr + z), -1.0), 1.0);
-        const double c = kappa * (pr - f);
-        if (c * (2.0 - c) - u2 > 0.0 || log(c / u2) + 1.0 - c >= 0.0) {
-          x = (u3 > 0.5 ? 1.0 : u3 < 0.5 ? -1.0 : 0.0) * acos(f);
-          break;
-        }
-      }
-      const double y = x + kPi + (double)locf, two_pi = 2.0 * kPi;
-      v = (float)(y - two_pi * floor(y / two_pi) - kPi);
-    }
+// The draw of family FAMILY with parameters p (the PPB_EVENT_* order) from Philox index idx
+template <int FAMILY>
+__device__ __forceinline__ float family_draw(const float (&p)[4], uint64_t seed, uint64_t idx, uint64_t offset) {
+  switch (FAMILY) {
+    case PPB_EVENT_NORMAL: return normal_draw(ppb_philox4x32_10(seed, idx, offset), p[0], p[1]);
+    case PPB_EVENT_UNIFORM: return uniform_draw(ppb_philox4x32_10(seed, idx, offset), p[0], p[1]);
+    case PPB_EVENT_POISSON: return poisson_draw(p[0], seed, idx, offset);
+    case PPB_EVENT_BERNOULLI: return bernoulli_one(ppb_philox4x32_10(seed, idx, offset), p[0]) ? 1.0f : 0.0f;
+    case PPB_EVENT_EXPONENTIAL: return exponential_draw(ppb_philox4x32_10(seed, idx, offset), p[0]);
+    case PPB_EVENT_GAMMA: return gamma_draw(p[0], p[1], seed, idx, offset);
+    case PPB_EVENT_LOGNORMAL: return lognormal_draw(ppb_philox4x32_10(seed, idx, offset), p[0], p[1]);
+    case PPB_EVENT_WEIBULL: return weibull_draw(ppb_philox4x32_10(seed, idx, offset), p[0], p[1]);
+    case PPB_EVENT_BETA: return beta_draw(p[0], p[1], p[2], p[3], seed, idx, offset);
+    case PPB_EVENT_BINOMIAL: return binomial_draw(p[0], p[1], seed, idx, offset);
+    default: return von_mises_draw(p[0], p[1], seed, idx, offset);
+  }
+}
+
+// The eleven element-wise families at D = 1: particle i draws from Philox index first + i, and lp_out is the Op's value.
+struct Operands {
+  P p[4];
+};
+
+template <class Op>
+__global__ void __launch_bounds__(kThreads) k_sample(Operands q, float* __restrict__ out, float* __restrict__ lp,
+                                                      int64_t n, uint64_t seed, uint64_t offset, int64_t first) {
+  __shared__ float tab[Op::kTable ? 64 : 1];
+  if (Op::kTable) {
+    if (threadIdx.x < 64) tab[threadIdx.x] = c_log_factorial[threadIdx.x];
+    __syncthreads();
+  }
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    float p[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) p[k] = q.p[k < Op::kParams ? k : 0].at(i);
+    const float v = family_draw<Op::kFamily>(p, seed, (uint64_t)(first + i), offset);
     out[i] = v;
-    if (lp) lp[i] = fam::von_mises_lp(v, locf, kf, fam::von_mises_const(kf));
+    if (lp) lp[i] = Op{}(v, p, tab);   // a fresh Op: the draw dominates, and a parameter-only term kept across
+                                       // particles would only hold registers
   }
 }
 
@@ -486,7 +372,7 @@ struct EvP {
   __device__ __forceinline__ float at(int64_t i, int64_t j) const { return p ? __ldg(p + i * ps + j * es) : 0.0f; }
 };
 
-template <int FAMILY>
+template <class Op>
 __global__ void __launch_bounds__(kThreads) k_event_sample(EvP p0, EvP p1, EvP p2, EvP p3, float* __restrict__ out,
                                                             int64_t n, int64_t D, uint64_t seed, uint64_t offset,
                                                             int64_t first) {
@@ -494,139 +380,15 @@ __global__ void __launch_bounds__(kThreads) k_event_sample(EvP p0, EvP p1, EvP p
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
     const int64_t i = e / D, j = e - i * D;
     const uint64_t idx = (uint64_t)(first + i) | ((uint64_t)j << 40);
-    const float a = p0.at(i, j), b = p1.at(i, j);
-    float v;
-    switch (FAMILY) {
-      case PPB_EVENT_NORMAL: v = normal_draw(ppb_philox4x32_10(seed, idx, offset), a, b); break;
-      case PPB_EVENT_UNIFORM: v = uniform_draw(ppb_philox4x32_10(seed, idx, offset), a, b); break;
-      case PPB_EVENT_POISSON: v = poisson_draw(a, seed, idx, offset); break;
-      case PPB_EVENT_BERNOULLI: v = bernoulli_one(ppb_philox4x32_10(seed, idx, offset), a) ? 1.0f : 0.0f; break;
-      case PPB_EVENT_EXPONENTIAL: v = exponential_draw(ppb_philox4x32_10(seed, idx, offset), a); break;
-      case PPB_EVENT_GAMMA: v = gamma_draw(a, b, seed, idx, offset); break;
-      case PPB_EVENT_LOGNORMAL: v = lognormal_draw(ppb_philox4x32_10(seed, idx, offset), a, b); break;
-      case PPB_EVENT_WEIBULL: v = weibull_draw(ppb_philox4x32_10(seed, idx, offset), a, b); break;
-      case PPB_EVENT_BETA: v = beta_draw(a, b, p2.at(i, j), p3.at(i, j), seed, idx, offset); break;
-      case PPB_EVENT_BINOMIAL: v = binomial_draw(a, b, seed, idx, offset); break;
-      default: v = von_mises_draw(a, b, seed, idx, offset); break;
-    }
-    out[e] = v;
+    const float p[4] = {p0.at(i, j), p1.at(i, j), Op::kParams > 2 ? p2.at(i, j) : 0.0f,
+                        Op::kParams > 2 ? p3.at(i, j) : 0.0f};
+    out[e] = family_draw<Op::kFamily>(p, seed, idx, offset);
   }
 }
 
 }  // namespace
 
 extern "C" {
-
-int ppb_normal_sample(const float* mean, int mean_stride, const float* stddev, int stddev_stride, float* value_out,
-                      float* lp_out, int64_t n, uint64_t seed, uint64_t offset, int64_t first_index, void* stream) {
-  if (n == 0) return PPB_OK;
-  PPB_CHECK_ARG(n >= 0 && mean && stddev && value_out, "bad arguments");
-  if (n == 0) return PPB_OK;
-  k_normal<<<ppb_grid_for(n, kThreads, 1), kThreads, 0, (cudaStream_t)stream>>>(
-      P{mean, mean_stride}, P{stddev, stddev_stride}, value_out, lp_out, n, seed, offset, first_index);
-  PPB_LAUNCH_CHECK();
-  return PPB_OK;
-}
-
-int ppb_uniform_sample(const float* low, int low_stride, const float* high, int high_stride, float* value_out,
-                       float* lp_out, int64_t n, uint64_t seed, uint64_t offset, int64_t first_index, void* stream) {
-  if (n == 0) return PPB_OK;
-  PPB_CHECK_ARG(n >= 0 && low && high && value_out, "bad arguments");
-  if (n == 0) return PPB_OK;
-  k_uniform<<<ppb_grid_for(n, kThreads, 1), kThreads, 0, (cudaStream_t)stream>>>(
-      P{low, low_stride}, P{high, high_stride}, value_out, lp_out, n, seed, offset, first_index);
-  PPB_LAUNCH_CHECK();
-  return PPB_OK;
-}
-
-int ppb_poisson_sample(const float* rate, int rate_stride, float* value_out, float* lp_out, int64_t n, uint64_t seed,
-                       uint64_t offset, int64_t first_index, void* stream) {
-  if (n == 0) return PPB_OK;
-  PPB_CHECK_ARG(n >= 0 && rate && value_out, "bad arguments");
-  if (n == 0) return PPB_OK;
-  k_poisson<<<ppb_grid_for(n, kThreads, 1), kThreads, 0, (cudaStream_t)stream>>>(P{rate, rate_stride}, value_out,
-                                                                                 lp_out, n, seed, offset, first_index);
-  PPB_LAUNCH_CHECK();
-  return PPB_OK;
-}
-
-int ppb_bernoulli_sample(const float* probs, int probs_stride, float* value_out, float* lp_out, int64_t n, uint64_t seed,
-                         uint64_t offset, int64_t first_index, void* stream) {
-  if (n == 0) return PPB_OK;
-  PPB_CHECK_ARG(n >= 0 && probs && value_out, "bad arguments");
-  PPB_CHECK_ARG((probs_stride | 1) == 1, "strides must be 0 or 1");
-  k_bernoulli<<<ppb_grid_for(n, kThreads, 1), kThreads, 0, (cudaStream_t)stream>>>(P{probs, probs_stride}, value_out,
-                                                                                   lp_out, n, seed, offset, first_index);
-  PPB_LAUNCH_CHECK();
-  return PPB_OK;
-}
-
-#define PPB_LAUNCH_SAMPLER(kernel, ...)                                                                              \
-  do {                                                                                                               \
-    if (n == 0) return PPB_OK;                                                                                       \
-    kernel<<<ppb_grid_for(n, kThreads, 1), kThreads, 0, (cudaStream_t)stream>>>(__VA_ARGS__, value_out, lp_out, n,   \
-                                                                                 seed, offset, first_index);         \
-    PPB_LAUNCH_CHECK();                                                                                              \
-    return PPB_OK;                                                                                                   \
-  } while (0)
-
-int ppb_exponential_sample(const float* rate, int rate_stride, float* value_out, float* lp_out, int64_t n,
-                           uint64_t seed, uint64_t offset, int64_t first_index, void* stream) {
-  PPB_CHECK_ARG(n >= 0 && rate && value_out, "bad arguments");
-  PPB_CHECK_ARG((rate_stride | 1) == 1, "strides must be 0 or 1");
-  PPB_LAUNCH_SAMPLER(k_exponential, P{rate, rate_stride});
-}
-
-int ppb_gamma_sample(const float* concentration, int concentration_stride, const float* rate, int rate_stride,
-                     float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset, int64_t first_index,
-                     void* stream) {
-  PPB_CHECK_ARG(n >= 0 && concentration && rate && value_out, "bad arguments");
-  PPB_CHECK_ARG((concentration_stride | 1) == 1 && (rate_stride | 1) == 1, "strides must be 0 or 1");
-  PPB_LAUNCH_SAMPLER(k_gamma, P{concentration, concentration_stride}, P{rate, rate_stride});
-}
-
-int ppb_lognormal_sample(const float* loc, int loc_stride, const float* scale, int scale_stride, float* value_out,
-                         float* lp_out, int64_t n, uint64_t seed, uint64_t offset, int64_t first_index, void* stream) {
-  PPB_CHECK_ARG(n >= 0 && loc && scale && value_out, "bad arguments");
-  PPB_CHECK_ARG((loc_stride | 1) == 1 && (scale_stride | 1) == 1, "strides must be 0 or 1");
-  PPB_LAUNCH_SAMPLER(k_lognormal, P{loc, loc_stride}, P{scale, scale_stride});
-}
-
-int ppb_weibull_sample(const float* scale, int scale_stride, const float* concentration, int concentration_stride,
-                       float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset, int64_t first_index,
-                       void* stream) {
-  PPB_CHECK_ARG(n >= 0 && scale && concentration && value_out, "bad arguments");
-  PPB_CHECK_ARG((scale_stride | 1) == 1 && (concentration_stride | 1) == 1, "strides must be 0 or 1");
-  PPB_LAUNCH_SAMPLER(k_weibull, P{scale, scale_stride}, P{concentration, concentration_stride});
-}
-
-int ppb_beta_sample(const float* concentration1, int concentration1_stride, const float* concentration0,
-                    int concentration0_stride, const float* low, int low_stride, const float* high, int high_stride,
-                    float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset, int64_t first_index,
-                    void* stream) {
-  PPB_CHECK_ARG(n >= 0 && concentration1 && concentration0 && low && high && value_out, "bad arguments");
-  PPB_CHECK_ARG((concentration1_stride | 1) == 1 && (concentration0_stride | 1) == 1 && (low_stride | 1) == 1 &&
-                    (high_stride | 1) == 1,
-                "strides must be 0 or 1");
-  PPB_LAUNCH_SAMPLER(k_beta, P{concentration1, concentration1_stride}, P{concentration0, concentration0_stride},
-                     P{low, low_stride}, P{high, high_stride});
-}
-
-int ppb_binomial_sample(const float* total_count, int total_count_stride, const float* probs, int probs_stride,
-                        float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset,
-                        int64_t first_index, void* stream) {
-  PPB_CHECK_ARG(n >= 0 && total_count && probs && value_out, "bad arguments");
-  PPB_CHECK_ARG((total_count_stride | 1) == 1 && (probs_stride | 1) == 1, "strides must be 0 or 1");
-  PPB_LAUNCH_SAMPLER(k_binomial, P{total_count, total_count_stride}, P{probs, probs_stride});
-}
-
-int ppb_von_mises_sample(const float* loc, int loc_stride, const float* concentration, int concentration_stride,
-                         float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset,
-                         int64_t first_index, void* stream) {
-  PPB_CHECK_ARG(n >= 0 && loc && concentration && value_out, "bad arguments");
-  PPB_CHECK_ARG((loc_stride | 1) == 1 && (concentration_stride | 1) == 1, "strides must be 0 or 1");
-  PPB_LAUNCH_SAMPLER(k_von_mises, P{loc, loc_stride}, P{concentration, concentration_stride});
-}
 
 int ppb_categorical_sample(const float* probs, int64_t probs_row_stride, int num_categories, float* value_out,
                            float* lp_out, int64_t n, uint64_t seed, uint64_t offset, int64_t first_index,
@@ -668,54 +430,73 @@ int ppb_mixture_truncated_normal_sample(const float* means, const float* stddevs
   return PPB_OK;
 }
 
+}  // extern "C"
+
+namespace {
+
+int event_sample(int family, const float* const* p, const int64_t* ps, const int64_t* es, float* value_out,
+                 float* lp_out, int64_t n, int64_t D, uint64_t seed, uint64_t offset, int64_t first_index,
+                 void* stream) {
+  const int np = ppb_event_num_params(family);
+  PPB_CHECK_ARG(np > 0, "unknown family id");
+  PPB_CHECK_ARG(n >= 0 && D > 0, "n must be >= 0 and D > 0");
+  PPB_CHECK_ARG(D <= ((int64_t)1 << 24), "D > 2^24: the element index does not fit Philox counter bits 40 .. 63");
+  PPB_CHECK_ARG(first_index >= 0 && first_index + n <= ((int64_t)1 << 40),
+                "first_index + n > 2^40: the particle index does not fit Philox counter bits 0 .. 39");
+  if (n == 0) return PPB_OK;
+  PPB_CHECK_ARG(value_out, "value_out is null");
+  EvP q[4] = {};
+  for (int k = 0; k < np; ++k) {
+    PPB_CHECK_ARG(p[k] && ((ps[k] == 0 && es[k] == 0) || (ps[k] == 1 && es[k] == 0) || (ps[k] == 0 && es[k] == 1) ||
+                           (ps[k] == D && es[k] == 1)),
+                  "parameter: null pointer, or strides not one of (0, 0), (1, 0), (0, 1), (D, 1)");
+    q[k] = EvP{p[k], ps[k], es[k]};
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  return ppb_with_family(family, [&](auto op) {
+    using Op = decltype(op);
+    if (D == 1) {   // one draw per particle, its log_prob fused (every operand is flat with stride ps, 0 or 1)
+      if (Op::kTable && lp_out) {
+        const int e = ppb_upload_log_factorial();
+        if (e != PPB_OK) return e;
+      }
+      Operands f;
+      for (int k = 0; k < 4; ++k) f.p[k] = P{q[k].p, (int)q[k].ps};
+      k_sample<Op><<<ppb_grid_for(n, kThreads, 1), kThreads, 0, st>>>(f, value_out, lp_out, n, seed, offset,
+                                                                        first_index);
+      PPB_LAUNCH_CHECK();
+      return PPB_OK;
+    }
+    k_event_sample<Op><<<ppb_grid_for(n * D, kThreads, 1), kThreads, 0, st>>>(q[0], q[1], q[2], q[3], value_out, n, D,
+                                                                                seed, offset, first_index);
+    PPB_LAUNCH_CHECK();
+    if (!lp_out) return PPB_OK;
+    // lp_out: the scoring kernel's row sums over the drawn rows (value operand (D, 1))
+    return ppb_event_score(family, value_out, D, 1, p, ps, es, n, D, nullptr, lp_out, nullptr, 0.0, stream);
+  });
+}
+
+}  // namespace
+
+extern "C" {
+
 int ppb_event_sample(int family, const float* p0, int64_t p0_ps, int64_t p0_es, const float* p1, int64_t p1_ps,
                      int64_t p1_es, const float* p2, int64_t p2_ps, int64_t p2_es, const float* p3, int64_t p3_ps,
                      int64_t p3_es, float* value_out, float* lp_out, int64_t n, int64_t D, uint64_t seed,
                      uint64_t offset, int64_t first_index, void* stream) {
-  const int np = ppb_event_num_params(family);
-  PPB_CHECK_ARG(np > 0, "unknown family id");
-  PPB_CHECK_ARG(n >= 0 && D > 0 && value_out, "n must be >= 0, D > 0 and value_out non-null");
-  PPB_CHECK_ARG(D <= ((int64_t)1 << 24), "D > 2^24: the element index does not fit Philox counter bits 40 .. 63");
-  PPB_CHECK_ARG(first_index >= 0 && first_index + n <= ((int64_t)1 << 40),
-                "first_index + n > 2^40: the particle index does not fit Philox counter bits 0 .. 39");
   const float* p[4] = {p0, p1, p2, p3};
   const int64_t ps[4] = {p0_ps, p1_ps, p2_ps, p3_ps}, es[4] = {p0_es, p1_es, p2_es, p3_es};
-  EvP q[4];
-  for (int k = 0; k < 4; ++k) {
-    if (k < np) {
-      PPB_CHECK_ARG(p[k] && ((ps[k] == 0 && es[k] == 0) || (ps[k] == 1 && es[k] == 0) || (ps[k] == 0 && es[k] == 1) ||
-                             (ps[k] == D && es[k] == 1)),
-                    "parameter: null pointer, or strides not one of (0, 0), (1, 0), (0, 1), (D, 1)");
-      q[k] = EvP{p[k], ps[k], es[k]};
-    } else {
-      q[k] = EvP{nullptr, 0, 0};
-    }
-  }
-  if (n == 0) return PPB_OK;
-  cudaStream_t st = (cudaStream_t)stream;
-  const int grid = ppb_grid_for(n * D, kThreads, 1);
-#define PPB_EVENT_CASE(F)                                                                                       \
-  case F:                                                                                                       \
-    k_event_sample<F><<<grid, kThreads, 0, st>>>(q[0], q[1], q[2], q[3], value_out, n, D, seed, offset, first_index); \
-    break;
-  switch (family) {
-    PPB_EVENT_CASE(PPB_EVENT_NORMAL)
-    PPB_EVENT_CASE(PPB_EVENT_UNIFORM)
-    PPB_EVENT_CASE(PPB_EVENT_POISSON)
-    PPB_EVENT_CASE(PPB_EVENT_BERNOULLI)
-    PPB_EVENT_CASE(PPB_EVENT_EXPONENTIAL)
-    PPB_EVENT_CASE(PPB_EVENT_GAMMA)
-    PPB_EVENT_CASE(PPB_EVENT_LOGNORMAL)
-    PPB_EVENT_CASE(PPB_EVENT_WEIBULL)
-    PPB_EVENT_CASE(PPB_EVENT_BETA)
-    PPB_EVENT_CASE(PPB_EVENT_BINOMIAL)
-    default: PPB_EVENT_CASE(PPB_EVENT_VON_MISES)
-  }
-#undef PPB_EVENT_CASE
-  PPB_LAUNCH_CHECK();
-  if (!lp_out) return PPB_OK;
-  // lp_out: the scoring kernel's row sums over the drawn rows (value operand (D, 1))
-  return ppb_event_score(family, value_out, D, 1, p, ps, es, n, D, nullptr, lp_out, nullptr, 0.0, stream);
+  return event_sample(family, p, ps, es, value_out, lp_out, n, D, seed, offset, first_index, stream);
+}
+
+int ppb_event_sample_d1(int family, const float* p0, const float* p1, const float* p2, const float* p3,
+                        int param_strides, float* value_out, float* lp_out, int64_t n, uint64_t seed, uint64_t offset,
+                        int64_t first_index, void* stream) {
+  const float* p[4] = {p0, p1, p2, p3};
+  const int64_t ps[4] = {param_strides & 1, (param_strides >> 1) & 1, (param_strides >> 2) & 1,
+                         (param_strides >> 3) & 1};
+  const int64_t es[4] = {0, 0, 0, 0};
+  return event_sample(family, p, ps, es, value_out, lp_out, n, 1, seed, offset, first_index, stream);
 }
 
 }  // extern "C"

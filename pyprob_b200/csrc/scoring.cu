@@ -61,104 +61,14 @@ struct Sink {
   bool vec_ok() const { return (!lp || ((((uintptr_t)lp) & 15u) == 0)) && (!acc || ((((uintptr_t)acc) & 15u) == 0)); }
 };
 
-// ---- two-parameter families ---------------------------------------------------------------------
-// MUFU approximations (<= 2 ulp): the scoring kernels are bound by instruction issue, not HBM, as soon as they carry an IEEE
-// division or a libm logf/expf; results stay within 1e-6 relative of the libm forms.
-__device__ __forceinline__ float fast_rcp(float x) { float r; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
-__device__ __forceinline__ float fast_ex2(float x) { float r; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
-__device__ __forceinline__ float fast_lg2(float x) { float r; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
-
-struct NormalOp {
-  static constexpr bool kTable = false;
-  // torch/distributions/normal.py log_prob: -((v - mu)^2) / (2 var) - log(sigma) - log(sqrt(2 pi))
-  __device__ __forceinline__ float operator()(float v, float mu, float sigma, const float*) const {
-    const float z = (v - mu) * fast_rcp(sigma);
-    return fmaf(-0.5f * z, z, -fast_lg2(sigma) * PPB_LN2) - PPB_LOG_SQRT_2PI;
-  }
-};
-struct UniformOp {
-  // torch/distributions/uniform.py log_prob: log(lb*ub) - log(high-low), lb = low<=v, ub = high>v
-  static constexpr bool kTable = false;
-  __device__ __forceinline__ float operator()(float v, float lo, float hi, const float*) const {
-    float inside = (lo <= v && hi > v) ? 0.0f : -INFINITY;
-    return inside - logf(hi - lo);
-  }
-};
-// log(k!) for the counts that actually occur (k < 64), correctly rounded from the double-precision lgamma: lgammaf costs
-// ~40 instructions per particle and made the Poisson kernel ALU-bound at 39 % of HBM; other values take lgammaf.
-// The table is copied to shared memory by every CTA: the lanes of a warp hold different counts, and a constant-bank read
-// with divergent indices is replayed once per distinct address (63 % of HBM), shared memory serves them in one pass.
-__constant__ float c_log_factorial[64];
-struct PoissonOp {
-  static constexpr bool kTable = true;
-  // torch/distributions/poisson.py log_prob: xlogy(v, rate) - rate - lgamma(v+1)
-  __device__ __forceinline__ float operator()(float v, float rate, float, const float* tab) const {
-    float xl = (v == 0.0f) ? 0.0f : v * (fast_lg2(rate) * PPB_LN2);
-    const int k = (int)v;
-    const float lg = (v >= 0.0f && v < 64.0f && (float)k == v) ? tab[k] : lgammaf(v + 1.0f);
-    return xl - rate - lg;
-  }
-};
-struct BernoulliOp {
-  static constexpr bool kTable = false;
-  // torch/distributions/bernoulli.py log_prob: -BCEWithLogits(log pc - log1p(-pc), v) = v log pc + (1 - v) log(1 - pc),
-  // pc = clamp_probs(p); values outside {0, 1} are rejected by the reference's argument validation: NaN here
-  __device__ __forceinline__ float operator()(float v, float p, float, const float*) const {
-    const float pc = ppb_clamp_prob(p);
-    return (v == 1.0f) ? logf(pc) : (v == 0.0f) ? log1pf(-pc) : NAN;
-  }
-};
-
-// Exponential .. VonMises (families.cuh).  An Op whose log_prob has a term that depends on the parameters only keeps it
-// in the thread together with the parameters it was computed for, and recomputes it only when they change: with shared
-// (stride-0) parameters that is once per thread instead of once per particle (lgammaf alone is ~40 instructions).
-struct ExponentialOp {
-  static constexpr bool kTable = false;
-  __device__ __forceinline__ float operator()(float v, float rate, float, const float*) const {
-    return fam::exponential_lp(v, rate);
-  }
-};
-struct GammaOp {
-  static constexpr bool kTable = false;
-  float c_ = NAN, r_ = NAN, k_ = NAN;
-  __device__ __forceinline__ float operator()(float v, float c, float r, const float*) {
-    if (!(c == c_ && r == r_)) { c_ = c; r_ = r; k_ = fam::gamma_const(c, r); }
-    return fam::gamma_lp(v, c, r, k_);
-  }
-};
-struct LogNormalOp {
-  static constexpr bool kTable = false;
-  __device__ __forceinline__ float operator()(float v, float mu, float s, const float*) const {
-    return fam::lognormal_lp(v, mu, s);
-  }
-};
-struct WeibullOp {
-  static constexpr bool kTable = false;
-  __device__ __forceinline__ float operator()(float v, float scale, float k, const float*) const {
-    return fam::weibull_lp(v, scale, k);
-  }
-};
-struct BinomialOp {
-  static constexpr bool kTable = false;
-  float n_ = NAN, p_ = NAN;
-  fam::BinomialConst k_{NAN, NAN};
-  __device__ __forceinline__ float operator()(float v, float n, float p, const float*) {
-    if (!(n == n_ && p == p_)) { n_ = n; p_ = p; k_ = fam::binomial_const(n, p); }
-    return fam::binomial_lp(v, n, p, k_);
-  }
-};
-struct VonMisesOp {
-  static constexpr bool kTable = false;
-  float kappa_ = NAN, k_ = NAN;
-  __device__ __forceinline__ float operator()(float v, float loc, float kappa, const float*) {
-    if (!(kappa == kappa_)) { kappa_ = kappa; k_ = fam::von_mises_const(kappa); }
-    return fam::von_mises_lp(v, loc, kappa, k_);
-  }
+// ---- the eleven element-wise families at D = 1: one particle-flat kernel over the Ops of families.cuh ---------------------
+// The value and each of the Op::kParams parameters is a scalar (stride 0) or one per particle (stride 1).
+struct Operands {
+  Param p[4];
 };
 
 template <class Op, bool VEC>
-__global__ void __launch_bounds__(kThreads) k_score2(const float* __restrict__ value, Param a, Param b, Sink out,
-                                                      int64_t n, Op op) {
+__global__ void __launch_bounds__(kThreads) k_score2(Param value, Operands q, Sink out, int64_t n, Op op) {
   __shared__ float tab[Op::kTable ? 64 : 1];
   if (Op::kTable) {
     if (threadIdx.x < 64) tab[threadIdx.x] = c_log_factorial[threadIdx.x];
@@ -166,70 +76,46 @@ __global__ void __launch_bounds__(kThreads) k_score2(const float* __restrict__ v
   }
   int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   int64_t nth = (int64_t)gridDim.x * blockDim.x;
-  if (VEC) {
-    int64_t n4 = n >> 2;
-    for (int64_t q = tid; q < n4; q += nth) {
-      int64_t i = q << 2;
-      float4 vv = ldg_stream4(value + i);
-      float v[4] = {vv.x, vv.y, vv.z, vv.w};
-      float pa[4], pb[4], r[4];
-      a.load4(i, pa);
-      b.load4(i, pb);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) r[j] = op(v[j], pa[j], pb[j], tab);
-      out.put4(i, r);
-    }
-    for (int64_t i = (n4 << 2) + tid; i < n; i += nth) out.put(i, op(__ldg(value + i), a.at(i), b.at(i), tab));
-  } else {
-    for (int64_t i = tid; i < n; i += nth) out.put(i, op(__ldg(value + i), a.at(i), b.at(i), tab));
-  }
-}
-
-template <class Op>
-int launch_score2(const float* value, Param a, Param b, Sink out, int64_t n, void* stream, Op op) {
-  if (n == 0) return PPB_OK;
-  bool vec = aligned16(value) && a.vec_ok() && b.vec_ok() && out.vec_ok();
-  cudaStream_t st = (cudaStream_t)stream;
-  int grid = ppb_grid_for(n, kThreads, 4);
-  if (vec)
-    k_score2<Op, true><<<grid, kThreads, 0, st>>>(value, a, b, out, n, op);
-  else
-    k_score2<Op, false><<<grid, kThreads, 0, st>>>(value, a, b, out, n, op);
-  PPB_LAUNCH_CHECK();
-  return PPB_OK;
-}
-
-// ---- beta (four parameters) ----------------------------------------------------------------------------------------------
-// lbeta(c1, c0) is kept per thread while (c1, c0) repeat, as in the Ops above
-template <bool VEC>
-__global__ void __launch_bounds__(kThreads) k_beta(const float* __restrict__ value, Param c1, Param c0, Param low,
-                                                    Param high, Sink out, int64_t n) {
-  int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  int64_t nth = (int64_t)gridDim.x * blockDim.x;
-  float a_ = NAN, b_ = NAN, k_ = NAN;
-  auto lp = [&](float v, float a, float b, float lo, float hi) {
-    if (!(a == a_ && b == b_)) { a_ = a; b_ = b; k_ = fam::beta_const(a, b); }
-    return fam::beta_lp(v, a, b, lo, hi, k_);
-  };
   int64_t i0 = 0;
   if (VEC) {
     int64_t n4 = n >> 2;
-    for (int64_t q = tid; q < n4; q += nth) {
-      int64_t i = q << 2;
-      float4 vv = ldg_stream4(value + i);
-      float v[4] = {vv.x, vv.y, vv.z, vv.w};
-      float pa[4], pb[4], pl[4], ph[4], r[4];
-      c1.load4(i, pa);
-      c0.load4(i, pb);
-      low.load4(i, pl);
-      high.load4(i, ph);
+    for (int64_t q4 = tid; q4 < n4; q4 += nth) {
+      int64_t i = q4 << 2;
+      const float4 vv = ldg_stream4(value.p + i);   // VEC: the value is one per particle
+      const float v[4] = {vv.x, vv.y, vv.z, vv.w};
+      float p[Op::kParams][4], r[4];
 #pragma unroll
-      for (int j = 0; j < 4; ++j) r[j] = lp(v[j], pa[j], pb[j], pl[j], ph[j]);
+      for (int k = 0; k < Op::kParams; ++k) q.p[k].load4(i, p[k]);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        float pj[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) pj[k] = p[k < Op::kParams ? k : 0][j];
+        r[j] = op(v[j], pj, tab);
+      }
       out.put4(i, r);
     }
     i0 = n4 << 2;
   }
-  for (int64_t i = i0 + tid; i < n; i += nth) out.put(i, lp(__ldg(value + i), c1.at(i), c0.at(i), low.at(i), high.at(i)));
+  for (int64_t i = i0 + tid; i < n; i += nth) {
+    float p[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) p[k] = q.p[k < Op::kParams ? k : 0].at(i);
+    out.put(i, op(value.at(i), p, tab));
+  }
+}
+
+template <class Op>
+int launch_score2(Param value, const Operands& q, Sink out, int64_t n, cudaStream_t st) {
+  bool vec = value.stride == 1 && value.vec_ok() && out.vec_ok();
+  for (int k = 0; k < Op::kParams; ++k) vec = vec && q.p[k].vec_ok();
+  const int grid = ppb_grid_for(n, kThreads, 4);
+  if (vec)
+    k_score2<Op, true><<<grid, kThreads, 0, st>>>(value, q, out, n, Op{});
+  else
+    k_score2<Op, false><<<grid, kThreads, 0, st>>>(value, q, out, n, Op{});
+  PPB_LAUNCH_CHECK();
+  return PPB_OK;
 }
 
 // ---- categorical --------------------------------------------------------------------------------
@@ -367,7 +253,8 @@ int launch_mixture(const float* value, const float* means, const float* stddevs,
 // four 32-bit loads elsewhere.  Per-particle rows stream past L1; a shared event row is read through L1 / L2.
 // Each lane sums its elements in fp64 in element order, and the group combines its lanes with a fixed butterfly: the
 // order depends on (n, D) only (G is a function of D; the load width does not change what is summed), so a call is
-// bit-reproducible, and with D = 1 the sum is the single term, exactly k_score2's accumulator update.
+// bit-reproducible.  Each element is the Op's value, as k_score2 gives it for a particle; ppb_event_score runs D = 1 on
+// k_score2, whose accumulator update is this kernel's at D = 1 (the fp64 sum of a single term).
 struct EvOperand {
   const float* p;
   int64_t ps, es;
@@ -399,28 +286,11 @@ struct EvArgs {
   int64_t n, D;
 };
 
-// (value, parameter vector) -> log-density, over the two-parameter Ops (one-parameter families ignore p[1])
-template <class Op>
-struct EvFamily {
-  static constexpr bool kTable = Op::kTable;
-  Op op;
-  __device__ __forceinline__ float operator()(float v, const float (&p)[4], const float* tab) {
-    return op(v, p[0], p[1], tab);
-  }
-};
-struct EvBeta {
-  static constexpr bool kTable = false;
-  float a_ = NAN, b_ = NAN, k_ = NAN;
-  __device__ __forceinline__ float operator()(float v, const float (&p)[4], const float*) {
-    if (!(p[0] == a_ && p[1] == b_)) { a_ = p[0]; b_ = p[1]; k_ = fam::beta_const(p[0], p[1]); }
-    return fam::beta_lp(v, p[0], p[1], p[2], p[3], k_);
-  }
-};
-
-template <class F, int NP, int G>
-__global__ void __launch_bounds__(kThreads) k_event(EvArgs a, F f) {
-  __shared__ float tab[F::kTable ? 64 : 1];
-  if (F::kTable) {
+template <class Op, int G>
+__global__ void __launch_bounds__(kThreads) k_event(EvArgs a, Op op) {
+  constexpr int NP = Op::kParams;
+  __shared__ float tab[Op::kTable ? 64 : 1];
+  if (Op::kTable) {
     if (threadIdx.x < 64) tab[threadIdx.x] = c_log_factorial[threadIdx.x];
     __syncthreads();
   }
@@ -444,7 +314,7 @@ __global__ void __launch_bounds__(kThreads) k_event(EvArgs a, F f) {
           float pe[4];
 #pragma unroll
           for (int k = 0; k < 4; ++k) pe[k] = p[k < NP ? k : 0][e];
-          r[e] = f(v[e], pe, tab);
+          r[e] = op(v[e], pe, tab);
         }
         const int m = (D - j0 < 4) ? (int)(D - j0) : 4;
 #pragma unroll
@@ -471,33 +341,21 @@ __global__ void __launch_bounds__(kThreads) k_event(EvArgs a, F f) {
   }
 }
 
-template <class F, int NP>
-int launch_event(const EvArgs& a, cudaStream_t st, F f) {
+template <class Op>
+int launch_event(const EvArgs& a, cudaStream_t st) {
   const int64_t chunks = (a.D + 3) >> 2;
   int g = 1;
   while (g < chunks && g < 32) g <<= 1;
   const int grid = ppb_grid_for(a.n, kThreads / g, 1);
   switch (g) {
-    case 1: k_event<F, NP, 1><<<grid, kThreads, 0, st>>>(a, f); break;
-    case 2: k_event<F, NP, 2><<<grid, kThreads, 0, st>>>(a, f); break;
-    case 4: k_event<F, NP, 4><<<grid, kThreads, 0, st>>>(a, f); break;
-    case 8: k_event<F, NP, 8><<<grid, kThreads, 0, st>>>(a, f); break;
-    case 16: k_event<F, NP, 16><<<grid, kThreads, 0, st>>>(a, f); break;
-    default: k_event<F, NP, 32><<<grid, kThreads, 0, st>>>(a, f); break;
+    case 1: k_event<Op, 1><<<grid, kThreads, 0, st>>>(a, Op{}); break;
+    case 2: k_event<Op, 2><<<grid, kThreads, 0, st>>>(a, Op{}); break;
+    case 4: k_event<Op, 4><<<grid, kThreads, 0, st>>>(a, Op{}); break;
+    case 8: k_event<Op, 8><<<grid, kThreads, 0, st>>>(a, Op{}); break;
+    case 16: k_event<Op, 16><<<grid, kThreads, 0, st>>>(a, Op{}); break;
+    default: k_event<Op, 32><<<grid, kThreads, 0, st>>>(a, Op{}); break;
   }
   PPB_LAUNCH_CHECK();
-  return PPB_OK;
-}
-
-// c_log_factorial, uploaded once per process by the first Poisson log_prob call (per-particle or event)
-int upload_log_factorial() {
-  static bool table_ready = false;
-  if (!table_ready) {
-    float t[64];
-    for (int k = 0; k < 64; ++k) t[k] = (float)lgamma((double)k + 1.0);
-    PPB_CUDA(cudaMemcpyToSymbol(c_log_factorial, t, sizeof(t)));
-    table_ready = true;
-  }
   return PPB_OK;
 }
 
@@ -507,60 +365,35 @@ bool ev_layout_ok(const void* p, int64_t ps, int64_t es, int64_t D) {
 
 }  // namespace
 
-int ppb_event_num_params(int family) {
-  switch (family) {
-    case PPB_EVENT_POISSON: case PPB_EVENT_BERNOULLI: case PPB_EVENT_EXPONENTIAL: return 1;
-    case PPB_EVENT_BETA: return 4;
-    case PPB_EVENT_NORMAL: case PPB_EVENT_UNIFORM: case PPB_EVENT_GAMMA: case PPB_EVENT_LOGNORMAL:
-    case PPB_EVENT_WEIBULL: case PPB_EVENT_BINOMIAL: case PPB_EVENT_VON_MISES: return 2;
-    default: return -1;
-  }
-}
-
 int ppb_event_score(int family, const float* value, int64_t value_ps, int64_t value_es, const float* const* params,
                     const int64_t* params_ps, const int64_t* params_es, int64_t n, int64_t D, float* lp_out,
                     float* row_lp, double* acc, double acc_scale, void* stream) {
   const int np = ppb_event_num_params(family);
   PPB_CHECK_ARG(np > 0, "unknown family id");
   PPB_CHECK_ARG(n >= 0 && D > 0, "n must be >= 0 and D > 0");
+  PPB_CHECK_ARG(D > 1 || !row_lp, "row_lp at D = 1: a row's sum is its one element, lp_out");
+  if (n == 0) return PPB_OK;
   PPB_CHECK_ARG(ev_layout_ok(value, value_ps, value_es, D),
                 "value: null pointer, or strides not one of (0, 0), (1, 0), (0, 1), (D, 1)");
-  EvArgs a;
-  a.v = EvOperand{value, value_ps, value_es};
-  for (int k = 0; k < 4; ++k) {
-    if (k < np) {
-      PPB_CHECK_ARG(ev_layout_ok(params[k], params_ps[k], params_es[k], D),
-                    "parameter: null pointer, or strides not one of (0, 0), (1, 0), (0, 1), (D, 1)");
-      a.p[k] = EvOperand{params[k], params_ps[k], params_es[k]};
-    } else {
-      a.p[k] = EvOperand{nullptr, 0, 0};
-    }
+  EvArgs a{EvOperand{value, value_ps, value_es}, {}, lp_out, row_lp, acc, acc_scale, n, D};
+  for (int k = 0; k < np; ++k) {
+    PPB_CHECK_ARG(ev_layout_ok(params[k], params_ps[k], params_es[k], D),
+                  "parameter: null pointer, or strides not one of (0, 0), (1, 0), (0, 1), (D, 1)");
+    a.p[k] = EvOperand{params[k], params_ps[k], params_es[k]};
   }
-  if (n == 0) return PPB_OK;
-  a.lp = lp_out;
-  a.row_lp = row_lp;
-  a.acc = acc;
-  a.scale = acc_scale;
-  a.n = n;
-  a.D = D;
   cudaStream_t st = (cudaStream_t)stream;
-  switch (family) {
-    case PPB_EVENT_NORMAL: return launch_event<EvFamily<NormalOp>, 2>(a, st, {});
-    case PPB_EVENT_UNIFORM: return launch_event<EvFamily<UniformOp>, 2>(a, st, {});
-    case PPB_EVENT_POISSON: {
-      const int e = upload_log_factorial();
+  return ppb_with_family(family, [&](auto op) {
+    using Op = decltype(op);
+    if (Op::kTable) {
+      const int e = ppb_upload_log_factorial();
       if (e != PPB_OK) return e;
-      return launch_event<EvFamily<PoissonOp>, 1>(a, st, {});
     }
-    case PPB_EVENT_BERNOULLI: return launch_event<EvFamily<BernoulliOp>, 1>(a, st, {});
-    case PPB_EVENT_EXPONENTIAL: return launch_event<EvFamily<ExponentialOp>, 1>(a, st, {});
-    case PPB_EVENT_GAMMA: return launch_event<EvFamily<GammaOp>, 2>(a, st, {});
-    case PPB_EVENT_LOGNORMAL: return launch_event<EvFamily<LogNormalOp>, 2>(a, st, {});
-    case PPB_EVENT_WEIBULL: return launch_event<EvFamily<WeibullOp>, 2>(a, st, {});
-    case PPB_EVENT_BETA: return launch_event<EvBeta, 4>(a, st, {});
-    case PPB_EVENT_BINOMIAL: return launch_event<EvFamily<BinomialOp>, 2>(a, st, {});
-    default: return launch_event<EvFamily<VonMisesOp>, 2>(a, st, {});
-  }
+    if (D > 1) return launch_event<Op>(a, st);
+    // D = 1: every operand is flat with stride ps (0 or 1), and each row one particle's element
+    Operands q;
+    for (int k = 0; k < 4; ++k) q.p[k] = Param{a.p[k].p, (int)a.p[k].ps};
+    return launch_score2<Op>(Param{value, (int)value_ps}, q, Sink{lp_out, acc, acc_scale}, n, st);
+  });
 }
 
 extern "C" {
@@ -574,120 +407,14 @@ int ppb_event_log_prob(int family, const float* value, int64_t value_ps, int64_t
   return ppb_event_score(family, value, value_ps, value_es, p, ps, es, n, D, lp_out, nullptr, acc, acc_scale, stream);
 }
 
-int ppb_normal_log_prob(const float* value, const float* mean, int mean_stride, const float* stddev,
-                        int stddev_stride, float* lp_out, double* acc, double acc_scale, int64_t n, void* stream) {
-  if (n == 0) return PPB_OK;
-  PPB_CHECK_ARG(n >= 0 && value && mean && stddev, "null pointer or negative n");
-  PPB_CHECK_ARG((mean_stride | 1) == 1 && (stddev_stride | 1) == 1, "strides must be 0 or 1");
-  return launch_score2(value, Param{mean, mean_stride}, Param{stddev, stddev_stride}, Sink{lp_out, acc, acc_scale}, n,
-                       stream, NormalOp{});
-}
-
-int ppb_uniform_log_prob(const float* value, const float* low, int low_stride, const float* high, int high_stride,
-                         float* lp_out, double* acc, double acc_scale, int64_t n, void* stream) {
-  if (n == 0) return PPB_OK;
-  PPB_CHECK_ARG(n >= 0 && value && low && high, "null pointer or negative n");
-  PPB_CHECK_ARG((low_stride | 1) == 1 && (high_stride | 1) == 1, "strides must be 0 or 1");
-  return launch_score2(value, Param{low, low_stride}, Param{high, high_stride}, Sink{lp_out, acc, acc_scale}, n, stream,
-                       UniformOp{});
-}
-
-int ppb_poisson_log_prob(const float* value, const float* rate, int rate_stride, float* lp_out, double* acc,
-                         double acc_scale, int64_t n, void* stream) {
-  if (n == 0) return PPB_OK;
-  PPB_CHECK_ARG(n >= 0 && value && rate, "null pointer or negative n");
-  PPB_CHECK_ARG((rate_stride | 1) == 1, "strides must be 0 or 1");
-  const int e = upload_log_factorial();
-  if (e != PPB_OK) return e;
-  return launch_score2(value, Param{rate, rate_stride}, Param{rate, 0}, Sink{lp_out, acc, acc_scale}, n, stream,
-                       PoissonOp{});
-}
-
-int ppb_bernoulli_log_prob(const float* value, const float* probs, int probs_stride, float* lp_out, double* acc,
-                           double acc_scale, int64_t n, void* stream) {
-  if (n == 0) return PPB_OK;
-  PPB_CHECK_ARG(n >= 0 && value && probs, "null pointer or negative n");
-  PPB_CHECK_ARG((probs_stride | 1) == 1, "strides must be 0 or 1");
-  return launch_score2(value, Param{probs, probs_stride}, Param{probs, 0}, Sink{lp_out, acc, acc_scale}, n, stream,
-                       BernoulliOp{});
-}
-
-int ppb_exponential_log_prob(const float* value, const float* rate, int rate_stride, float* lp_out, double* acc,
-                             double acc_scale, int64_t n, void* stream) {
-  if (n == 0) return PPB_OK;
-  PPB_CHECK_ARG(n >= 0 && value && rate, "null pointer or negative n");
-  PPB_CHECK_ARG((rate_stride | 1) == 1, "strides must be 0 or 1");
-  return launch_score2(value, Param{rate, rate_stride}, Param{rate, 0}, Sink{lp_out, acc, acc_scale}, n, stream,
-                       ExponentialOp{});
-}
-
-int ppb_gamma_log_prob(const float* value, const float* concentration, int concentration_stride, const float* rate,
-                       int rate_stride, float* lp_out, double* acc, double acc_scale, int64_t n, void* stream) {
-  if (n == 0) return PPB_OK;
-  PPB_CHECK_ARG(n >= 0 && value && concentration && rate, "null pointer or negative n");
-  PPB_CHECK_ARG((concentration_stride | 1) == 1 && (rate_stride | 1) == 1, "strides must be 0 or 1");
-  return launch_score2(value, Param{concentration, concentration_stride}, Param{rate, rate_stride},
-                       Sink{lp_out, acc, acc_scale}, n, stream, GammaOp{});
-}
-
-int ppb_lognormal_log_prob(const float* value, const float* loc, int loc_stride, const float* scale, int scale_stride,
-                           float* lp_out, double* acc, double acc_scale, int64_t n, void* stream) {
-  if (n == 0) return PPB_OK;
-  PPB_CHECK_ARG(n >= 0 && value && loc && scale, "null pointer or negative n");
-  PPB_CHECK_ARG((loc_stride | 1) == 1 && (scale_stride | 1) == 1, "strides must be 0 or 1");
-  return launch_score2(value, Param{loc, loc_stride}, Param{scale, scale_stride}, Sink{lp_out, acc, acc_scale}, n,
-                       stream, LogNormalOp{});
-}
-
-int ppb_weibull_log_prob(const float* value, const float* scale, int scale_stride, const float* concentration,
-                         int concentration_stride, float* lp_out, double* acc, double acc_scale, int64_t n,
-                         void* stream) {
-  if (n == 0) return PPB_OK;
-  PPB_CHECK_ARG(n >= 0 && value && scale && concentration, "null pointer or negative n");
-  PPB_CHECK_ARG((scale_stride | 1) == 1 && (concentration_stride | 1) == 1, "strides must be 0 or 1");
-  return launch_score2(value, Param{scale, scale_stride}, Param{concentration, concentration_stride},
-                       Sink{lp_out, acc, acc_scale}, n, stream, WeibullOp{});
-}
-
-int ppb_beta_log_prob(const float* value, const float* concentration1, int concentration1_stride,
-                      const float* concentration0, int concentration0_stride, const float* low, int low_stride,
-                      const float* high, int high_stride, float* lp_out, double* acc, double acc_scale, int64_t n,
-                      void* stream) {
-  if (n == 0) return PPB_OK;
-  PPB_CHECK_ARG(n >= 0 && value && concentration1 && concentration0 && low && high, "null pointer or negative n");
-  PPB_CHECK_ARG((concentration1_stride | 1) == 1 && (concentration0_stride | 1) == 1 && (low_stride | 1) == 1 &&
-                    (high_stride | 1) == 1,
-                "strides must be 0 or 1");
-  Param a{concentration1, concentration1_stride}, b{concentration0, concentration0_stride}, lo{low, low_stride},
-      hi{high, high_stride};
-  Sink out{lp_out, acc, acc_scale};
-  const bool vec = aligned16(value) && a.vec_ok() && b.vec_ok() && lo.vec_ok() && hi.vec_ok() && out.vec_ok();
-  const int grid = ppb_grid_for(n, kThreads, 4);
-  if (vec)
-    k_beta<true><<<grid, kThreads, 0, (cudaStream_t)stream>>>(value, a, b, lo, hi, out, n);
-  else
-    k_beta<false><<<grid, kThreads, 0, (cudaStream_t)stream>>>(value, a, b, lo, hi, out, n);
-  PPB_LAUNCH_CHECK();
-  return PPB_OK;
-}
-
-int ppb_binomial_log_prob(const float* value, const float* total_count, int total_count_stride, const float* probs,
-                          int probs_stride, float* lp_out, double* acc, double acc_scale, int64_t n, void* stream) {
-  if (n == 0) return PPB_OK;
-  PPB_CHECK_ARG(n >= 0 && value && total_count && probs, "null pointer or negative n");
-  PPB_CHECK_ARG((total_count_stride | 1) == 1 && (probs_stride | 1) == 1, "strides must be 0 or 1");
-  return launch_score2(value, Param{total_count, total_count_stride}, Param{probs, probs_stride},
-                       Sink{lp_out, acc, acc_scale}, n, stream, BinomialOp{});
-}
-
-int ppb_von_mises_log_prob(const float* value, const float* loc, int loc_stride, const float* concentration,
-                           int concentration_stride, float* lp_out, double* acc, double acc_scale, int64_t n,
-                           void* stream) {
-  if (n == 0) return PPB_OK;
-  PPB_CHECK_ARG(n >= 0 && value && loc && concentration, "null pointer or negative n");
-  PPB_CHECK_ARG((loc_stride | 1) == 1 && (concentration_stride | 1) == 1, "strides must be 0 or 1");
-  return launch_score2(value, Param{loc, loc_stride}, Param{concentration, concentration_stride},
-                       Sink{lp_out, acc, acc_scale}, n, stream, VonMisesOp{});
+int ppb_event_log_prob_d1(int family, const float* value, const float* p0, const float* p1, const float* p2,
+                          const float* p3, int param_strides, float* lp_out, double* acc, double acc_scale, int64_t n,
+                          void* stream) {
+  const float* p[4] = {p0, p1, p2, p3};
+  const int64_t ps[4] = {param_strides & 1, (param_strides >> 1) & 1, (param_strides >> 2) & 1,
+                         (param_strides >> 3) & 1};
+  const int64_t es[4] = {0, 0, 0, 0};
+  return ppb_event_score(family, value, 1, 0, p, ps, es, n, 1, lp_out, nullptr, acc, acc_scale, stream);
 }
 
 int ppb_categorical_log_prob(const float* value, const float* probs, int64_t probs_row_stride, int num_categories,

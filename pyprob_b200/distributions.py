@@ -150,10 +150,6 @@ def _resolve_event(dist, n, value=_NO_VALUE, per_particle_value=False):
         return None
     E, forms, vform, value = layout
     D = math.prod(E)
-    family = ops.EVENT_FAMILIES.get(dist.name)
-    if family is None:
-        raise NotImplementedError('{} has no event-shaped form in pyprob_b200 (event shape {}) {}'.format(
-            dist.name, E, _REFERENCE_NOTE))
 
     def particle_rows(t, e):
         t = t.reshape(n, *([1] * (len(E) - len(e))), *e)
@@ -178,7 +174,7 @@ def _resolve_event(dist, n, value=_NO_VALUE, per_particle_value=False):
     else:
         t = value.to(device='cuda', dtype=torch.float32)
         v = particle_rows(t, tuple(t.shape[1:])) if vform == 'particle_event' else shared_row(t, tuple(t.shape))
-    return EventSite(family, E, n, params, v)
+    return EventSite(dist.family, E, n, params, v)
 
 
 def _length(*params):
@@ -266,86 +262,68 @@ class Distribution:
         return util._seed, util.next_draw_offset(), _shard_first_index
 
 
-class Normal(Distribution):
-    def __init__(self, loc, scale):
-        super().__init__('Normal', 'Normal')
-        (self.loc, self.scale), self._shaped = _params(loc, scale)
+class _ElementWise(Distribution):
+    """A family with an element-wise log_prob (ops.EVENT_FAMILIES), scored and drawn by the family-id kernels; the
+    parameters are kept in the kernels' order (self._params), each a Python scalar or a length-n CUDA tensor."""
+
+    def __init__(self, name, *params):
+        super().__init__(name, name)
+        self.family = ops.EVENT_FAMILIES[name]
+        self._params, self._shaped = _params(*params)
 
     @property
     def batch_length(self):
-        return _length(self.loc, self.scale)
+        return _length(*self._params)
+
+    def _draw(self, n, with_log_prob):
+        s, o, f = self._seed_args()
+        return ops._sample(self.family, self._params, n, s, o, f, with_log_prob, 'cuda')
+
+    def _log_prob(self, value):
+        return ops._score(self.family, _value(value, self.batch_length), self._params, None, None, 1.0)
+
+    def score_into(self, value, acc, scale):
+        ops._score(self.family, value, self._params, None, acc, scale)
+
+
+class Normal(_ElementWise):
+    def __init__(self, loc, scale):
+        super().__init__('Normal', loc, scale)
+        self.loc, self.scale = self._params
 
     mean = property(lambda self: self.loc)
     variance = property(lambda self: self.scale ** 2)
     stddev = property(lambda self: self.scale)
 
-    def _draw(self, n, with_log_prob):
-        s, o, f = self._seed_args()
-        return ops.normal_sample(self.loc, self.scale, n, s, o, f, with_log_prob)
-
-    def _log_prob(self, value):
-        return ops.normal_log_prob(_value(value, self.batch_length), self.loc, self.scale)
-
-    def score_into(self, value, acc, scale):
-        ops.normal_log_prob(value, self.loc, self.scale, acc=acc, acc_scale=scale)
-
     def __repr__(self):
         return 'Normal({}, {})'.format(self.loc, self.scale)
 
 
-class Uniform(Distribution):
+class Uniform(_ElementWise):
     def __init__(self, low, high):
-        super().__init__('Uniform', 'Uniform')
-        (self.low, self.high), self._shaped = _params(low, high)
-
-    @property
-    def batch_length(self):
-        return _length(self.low, self.high)
+        super().__init__('Uniform', low, high)
+        self.low, self.high = self._params
 
     mean = property(lambda self: (self.low + self.high) / 2)
     variance = property(lambda self: (self.high - self.low) ** 2 / 12)
-
-    def _draw(self, n, with_log_prob):
-        s, o, f = self._seed_args()
-        return ops.uniform_sample(self.low, self.high, n, s, o, f, with_log_prob)
-
-    def _log_prob(self, value):
-        return ops.uniform_log_prob(_value(value, self.batch_length), self.low, self.high)
-
-    def score_into(self, value, acc, scale):
-        ops.uniform_log_prob(value, self.low, self.high, acc=acc, acc_scale=scale)
 
     def __repr__(self):
         return 'Uniform(low={}, high={})'.format(self.low, self.high)
 
 
-class Poisson(Distribution):
+class Poisson(_ElementWise):
     def __init__(self, rate):
-        super().__init__('Poisson', 'Poisson')
-        (self.rate,), self._shaped = _params(rate)
-
-    @property
-    def batch_length(self):
-        return _length(self.rate)
+        super().__init__('Poisson', rate)
+        self.rate, = self._params
 
     mean = property(lambda self: self.rate)
     variance = property(lambda self: self.rate)
-
-    def _draw(self, n, with_log_prob):
-        s, o, f = self._seed_args()
-        return ops.poisson_sample(self.rate, n, s, o, f, with_log_prob)
-
-    def _log_prob(self, value):
-        return ops.poisson_log_prob(_value(value, self.batch_length), self.rate)
-
-    def score_into(self, value, acc, scale):
-        ops.poisson_log_prob(value, self.rate, acc=acc, acc_scale=scale)
 
     def __repr__(self):
         return 'Poisson({})'.format(self.rate)
 
 
-class Bernoulli(Distribution):
+class Bernoulli(_ElementWise):
     """probs (or logits, converted with a sigmoid): a scalar shared by all particles or one per particle (reference:
     bernoulli.py, torch Bernoulli).  Values are 0. / 1.; any other value scores NaN.
 
@@ -354,16 +332,12 @@ class Bernoulli(Distribution):
     logits = -30 it gives -30 for the value 1 where this gives -15.9 (DESIGN.md section 8)."""
 
     def __init__(self, probs=None, logits=None):
-        super().__init__('Bernoulli', 'Bernoulli')
         if probs is None:
             if logits is None:
                 raise ValueError('Either probs or logits must be given.')
             probs = torch.sigmoid(torch.as_tensor(logits, dtype=torch.float32))
-        (self.probs,), self._shaped = _params(probs)
-
-    @property
-    def batch_length(self):
-        return _length(self.probs)
+        super().__init__('Bernoulli', probs)
+        self.probs, = self._params
 
     @property
     def logits(self):
@@ -372,16 +346,6 @@ class Bernoulli(Distribution):
 
     mean = property(lambda self: self.probs)
     variance = property(lambda self: self.probs * (1 - self.probs))
-
-    def _draw(self, n, with_log_prob):
-        s, o, f = self._seed_args()
-        return ops.bernoulli_sample(self.probs, n, s, o, f, with_log_prob)
-
-    def _log_prob(self, value):
-        return ops.bernoulli_log_prob(_value(value, self.batch_length), self.probs)
-
-    def score_into(self, value, acc, scale):
-        ops.bernoulli_log_prob(value, self.probs, acc=acc, acc_scale=scale)
 
     def __repr__(self):
         return 'Bernoulli({})'.format(self.probs)
@@ -395,103 +359,57 @@ def _moment(fn, *params):
     return float(fn(*(torch.tensor(p, dtype=torch.float32) for p in params)))
 
 
-class Exponential(Distribution):
+class Exponential(_ElementWise):
     """rate: a scalar shared by all particles or one per particle (reference: exponential.py, torch Exponential).  Values
     below 0 and rates that are not positive score NaN."""
 
     def __init__(self, rate):
-        super().__init__('Exponential', 'Exponential')
-        (self.rate,), self._shaped = _params(rate)
-
-    @property
-    def batch_length(self):
-        return _length(self.rate)
+        super().__init__('Exponential', rate)
+        self.rate, = self._params
 
     mean = property(lambda self: _moment(lambda r: 1 / r, self.rate))
     variance = property(lambda self: _moment(lambda r: r.pow(-2), self.rate))
-
-    def _draw(self, n, with_log_prob):
-        s, o, f = self._seed_args()
-        return ops.exponential_sample(self.rate, n, s, o, f, with_log_prob)
-
-    def _log_prob(self, value):
-        return ops.exponential_log_prob(_value(value, self.batch_length), self.rate)
-
-    def score_into(self, value, acc, scale):
-        ops.exponential_log_prob(value, self.rate, acc=acc, acc_scale=scale)
 
     def __repr__(self):
         return 'Exponential({})'.format(self.rate)
 
 
-class Gamma(Distribution):
+class Gamma(_ElementWise):
     """Gamma(concentration, rate) (reference: gamma.py, torch Gamma).  Draws are clamped below at the smallest normal
     float, as torch's are, so no draw is 0."""
 
     def __init__(self, concentration, rate):
-        super().__init__('Gamma', 'Gamma')
-        (self.concentration, self.rate), self._shaped = _params(concentration, rate)
-
-    @property
-    def batch_length(self):
-        return _length(self.concentration, self.rate)
+        super().__init__('Gamma', concentration, rate)
+        self.concentration, self.rate = self._params
 
     mean = property(lambda self: _moment(lambda c, r: c / r, self.concentration, self.rate))
     variance = property(lambda self: _moment(lambda c, r: c / r.pow(2), self.concentration, self.rate))
-
-    def _draw(self, n, with_log_prob):
-        s, o, f = self._seed_args()
-        return ops.gamma_sample(self.concentration, self.rate, n, s, o, f, with_log_prob)
-
-    def _log_prob(self, value):
-        return ops.gamma_log_prob(_value(value, self.batch_length), self.concentration, self.rate)
-
-    def score_into(self, value, acc, scale):
-        ops.gamma_log_prob(value, self.concentration, self.rate, acc=acc, acc_scale=scale)
 
     def __repr__(self):
         return 'Gamma(concentration={}, rate={})'.format(self.concentration, self.rate)
 
 
-class LogNormal(Distribution):
+class LogNormal(_ElementWise):
     """LogNormal(loc, scale): exp of a Normal(loc, scale) (reference: log_normal.py, torch LogNormal)."""
 
     def __init__(self, loc, scale):
-        super().__init__('LogNormal', 'LogNormal')
-        (self.loc, self.scale), self._shaped = _params(loc, scale)
-
-    @property
-    def batch_length(self):
-        return _length(self.loc, self.scale)
+        super().__init__('LogNormal', loc, scale)
+        self.loc, self.scale = self._params
 
     mean = property(lambda self: _moment(lambda m, s: (m + s.pow(2) / 2).exp(), self.loc, self.scale))
     variance = property(lambda self: _moment(lambda m, s: (s.pow(2).exp() - 1) * (2 * m + s.pow(2)).exp(),
                                              self.loc, self.scale))
 
-    def _draw(self, n, with_log_prob):
-        s, o, f = self._seed_args()
-        return ops.lognormal_sample(self.loc, self.scale, n, s, o, f, with_log_prob)
-
-    def _log_prob(self, value):
-        return ops.lognormal_log_prob(_value(value, self.batch_length), self.loc, self.scale)
-
-    def score_into(self, value, acc, scale):
-        ops.lognormal_log_prob(value, self.loc, self.scale, acc=acc, acc_scale=scale)
-
     def __repr__(self):
         return 'LogNormal({}, {})'.format(self.loc, self.scale)
 
 
-class Weibull(Distribution):
+class Weibull(_ElementWise):
     """Weibull(scale, concentration) (reference: weibull.py, torch Weibull)."""
 
     def __init__(self, scale, concentration):
-        super().__init__('Weibull', 'Weibull')
-        (self.scale, self.concentration), self._shaped = _params(scale, concentration)
-
-    @property
-    def batch_length(self):
-        return _length(self.scale, self.concentration)
+        super().__init__('Weibull', scale, concentration)
+        self.scale, self.concentration = self._params
 
     mean = property(lambda self: _moment(lambda s, k: s * torch.exp(torch.lgamma(1 + k.reciprocal())),
                                          self.scale, self.concentration))
@@ -499,21 +417,11 @@ class Weibull(Distribution):
         lambda s, k: s.pow(2) * (torch.exp(torch.lgamma(1 + 2 * k.reciprocal())) -
                                  torch.exp(2 * torch.lgamma(1 + k.reciprocal()))), self.scale, self.concentration))
 
-    def _draw(self, n, with_log_prob):
-        s, o, f = self._seed_args()
-        return ops.weibull_sample(self.scale, self.concentration, n, s, o, f, with_log_prob)
-
-    def _log_prob(self, value):
-        return ops.weibull_log_prob(_value(value, self.batch_length), self.scale, self.concentration)
-
-    def score_into(self, value, acc, scale):
-        ops.weibull_log_prob(value, self.scale, self.concentration, acc=acc, acc_scale=scale)
-
     def __repr__(self):
         return 'Weibull(scale={}, concentration={})'.format(self.scale, self.concentration)
 
 
-class Beta(Distribution):
+class Beta(_ElementWise):
     """Beta(concentration1, concentration0) on [low, high] (reference: beta.py): a draw is low + (high - low) u with
     u ~ torch Beta(concentration1, concentration0), and log_prob(x) is torch's Beta log_prob of u = (x - low) / (high - low).
 
@@ -521,13 +429,8 @@ class Beta(Distribution):
     of x (DESIGN.md section 8)."""
 
     def __init__(self, concentration1, concentration0, low=0, high=1):
-        super().__init__('Beta', 'Beta')
-        (self.concentration1, self.concentration0, self.low, self.high), self._shaped = _params(
-            concentration1, concentration0, low, high)
-
-    @property
-    def batch_length(self):
-        return _length(self.concentration1, self.concentration0, self.low, self.high)
+        super().__init__('Beta', concentration1, concentration0, low, high)
+        self.concentration1, self.concentration0, self.low, self.high = self._params
 
     @property
     def mean(self):
@@ -541,24 +444,12 @@ class Beta(Distribution):
             return a * b / (total.pow(2) * (total + 1)) * (hi - lo) * (hi - lo)
         return _moment(var, self.concentration1, self.concentration0, self.low, self.high)
 
-    def _draw(self, n, with_log_prob):
-        s, o, f = self._seed_args()
-        return ops.beta_sample(self.concentration1, self.concentration0, self.low, self.high, n, s, o, f, with_log_prob)
-
-    def _log_prob(self, value):
-        return ops.beta_log_prob(_value(value, self.batch_length), self.concentration1, self.concentration0, self.low,
-                                 self.high)
-
-    def score_into(self, value, acc, scale):
-        ops.beta_log_prob(value, self.concentration1, self.concentration0, self.low, self.high, acc=acc,
-                          acc_scale=scale)
-
     def __repr__(self):
         return 'Beta(concentration1={}, concentration0={}, low={}, high={})'.format(
             self.concentration1, self.concentration0, self.low, self.high)
 
 
-class Binomial(Distribution):
+class Binomial(_ElementWise):
     """Binomial(total_count, probs) (reference: binomial.py, torch Binomial); total_count and probs are each a scalar or
     one per particle.  Values are the integers 0 .. total_count stored as floats; any other value scores NaN.
 
@@ -569,16 +460,12 @@ class Binomial(Distribution):
     |logits| = 16 the clamp takes over (DESIGN.md section 8)."""
 
     def __init__(self, total_count=1, probs=None, logits=None):
-        super().__init__('Binomial', 'Binomial')
         if probs is None:
             if logits is None:
                 raise ValueError('Either probs or logits must be given.')
             probs = torch.sigmoid(torch.as_tensor(logits, dtype=torch.float32))
-        (self.total_count, self.probs), self._shaped = _params(total_count, probs)
-
-    @property
-    def batch_length(self):
-        return _length(self.total_count, self.probs)
+        super().__init__('Binomial', total_count, probs)
+        self.total_count, self.probs = self._params
 
     @property
     def logits(self):
@@ -588,46 +475,22 @@ class Binomial(Distribution):
     mean = property(lambda self: _moment(lambda n, p: n * p, self.total_count, self.probs))
     variance = property(lambda self: _moment(lambda n, p: n * p * (1 - p), self.total_count, self.probs))
 
-    def _draw(self, n, with_log_prob):
-        s, o, f = self._seed_args()
-        return ops.binomial_sample(self.total_count, self.probs, n, s, o, f, with_log_prob)
-
-    def _log_prob(self, value):
-        return ops.binomial_log_prob(_value(value, self.batch_length), self.total_count, self.probs)
-
-    def score_into(self, value, acc, scale):
-        ops.binomial_log_prob(value, self.total_count, self.probs, acc=acc, acc_scale=scale)
-
     def __repr__(self):
         return 'Binomial(total_count={}, probs={})'.format(self.total_count, self.probs)
 
 
-class VonMises(Distribution):
+class VonMises(_ElementWise):
     """VonMises(loc, concentration) (reference: von_mises.py, torch VonMises).  Draws lie in [-pi, pi); any real value
     can be scored.  variance is torch's circular variance 1 - I1(concentration) / I0(concentration)."""
 
     def __init__(self, loc, concentration):
-        super().__init__('VonMises', 'VonMises')
-        (self.loc, self.concentration), self._shaped = _params(loc, concentration)
-
-    @property
-    def batch_length(self):
-        return _length(self.loc, self.concentration)
+        super().__init__('VonMises', loc, concentration)
+        self.loc, self.concentration = self._params
 
     mean = property(lambda self: self.loc)
     # torch's own fp32 formula, so that the value is the reference's (it loses digits at large concentration)
     variance = property(lambda self: _moment(
         lambda k: torch.distributions.VonMises(torch.zeros_like(k), k, validate_args=False).variance, self.concentration))
-
-    def _draw(self, n, with_log_prob):
-        s, o, f = self._seed_args()
-        return ops.von_mises_sample(self.loc, self.concentration, n, s, o, f, with_log_prob)
-
-    def _log_prob(self, value):
-        return ops.von_mises_log_prob(_value(value, self.batch_length), self.loc, self.concentration)
-
-    def score_into(self, value, acc, scale):
-        ops.von_mises_log_prob(value, self.loc, self.concentration, acc=acc, acc_scale=scale)
 
     def __repr__(self):
         return 'VonMises(loc={}, concentration={})'.format(self.loc, self.concentration)

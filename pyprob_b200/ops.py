@@ -50,81 +50,77 @@ def _sink(n, device, lp_out, acc):
     return lp_out, acc
 
 
-def normal_log_prob(value, mean, stddev, lp_out=None, acc=None, acc_scale=1.0):
+# ---- the eleven families with an element-wise log_prob: the family-id entry points at D = 1 ----------------------------
+
+EVENT_FAMILIES = {'Normal': 0, 'Uniform': 1, 'Poisson': 2, 'Bernoulli': 3, 'Exponential': 4, 'Gamma': 5,
+                  'LogNormal': 6, 'Weibull': 7, 'Beta': 8, 'Binomial': 9, 'VonMises': 10}
+EVENT_NUM_PARAMS = {0: 2, 1: 2, 2: 1, 3: 1, 4: 1, 5: 2, 6: 2, 7: 2, 8: 4, 9: 2, 10: 2}
+
+
+def _slots(params, n, device):
+    """-> (tensors kept alive, the four parameter pointers, the stride mask: bit k set where parameter k is per
+    particle) of a D = 1 call"""
+    held, ptrs, mask = [], [None, None, None, None], 0
+    for k, x in enumerate(params):
+        t, ptrs[k], stride = _param(x, n, device)
+        held.append(t)
+        mask |= stride << k
+    return held, ptrs, mask
+
+
+def _score(family, value, params, lp_out, acc, acc_scale):
+    """log_prob of a family over the particle axis: value [n], each parameter a scalar or [n]."""
     value = _f32(value, value.device).reshape(-1)
     n = value.numel()
-    m, mp, ms = _param(mean, n, value.device)
-    s, sp, ss = _param(stddev, n, value.device)
+    held, p, mask = _slots(params, n, value.device)
     lp_out, acc = _sink(n, value.device, lp_out, acc)
-    call('ppb_normal_log_prob', ptr(value), mp, ms, sp, ss, ptr(lp_out), ptr(acc), float(acc_scale), n, stream())
+    call('ppb_event_log_prob_d1', family, ptr(value), p[0], p[1], p[2], p[3], mask, ptr(lp_out), ptr(acc),
+         float(acc_scale), n, stream())
     return lp_out
+
+
+def normal_log_prob(value, mean, stddev, lp_out=None, acc=None, acc_scale=1.0):
+    return _score(EVENT_FAMILIES['Normal'], value, (mean, stddev), lp_out, acc, acc_scale)
 
 
 def uniform_log_prob(value, low, high, lp_out=None, acc=None, acc_scale=1.0):
-    value = _f32(value, value.device).reshape(-1)
-    n = value.numel()
-    a, ap, as_ = _param(low, n, value.device)
-    b, bp, bs = _param(high, n, value.device)
-    lp_out, acc = _sink(n, value.device, lp_out, acc)
-    call('ppb_uniform_log_prob', ptr(value), ap, as_, bp, bs, ptr(lp_out), ptr(acc), float(acc_scale), n, stream())
-    return lp_out
+    return _score(EVENT_FAMILIES['Uniform'], value, (low, high), lp_out, acc, acc_scale)
 
 
 def poisson_log_prob(value, rate, lp_out=None, acc=None, acc_scale=1.0):
-    value = _f32(value, value.device).reshape(-1)
-    n = value.numel()
-    r, rp, rs = _param(rate, n, value.device)
-    lp_out, acc = _sink(n, value.device, lp_out, acc)
-    call('ppb_poisson_log_prob', ptr(value), rp, rs, ptr(lp_out), ptr(acc), float(acc_scale), n, stream())
-    return lp_out
+    return _score(EVENT_FAMILIES['Poisson'], value, (rate,), lp_out, acc, acc_scale)
 
 
 def bernoulli_log_prob(value, probs, lp_out=None, acc=None, acc_scale=1.0):
-    value = _f32(value, value.device).reshape(-1)
-    n = value.numel()
-    p, pp, ps = _param(probs, n, value.device)
-    lp_out, acc = _sink(n, value.device, lp_out, acc)
-    call('ppb_bernoulli_log_prob', ptr(value), pp, ps, ptr(lp_out), ptr(acc), float(acc_scale), n, stream())
-    return lp_out
-
-
-def _score(name, value, params, lp_out, acc, acc_scale):
-    """log_prob entry points of the form (value, (param, stride)..., lp_out, acc, acc_scale, n, stream)."""
-    value = _f32(value, value.device).reshape(-1)
-    n = value.numel()
-    held = [_param(p, n, value.device) for p in params]
-    lp_out, acc = _sink(n, value.device, lp_out, acc)
-    args = [a for _, pp, ps in held for a in (pp, ps)]
-    call(name, ptr(value), *args, ptr(lp_out), ptr(acc), float(acc_scale), n, stream())
-    return lp_out
+    return _score(EVENT_FAMILIES['Bernoulli'], value, (probs,), lp_out, acc, acc_scale)
 
 
 def exponential_log_prob(value, rate, lp_out=None, acc=None, acc_scale=1.0):
-    return _score('ppb_exponential_log_prob', value, (rate,), lp_out, acc, acc_scale)
+    return _score(EVENT_FAMILIES['Exponential'], value, (rate,), lp_out, acc, acc_scale)
 
 
 def gamma_log_prob(value, concentration, rate, lp_out=None, acc=None, acc_scale=1.0):
-    return _score('ppb_gamma_log_prob', value, (concentration, rate), lp_out, acc, acc_scale)
+    return _score(EVENT_FAMILIES['Gamma'], value, (concentration, rate), lp_out, acc, acc_scale)
 
 
 def lognormal_log_prob(value, loc, scale, lp_out=None, acc=None, acc_scale=1.0):
-    return _score('ppb_lognormal_log_prob', value, (loc, scale), lp_out, acc, acc_scale)
+    return _score(EVENT_FAMILIES['LogNormal'], value, (loc, scale), lp_out, acc, acc_scale)
 
 
 def weibull_log_prob(value, scale, concentration, lp_out=None, acc=None, acc_scale=1.0):
-    return _score('ppb_weibull_log_prob', value, (scale, concentration), lp_out, acc, acc_scale)
+    return _score(EVENT_FAMILIES['Weibull'], value, (scale, concentration), lp_out, acc, acc_scale)
 
 
 def beta_log_prob(value, concentration1, concentration0, low=0.0, high=1.0, lp_out=None, acc=None, acc_scale=1.0):
-    return _score('ppb_beta_log_prob', value, (concentration1, concentration0, low, high), lp_out, acc, acc_scale)
+    return _score(EVENT_FAMILIES['Beta'], value, (concentration1, concentration0, low, high), lp_out, acc, acc_scale)
 
 
 def binomial_log_prob(value, total_count, probs, lp_out=None, acc=None, acc_scale=1.0):
-    return _score('ppb_binomial_log_prob', value, (total_count, probs), lp_out, acc, acc_scale)
+    return _score(EVENT_FAMILIES['Binomial'], value, (total_count, probs), lp_out, acc, acc_scale)
 
 
 def von_mises_log_prob(value, loc, concentration, lp_out=None, acc=None, acc_scale=1.0):
-    return _score('ppb_von_mises_log_prob', value, (loc, concentration), lp_out, acc, acc_scale)
+    return _score(EVENT_FAMILIES['VonMises'], value, (loc, concentration), lp_out, acc, acc_scale)
 
 
 def _rows(t, n, device):
@@ -191,73 +187,62 @@ def _out(n, device, want_lp):
     return v, lp
 
 
-def normal_sample(mean, stddev, n, seed, offset, first_index=0, with_log_prob=False, device='cuda'):
-    m, mp, ms = _param(mean, n, device)
-    s, sp, ss = _param(stddev, n, device)
+def _sample(family, params, n, seed, offset, first_index, with_log_prob, device):
+    """n draws of a family (particle i from Philox index first_index + i), each parameter a scalar or [n]."""
+    held, p, mask = _slots(params, n, device)
     v, lp = _out(n, device, with_log_prob)
-    call('ppb_normal_sample', mp, ms, sp, ss, ptr(v), ptr(lp), n, seed, offset, first_index, stream())
+    call('ppb_event_sample_d1', family, p[0], p[1], p[2], p[3], mask, ptr(v), ptr(lp), n, seed, offset, first_index,
+         stream())
     return (v, lp) if with_log_prob else v
+
+
+def normal_sample(mean, stddev, n, seed, offset, first_index=0, with_log_prob=False, device='cuda'):
+    return _sample(EVENT_FAMILIES['Normal'], (mean, stddev), n, seed, offset, first_index, with_log_prob, device)
 
 
 def uniform_sample(low, high, n, seed, offset, first_index=0, with_log_prob=False, device='cuda'):
-    a, ap, as_ = _param(low, n, device)
-    b, bp, bs = _param(high, n, device)
-    v, lp = _out(n, device, with_log_prob)
-    call('ppb_uniform_sample', ap, as_, bp, bs, ptr(v), ptr(lp), n, seed, offset, first_index, stream())
-    return (v, lp) if with_log_prob else v
+    return _sample(EVENT_FAMILIES['Uniform'], (low, high), n, seed, offset, first_index, with_log_prob, device)
 
 
 def poisson_sample(rate, n, seed, offset, first_index=0, with_log_prob=False, device='cuda'):
-    r, rp, rs = _param(rate, n, device)
-    v, lp = _out(n, device, with_log_prob)
-    call('ppb_poisson_sample', rp, rs, ptr(v), ptr(lp), n, seed, offset, first_index, stream())
-    return (v, lp) if with_log_prob else v
+    return _sample(EVENT_FAMILIES['Poisson'], (rate,), n, seed, offset, first_index, with_log_prob, device)
 
 
 def bernoulli_sample(probs, n, seed, offset, first_index=0, with_log_prob=False, device='cuda'):
-    p, pp, ps = _param(probs, n, device)
-    v, lp = _out(n, device, with_log_prob)
-    call('ppb_bernoulli_sample', pp, ps, ptr(v), ptr(lp), n, seed, offset, first_index, stream())
-    return (v, lp) if with_log_prob else v
-
-
-def _sample(name, params, n, seed, offset, first_index, with_log_prob, device):
-    """sampler entry points of the form ((param, stride)..., value_out, lp_out, n, seed, offset, first_index, stream)."""
-    held = [_param(p, n, device) for p in params]
-    v, lp = _out(n, device, with_log_prob)
-    args = [a for _, pp, ps in held for a in (pp, ps)]
-    call(name, *args, ptr(v), ptr(lp), n, seed, offset, first_index, stream())
-    return (v, lp) if with_log_prob else v
+    return _sample(EVENT_FAMILIES['Bernoulli'], (probs,), n, seed, offset, first_index, with_log_prob, device)
 
 
 def exponential_sample(rate, n, seed, offset, first_index=0, with_log_prob=False, device='cuda'):
-    return _sample('ppb_exponential_sample', (rate,), n, seed, offset, first_index, with_log_prob, device)
+    return _sample(EVENT_FAMILIES['Exponential'], (rate,), n, seed, offset, first_index, with_log_prob, device)
 
 
 def gamma_sample(concentration, rate, n, seed, offset, first_index=0, with_log_prob=False, device='cuda'):
-    return _sample('ppb_gamma_sample', (concentration, rate), n, seed, offset, first_index, with_log_prob, device)
+    return _sample(EVENT_FAMILIES['Gamma'], (concentration, rate), n, seed, offset, first_index, with_log_prob, device)
 
 
 def lognormal_sample(loc, scale, n, seed, offset, first_index=0, with_log_prob=False, device='cuda'):
-    return _sample('ppb_lognormal_sample', (loc, scale), n, seed, offset, first_index, with_log_prob, device)
+    return _sample(EVENT_FAMILIES['LogNormal'], (loc, scale), n, seed, offset, first_index, with_log_prob, device)
 
 
 def weibull_sample(scale, concentration, n, seed, offset, first_index=0, with_log_prob=False, device='cuda'):
-    return _sample('ppb_weibull_sample', (scale, concentration), n, seed, offset, first_index, with_log_prob, device)
+    return _sample(EVENT_FAMILIES['Weibull'], (scale, concentration), n, seed, offset, first_index, with_log_prob,
+                   device)
 
 
 def beta_sample(concentration1, concentration0, low, high, n, seed, offset, first_index=0, with_log_prob=False,
                 device='cuda'):
-    return _sample('ppb_beta_sample', (concentration1, concentration0, low, high), n, seed, offset, first_index,
+    return _sample(EVENT_FAMILIES['Beta'], (concentration1, concentration0, low, high), n, seed, offset, first_index,
                    with_log_prob, device)
 
 
 def binomial_sample(total_count, probs, n, seed, offset, first_index=0, with_log_prob=False, device='cuda'):
-    return _sample('ppb_binomial_sample', (total_count, probs), n, seed, offset, first_index, with_log_prob, device)
+    return _sample(EVENT_FAMILIES['Binomial'], (total_count, probs), n, seed, offset, first_index, with_log_prob,
+                   device)
 
 
 def von_mises_sample(loc, concentration, n, seed, offset, first_index=0, with_log_prob=False, device='cuda'):
-    return _sample('ppb_von_mises_sample', (loc, concentration), n, seed, offset, first_index, with_log_prob, device)
+    return _sample(EVENT_FAMILIES['VonMises'], (loc, concentration), n, seed, offset, first_index, with_log_prob,
+                   device)
 
 
 def categorical_sample(probs, n, seed, offset, first_index=0, with_log_prob=False, device='cuda'):
@@ -288,9 +273,6 @@ def mixture_truncated_normal_sample(means, stddevs, probs, low, high, n, seed, o
 
 # ---- event-shaped sites (C-ABI section 2b): D elements per particle ---------------------------------------------------
 
-EVENT_FAMILIES = {'Normal': 0, 'Uniform': 1, 'Poisson': 2, 'Bernoulli': 3, 'Exponential': 4, 'Gamma': 5,
-                  'LogNormal': 6, 'Weibull': 7, 'Beta': 8, 'Binomial': 9, 'VonMises': 10}
-EVENT_NUM_PARAMS = {0: 2, 1: 2, 2: 1, 3: 1, 4: 1, 5: 2, 6: 2, 7: 2, 8: 4, 9: 2, 10: 2}
 EVENT_MAX_D = 1 << 24          # element index: Philox counter bits 40 .. 63
 EVENT_MAX_PARTICLES = 1 << 40  # particle index: Philox counter bits 0 .. 39
 

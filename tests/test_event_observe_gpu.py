@@ -164,6 +164,28 @@ def test_d1_equals_scalar_accumulator(cuda, family):
     ops.event_log_prob(ops.EVENT_FAMILIES[family], v, [p.reshape(n, 1) for p in params], n, 1, acc=a2, acc_scale=1.3)
     assert torch.equal(a1.view(torch.int64), a2.view(torch.int64))
 
+    # every D = 1 layout is a flat stride: (1, 1) is (1, 0), and a shared (0, 1) or (0, 0) operand is (1, 0) over its
+    # expanded copy, for the value and every parameter, accumulator and lp_out bit for bit
+    def run(operands):
+        acc, lp = a1.clone(), torch.empty(n, device='cuda')
+        slots = [a for t, ps, es in operands[1:] for a in (ops.ptr(t), ps, es)] + [None, 0, 0] * (5 - len(operands))
+        t, ps, es = operands[0]
+        ops._lib.call('ppb_event_log_prob', ops.EVENT_FAMILIES[family], ops.ptr(t), ps, es, *slots, n, 1, ops.ptr(lp),
+                      ops.ptr(acc), 1.3, ops.stream())
+        return acc.view(torch.int64), lp
+    flat = [t.reshape(n).contiguous() for t in [v] + params]
+    want = run([(t, 1, 0) for t in flat])
+    got = run([(t, 1, 1) for t in flat])
+    assert torch.equal(got[0], want[0]) and torch.equal(got[1], want[1])
+    for k in range(len(flat)):
+        shared = [t[:1].clone() if j == k else t for j, t in enumerate(flat)]
+        want = run([(t.expand(n).contiguous(), 1, 0) for t in shared])
+        for es in (0, 1):
+            got = run([(t, 0, es) if j == k else (t, 1, 0) for j, t in enumerate(shared)])
+            assert torch.equal(got[0], want[0]) and torch.equal(got[1].isnan(), want[1].isnan()), (family, k, es)
+            ok = ~want[1].isnan()
+            assert torch.equal(got[1][ok], want[1][ok]), (family, k, es)
+
 
 def test_beyond_2_31_elements(cuda):
     """n D = 2^32 with a shared value row and scalar parameters: nothing large is allocated."""
