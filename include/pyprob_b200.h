@@ -308,7 +308,7 @@ typedef struct {
   const int32_t* step_prev_row0; /* [n_steps] first row of the same sub-batch at t-1 (-1 at t=0)  */
   const int32_t* group_addr;     /* [n_groups]   device copy of group_addr_host                   */
   const int32_t* group_start;    /* [n_groups+1] device copy of group_start_host                  */
-  /* host copies of the per-step arrays (planning of the tensor-core path) */
+  /* host copies of the per-step arrays, used to plan launches: required at every precision */
   const int32_t* step_addr_host;
   const int32_t* step_row0_host;
   const int32_t* step_nrows_host;

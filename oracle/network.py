@@ -126,8 +126,11 @@ def sample_embedding(params, address, family, num_categories, values):
     return _ff(x, params, '_layers_sample_embedding.{}'.format(address), True)
 
 
-def loss(params, sub_batches, observe_names, observe_in_dims, K, sample_dim=4, addr_dim=64, type_dim=8,
-         repaired_rows='reference'):
+def _sample_dim(params):
+    return next(v.size(0) for k, v in params.items() if k.startswith('_layers_sample_embedding.') and k.endswith('.bias'))
+
+
+def loss(params, sub_batches, observe_names, observe_in_dims, K, addr_dim=64, type_dim=8, repaired_rows='reference'):
     """-> (loss, per-sub-batch list of [T,B] log-prob tensors).  sub_batches: dicts from sub_batch_from_traces.
 
     repaired_rows: what happens to the GRADIENT of rows whose log q is -inf and gets replaced by log(1e-8)
@@ -137,6 +140,7 @@ def loss(params, sub_batches, observe_names, observe_in_dims, K, sample_dim=4, a
                    a NaN gradient (and the reference's next optimizer.step() destroys the network) — kept to document it;
       'constant'   the replaced value is the constant the reference's code intends: such rows contribute no gradient
                    (the head is evaluated on the remaining rows only).  This is what the CUDA path implements."""
+    sample_dim = _sample_dim(params)
     total = 0.0
     batch_size = sum(sb['values'].size(1) for sb in sub_batches)
     all_lp = []
@@ -220,8 +224,7 @@ def infer_sequence(params, obs_row, observe_names, observe_in_dims, K, steps, n=
     b_ih, b_hh = params['_layers_lstm.bias_ih_l0'], params['_layers_lstm.bias_hh_l0']
     H = W_hh.size(1)
     h, c = torch.zeros(n, H), torch.zeros(n, H)
-    smp_dim = next(v.size(0) for k, v in params.items() if k.startswith('_layers_sample_embedding.') and
-                   k.endswith('.bias'))
+    smp_dim = _sample_dim(params)
     out = []
     for t, st in enumerate(steps):
         cur_t = params['_layers_distribution_type_embedding.' + st['family']]

@@ -5,7 +5,7 @@
 // Algorithmic restructuring relative to the reference's per-(t,b) concatenation (:146-182): the LSTM
 // input GEMM x_t W_ih^T is split by the block structure of x_t = [obs_emb(b) | smp_emb(t,b) | step_emb(t,s)]:
 //   P_obs[b]    = obs_emb[b]  W_ih[:, :E]^T           once per trace          (GEMM, K = E)
-//   P_step[t,s] = step_emb    W_ih[:, E+S:]^T + b_ih + b_hh   once per (step, sub-batch) (GEMM, K = 2(td+ad))
+//   P_step[t,s] = step_emb    W_ih[:, E+S:]^T + b_ih + b_hh   once per (step, sub-batch) (k_pstep_fwd, K = 2(td+ad))
 //   smp term    = sum_j smp_emb[t,b,j] W_ih[:, E+j]   S FMAs per gate element, fused in the cell kernel
 // which removes the T-fold recomputation of the observation block.
 #include <vector>
@@ -120,7 +120,7 @@ struct Ws {
   float* gates; float* c; float* h; float* hid; float* out_raw; float* row_lp; float* d_out;
   float* loss_acc;  // [0] = sum of -lp ; int status at [1]
   // backward
-  float* d_hid; float* dh; float* dh_rec; float* dc; float* d_pobs; float* d_pstep; float* d_smp; float* d_embcat;
+  float* d_hid; float* dh; float* dh_rec; float* dc; float* d_pobs; float* d_pstep;
   float* d_obs_emb; float* d_fin_act[PPB_MAX_FF_LAYERS]; float* d_obs_cat; float* d_obs_act[PPB_MAX_OBS][PPB_MAX_FF_LAYERS];
   Problem* problems; // device problem list
   int64_t max_problems;
@@ -169,8 +169,6 @@ Ws carve(const ppb_net* net, Dims d, void* base) {
   w.dh_rec = take((int64_t)d.R * H);
   w.dc = take((int64_t)d.R * H);
   w.d_pobs = take((int64_t)d.B * 4 * H);
-  w.d_smp = take((int64_t)d.R * S);
-  w.d_embcat = take((int64_t)d.NS * C2);
   w.d_pstep = take((int64_t)d.NS * 4 * H);   // d_pstep and d_obs_emb are adjacent: the tensor-core backward zeroes both at once
   w.d_obs_emb = take((int64_t)d.B * E);
   for (int l = 0; l + 1 < D.obs_final.num_layers; ++l) w.d_fin_act[l] = take((int64_t)d.B * D.obs_final.layers[l].out_dim);
@@ -348,7 +346,34 @@ int run_phase(const gemm::Phase& ph, const Problem* dev, cudaStream_t st, const 
 // ---------------------------------------------------------------------------------------------------
 // element-wise / fused kernels
 // ---------------------------------------------------------------------------------------------------
-// step embedding rows: [prev_type | prev_addr | cur_type | cur_addr] (inference_network_lstm.py:175-180)
+// Arena offset of column j of a step-embedding row [prev_type | prev_addr | cur_type | cur_addr]
+// (inference_network_lstm.py:175-180), or -1 in the previous half when there is no previous site (t = 0).
+// desc(is_prev, a) points a at the descriptor of that half and returns false when there is no site; only the half that
+// column j needs is looked up.
+template <typename Desc>
+__device__ __forceinline__ int64_t step_embed_off(const int64_t* __restrict__ type_off, int td, int ad, int j, Desc desc) {
+  const bool is_prev = j < td + ad;
+  const ppb_addr_desc* a;
+  if (!desc(is_prev, a)) return -1;
+  const int jj = is_prev ? j : j - (td + ad);
+  return jj < td ? type_off[a->type_id] + jj : a->addr_emb_off + (jj - td);
+}
+
+// Pre-activation of unit j of an address's sample embedding at value x: b[j] + W[j] . x, with x one-hot for a Categorical
+// address (inference_network_lstm.py:168-169, embedding_feedforward.py:35-48)
+__device__ __forceinline__ float smp_embed_pre(const float* __restrict__ arena, const ppb_addr_desc& a, float x, int j) {
+  const float* W = arena + a.smp_w_off + (int64_t)j * a.smp_in;
+  float pre = arena[a.smp_b_off + j];
+  if (a.family == PPB_FAMILY_CATEGORICAL) {
+    const int c = (int)x;
+    if (c >= 0 && c < a.smp_in) pre += W[c];
+  } else {
+    pre += W[0] * x;
+  }
+  return pre;
+}
+
+// step embedding rows, one per (step, sub-batch)
 __global__ void k_step_embed(const float* __restrict__ arena, const ppb_addr_desc* __restrict__ addrs,
                              const int64_t* __restrict__ type_off, const int* __restrict__ step_addr,
                              const int* __restrict__ step_prev, int n_steps, int td, int ad,
@@ -357,14 +382,12 @@ __global__ void k_step_embed(const float* __restrict__ arena, const ppb_addr_des
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < (int64_t)n_steps * C2;
        e += (int64_t)gridDim.x * blockDim.x) {
     int st = (int)(e / C2), j = (int)(e % C2);
-    int which = j < (td + ad) ? step_prev[st] : step_addr[st];
-    int jj = j < (td + ad) ? j : j - (td + ad);
-    float v = 0.0f;
-    if (which >= 0) {
-      const ppb_addr_desc& a = addrs[which];
-      v = jj < td ? arena[type_off[a.type_id] + jj] : arena[a.addr_emb_off + (jj - td)];
-    }
-    emb_cat[e] = v;
+    const int64_t o = step_embed_off(type_off, td, ad, j, [&](bool is_prev, const ppb_addr_desc*& a) {
+      const int which = is_prev ? step_prev[st] : step_addr[st];
+      a = addrs + which;
+      return which >= 0;
+    });
+    emb_cat[e] = o >= 0 ? arena[o] : 0.0f;
   }
 }
 
@@ -377,8 +400,7 @@ __global__ void k_wsmp_transpose(const float* __restrict__ w_ih, int I, int E, i
   }
 }
 
-// previous-sample embedding per row: relu(W_se[prev_addr] x + b), x = value or one-hot(value)
-// (inference_network_lstm.py:168-169, embedding_feedforward.py:35-48); zeros at t = 0 (:157)
+// previous-sample embedding per row: relu of the previous address's sample-embedding layer; zeros at t = 0 (:157)
 __global__ void k_smp_embed(const float* __restrict__ arena, const ppb_addr_desc* __restrict__ addrs,
                             const int* __restrict__ row_step, const int* __restrict__ step_prev,
                             const int* __restrict__ row_prev, const float* __restrict__ values, int R, int S,
@@ -387,21 +409,7 @@ __global__ void k_smp_embed(const float* __restrict__ arena, const ppb_addr_desc
        e += (int64_t)gridDim.x * blockDim.x) {
     int row = (int)(e / S), j = (int)(e % S);
     int pa = step_prev[row_step[row]];
-    float v = 0.0f;
-    if (pa >= 0) {
-      const ppb_addr_desc& a = addrs[pa];
-      float x = values[row_prev[row]];
-      const float* W = arena + a.smp_w_off + (int64_t)j * a.smp_in;
-      float pre = arena[a.smp_b_off + j];
-      if (a.family == PPB_FAMILY_CATEGORICAL) {
-        int c = (int)x;
-        if (c >= 0 && c < a.smp_in) pre += W[c];
-      } else {
-        pre += W[0] * x;
-      }
-      v = fmaxf(pre, 0.0f);
-    }
-    smp_emb[e] = v;
+    smp_emb[e] = pa >= 0 ? fmaxf(smp_embed_pre(arena, addrs[pa], values[row_prev[row]], j), 0.0f) : 0.0f;
   }
 }
 
@@ -861,43 +869,10 @@ __global__ void __launch_bounds__(256) k_step_colsum(const float* __restrict__ d
   }
 }
 
-// d_smp[row, j] = sum_col dgates[row, col] * w_smp_t[j][col], masked by relu; then the per-address
-// sample-embedding layer gradients (atomics on tiny [S x smp_in] matrices)
-__global__ void __launch_bounds__(128) k_smp_bwd(const float* __restrict__ dgates, const float* __restrict__ w_smp_t,
-                                                  const float* __restrict__ smp_emb, const float* __restrict__ values,
-                                                  const int* __restrict__ row_step, const int* __restrict__ step_prev,
-                                                  const int* __restrict__ row_prev,
-                                                  const ppb_addr_desc* __restrict__ addrs, int R, int H4, int S,
-                                                  float* __restrict__ grad) {
-  // one warp per row
-  int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  int nwarps = (gridDim.x * blockDim.x) >> 5;
-  for (int row = warp; row < R; row += nwarps) {
-    int pa = step_prev[row_step[row]];
-    if (pa < 0) continue;
-    const ppb_addr_desc& a = addrs[pa];
-    float x = values[row_prev[row]];
-    for (int j = 0; j < S; ++j) {
-      float s = 0.0f;
-      for (int col = lane; col < H4; col += 32) s = fmaf(dgates[(int64_t)row * H4 + col], w_smp_t[(int64_t)j * H4 + col], s);
-      s = ppb_warp_sum(s);
-      if (lane == 0 && smp_emb[(int64_t)row * S + j] > 0.0f && s != 0.0f) {
-        atomicAdd(grad + a.smp_b_off + j, s);
-        if (a.family == PPB_FAMILY_CATEGORICAL) {
-          int cidx = (int)x;
-          if (cidx >= 0 && cidx < a.smp_in) atomicAdd(grad + a.smp_w_off + (int64_t)j * a.smp_in + cidx, s);
-        } else {
-          atomicAdd(grad + a.smp_w_off + (int64_t)j * a.smp_in, s * x);
-        }
-      }
-    }
-  }
-}
-
-// Same gradients with the atomics taken off the hot addresses: all rows of a (step, sub-batch) segment share their previous
-// address, so a block owns a slab of ONE segment, accumulates the tiny [S x smp_in] weight and [S] bias gradients of that
-// address in shared memory and issues one global atomic per entry per block (measured with the per-row atomics of k_smp_bwd
-// at T = 50, B = 512: 0.38 ms, 200 k atomics on ~500 addresses).
+// d smp_emb[row, j] = sum_col dgates[row, col] * w_smp_t[j][col], masked by relu; then the per-address sample-embedding layer
+// gradients.  All rows of a (step, sub-batch) segment share their previous address, so a block owns a slab of ONE segment,
+// accumulates the tiny [S x smp_in] weight and [S] bias gradients of that address in shared memory and issues one global
+// atomic per entry per block (one global atomic per row took 0.38 ms at T = 50, B = 512: 200 k atomics on ~500 addresses).
 __global__ void __launch_bounds__(128) k_smp_bwd_seg(const float* __restrict__ dgates, const float* __restrict__ w_smp_t,
                                                       const float* __restrict__ smp_emb, const float* __restrict__ values,
                                                       const int* __restrict__ step_prev, const int* __restrict__ step_row0,
@@ -955,10 +930,10 @@ __global__ void __launch_bounds__(128) k_smp_bwd_seg(const float* __restrict__ d
 }
 
 // ONE pass over dgates for everything that reduces it over rows (T = 50, B = 512: dgates is 210 MB; the three kernels it
-// replaces — k_step_colsum, k_smp_bwd(_seg), k_wsmp_grad — each streamed it again):
+// replaces — k_step_colsum, k_smp_bwd_seg, k_wsmp_grad — each streamed it again):
 //   d_pstep[st, col]        += sum over the rows of segment st of dgates[row, col]                 (atomics; zeroed before)
 //   dW_ih[col, E + j]       += sum_rows dgates[row, col] * smp_emb[row, j]
-//   d_smp[row, j]            = sum_col dgates[row, col] * W_ih[col, E + j]  -> ReLU mask -> the previous address's
+//   d smp_emb[row, j]        = sum_col dgates[row, col] * W_ih[col, E + j]  -> ReLU mask -> the previous address's
 //                              sample-embedding layer gradients (shared-memory accumulation per block, see k_smp_bwd_seg)
 // A block owns a slab of rows of one (step, sub-batch) segment; a thread owns NC = 4H / 256 columns.
 constexpr int kRedSlab = 64;
@@ -1092,32 +1067,103 @@ __global__ void k_wsmp_grad(const float* __restrict__ dgates, const float* __res
   }
 }
 
-// biases: db_ih = db_hh = column sums of d_pstep ; scatter d_embcat into the embedding tables
-__global__ void k_bias_grad(const float* __restrict__ d_pstep, int NS, int H4, float* __restrict__ db_ih,
-                            float* __restrict__ db_hh) {
-  for (int col = blockIdx.x * blockDim.x + threadIdx.x; col < H4; col += gridDim.x * blockDim.x) {
+// p_step[st, col] = b_ih[col] + b_hh[col] + sum_j emb_cat[st, j] W_ih[col, E + S + j]   (one warp per output)
+__global__ void __launch_bounds__(256) k_pstep_fwd(const float* __restrict__ emb_cat, const float* __restrict__ w_ih,
+                                                    const float* __restrict__ b_ih, const float* __restrict__ b_hh,
+                                                    int NS, int H4, int I, int off, int C2, float* __restrict__ p_step) {
+  int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  int nw = (gridDim.x * blockDim.x) >> 5;
+  for (int o = warp; o < NS * H4; o += nw) {
+    int st = o / H4, col = o % H4;
     float s = 0.0f;
-    for (int st = 0; st < NS; ++st) s += d_pstep[(int64_t)st * H4 + col];
-    db_ih[col] += s;
-    db_hh[col] += s;
+    for (int j = lane; j < C2; j += 32) s = fmaf(emb_cat[(int64_t)st * C2 + j], w_ih[(int64_t)col * I + off + j], s);
+    s = ppb_warp_sum(s);
+    if (lane == 0) p_step[o] = s + b_ih[col] + b_hh[col];
   }
 }
-__global__ void k_embed_scatter(const float* __restrict__ d_embcat, const ppb_addr_desc* __restrict__ addrs,
-                                const int64_t* __restrict__ type_off, const int* __restrict__ step_addr,
-                                const int* __restrict__ step_prev, int n_steps, int td, int ad,
-                                float* __restrict__ grad) {
-  int C2 = 2 * (td + ad);
-  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < (int64_t)n_steps * C2;
-       e += (int64_t)gridDim.x * blockDim.x) {
-    int st = (int)(e / C2), j = (int)(e % C2);
-    int which = j < (td + ad) ? step_prev[st] : step_addr[st];
-    int jj = j < (td + ad) ? j : j - (td + ad);
-    if (which < 0) continue;
-    const ppb_addr_desc& a = addrs[which];
-    float v = d_embcat[e];
-    if (v == 0.0f) continue;
-    if (jj < td) atomicAdd(grad + type_off[a.type_id] + jj, v);
-    else atomicAdd(grad + a.addr_emb_off + (jj - td), v);
+// Every gradient that follows from d_pstep, in ONE launch (T = 50: NS = 50 step segments):
+//   blocks [0, nx)  : d emb_cat[st, j] = sum_col d_pstep[st, col] W_ih[col, off + j], lanes over j, warps and blockIdx over
+//                     column slices; each block's partial sum goes straight into the type / address embedding it came from
+//   blocks [nx, ...): dW_ih[col, off + j] += sum_st d_pstep[st, col] emb_cat[st, j] (one thread per entry), then
+//                     db_ih[col] = db_hh[col] += sum_st d_pstep[st, col]
+__global__ void __launch_bounds__(256) k_pstep_bwd(const float* __restrict__ d_pstep, const float* __restrict__ w_ih,
+                                                    const float* __restrict__ emb_cat, const ppb_addr_desc* __restrict__ addrs,
+                                                    const int64_t* __restrict__ type_off, const int* __restrict__ step_addr,
+                                                    const int* __restrict__ step_prev, int NS, int H4, int I, int off, int td,
+                                                    int ad, int zsplit, int nx, float* __restrict__ grad, int64_t w_ih_off,
+                                                    int64_t b_ih_off, int64_t b_hh_off) {
+  const int C2 = 2 * (td + ad);
+  if ((int)blockIdx.x < nx) {
+    __shared__ float part[8][33];
+    const int jbs = (C2 + 31) / 32;
+    const int jb = blockIdx.x % jbs, st = (blockIdx.x / jbs) % NS, z = blockIdx.x / (jbs * NS);
+    const int lane = threadIdx.x & 31, slice = threadIdx.x >> 5;
+    const int j = jb * 32 + lane;
+    float s = 0.0f;
+    if (j < C2)
+      for (int col = z * 8 + slice; col < H4; col += 8 * zsplit)
+        s = fmaf(d_pstep[(int64_t)st * H4 + col], __ldg(w_ih + (int64_t)col * I + off + j), s);
+    part[slice][lane] = s;
+    __syncthreads();
+    if (slice == 0 && j < C2) {
+      float t = 0.0f;
+#pragma unroll
+      for (int k = 0; k < 8; ++k) t += part[k][lane];
+      const int64_t o = step_embed_off(type_off, td, ad, j, [&](bool is_prev, const ppb_addr_desc*& a) {
+        const int which = is_prev ? step_prev[st] : step_addr[st];
+        a = addrs + which;
+        return which >= 0;
+      });
+      if (o >= 0 && t != 0.0f) atomicAdd(grad + o, t);
+    }
+    return;
+  }
+  const int64_t nwe = (int64_t)H4 * C2;
+  for (int64_t e = (int64_t)(blockIdx.x - nx) * blockDim.x + threadIdx.x; e < nwe + H4;
+       e += (int64_t)(gridDim.x - nx) * blockDim.x) {
+    if (e < nwe) {
+      const int col = (int)(e / C2), j = (int)(e % C2);
+      float s = 0.0f;
+      for (int st = 0; st < NS; ++st) s = fmaf(d_pstep[(int64_t)st * H4 + col], emb_cat[(int64_t)st * C2 + j], s);
+      grad[w_ih_off + (int64_t)col * I + off + j] += s;
+    } else {
+      const int col = (int)(e - nwe);
+      float s = 0.0f;
+      for (int st = 0; st < NS; ++st) s += d_pstep[(int64_t)st * H4 + col];
+      grad[b_ih_off + col] += s;
+      grad[b_hh_off + col] += s;
+    }
+  }
+}
+
+// db2[a] += colsum(d_out rows of a), db1[a] += colsum(d_hid rows of a) for every address group in ONE launch:
+// blockIdx.y = group, blockIdx.x = 32-column block (first the hidden columns, then the output columns)
+__global__ void __launch_bounds__(256) k_head_bias_grad(const float* __restrict__ d_out, int out_pad,
+                                                         const float* __restrict__ d_hid, int dh_pad,
+                                                         const int* __restrict__ head_rows, const int* __restrict__ group_start,
+                                                         const int* __restrict__ group_addr,
+                                                         const ppb_addr_desc* __restrict__ addrs, float* __restrict__ grad) {
+  __shared__ float part[8][33];
+  const int g = blockIdx.y;
+  const ppb_addr_desc a = addrs[group_addr[g]];
+  const int hid_blocks = (dh_pad + 31) / 32;
+  const bool is_hid = (int)blockIdx.x < hid_blocks;
+  const int lane = threadIdx.x & 31, slice = threadIdx.x >> 5;
+  const int n = (is_hid ? blockIdx.x : blockIdx.x - hid_blocks) * 32 + lane;
+  const int width = is_hid ? a.head_hidden : a.head_out;
+  const float* src = is_hid ? d_hid : d_out;
+  const int ld = is_hid ? dh_pad : out_pad;
+  const int s0 = group_start[g], cnt = group_start[g + 1] - s0;
+  float s = 0.0f;
+  if (n < width)   // blockIdx.z splits the rows of the group
+    for (int m = blockIdx.z * 8 + slice; m < cnt; m += 8 * gridDim.z) s += src[(int64_t)head_rows[s0 + m] * ld + n];
+  part[slice][lane] = s;
+  __syncthreads();
+  if (slice == 0 && n < width) {
+    float t = 0.0f;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) t += part[k][lane];
+    if (t != 0.0f) atomicAdd(grad + (is_hid ? a.b1_off : a.b2_off) + n, t);
   }
 }
 // bias gradient of a Linear: db[n] += sum_m dY[gm(m), n].  Block = 32 columns x 8 row-slices; rows are
@@ -1147,10 +1193,6 @@ __global__ void k_scale(float* __restrict__ x, int64_t n, float a) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) x[i] *= a;
 }
 
-// p[i] += b[i mod H4]  (fold b_hh into the step projection, which already carries b_ih)
-__global__ void k_add_row_bias(float* __restrict__ p, const float* __restrict__ b, int64_t n, int H4) {
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) p[i] += b[i % H4];
-}
 // ReLU backward at the top of a chain: d[i] = y[i] > 0 ? d[i] : 0
 __global__ void k_mask_nonpos(float* __restrict__ d, const float* __restrict__ y, int64_t n) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
@@ -1243,14 +1285,101 @@ void simt_head_bwd(Builder& bl, const ppb_net* net, const float* arena, float* g
   }
 }
 
-// head bias gradients
-int simt_head_bias_grad(const ppb_net* net, const ppb_batch* b, const Ws& w, float* grad, cudaStream_t st) {
-  for (int g = 0; g < b->n_groups; ++g) {
-    const ppb_addr_desc& a = net->addrs[b->group_addr_host[g]];
-    int s0 = b->group_start_host[g], cnt = b->group_start_host[g + 1] - s0;
-    k_colsum_gather<<<dim3((a.head_out + 31) / 32, 8), 256, 0, st>>>(w.d_out, net->out_pad, b->head_rows + s0, cnt, a.head_out, grad + a.b2_off);
+// ---- CUDA-core side jobs of the training step, shared by every precision -------------------------------------------------
+// db2[a] += colsum(d_out rows of a), db1[a] += colsum(d_hid rows of a), every address group in one launch
+int launch_head_bias_grad(const ppb_net* net, const ppb_batch* b, const Ws& w, float* grad, cudaStream_t st) {
+  // a row split that brings the grid to about one block per SM (T = 1: 10 column blocks, one address group) and leaves
+  // each warp at least eight rows
+  const int G = b->n_groups;
+  const int cb = (net->dh_pad + 31) / 32 + (net->out_pad + 31) / 32;
+  int max_rows = 0;
+  for (int g = 0; g < G; ++g) max_rows = b->group_start_host[g + 1] - b->group_start_host[g] > max_rows ? b->group_start_host[g + 1] - b->group_start_host[g] : max_rows;
+  int zs = PPB_NUM_SMS / (cb * G);
+  const int zmax = (max_rows + 63) / 64;
+  zs = zs > zmax ? zmax : zs;
+  zs = zs < 1 ? 1 : zs;
+  k_head_bias_grad<<<dim3(cb, G, zs), 256, 0, st>>>(w.d_out, net->out_pad, w.d_hid, net->dh_pad, b->head_rows, b->group_start,
+                                                     b->group_addr, net->d_addrs, grad);
+  PPB_LAUNCH_CHECK();
+  return PPB_OK;
+}
+
+// The LSTM inputs that do not depend on the observation: step embeddings -> P_step (both biases folded in), and at T > 1 the
+// transposed sample-embedding columns of W_ih and the previous-sample embeddings (they only enter at t >= 1)
+int launch_step_inputs_fwd(const ppb_net* net, const float* arena, const ppb_batch* b, const Ws& w, cudaStream_t st) {
+  const ppb_net_desc& D = net->desc;
+  const Dims d = dims_of(b);
+  const int H4 = 4 * D.lstm_dim, E = D.obs_dim, S = D.sample_dim, I = net->I;
+  const int C2 = 2 * (D.type_dim + D.addr_dim);
+  k_step_embed<<<ew_grid((int64_t)d.NS * C2), 256, 0, st>>>(arena, net->d_addrs, net->d_type_off, b->step_addr,
+                                                            b->step_prev_addr, d.NS, D.type_dim, D.addr_dim, w.emb_cat);
+  PPB_LAUNCH_CHECK();
+  k_pstep_fwd<<<ew_grid((int64_t)d.NS * H4 * 32), 256, 0, st>>>(w.emb_cat, arena + D.w_ih_off, arena + D.b_ih_off,
+                                                                arena + D.b_hh_off, d.NS, H4, I, E + S, C2, w.p_step);
+  PPB_LAUNCH_CHECK();
+  if (d.T > 1) {
+    k_wsmp_transpose<<<ew_grid(S * H4), 256, 0, st>>>(arena + D.w_ih_off, I, E, S, H4, w.w_smp_t);
     PPB_LAUNCH_CHECK();
-    k_colsum_gather<<<dim3((a.head_hidden + 31) / 32, 8), 256, 0, st>>>(w.d_hid, net->dh_pad, b->head_rows + s0, cnt, a.head_hidden, grad + a.b1_off);
+    k_smp_embed<<<ew_grid((int64_t)d.R * S), 256, 0, st>>>(arena, net->d_addrs, b->row_step, b->step_prev_addr,
+                                                           b->row_prev, b->values, d.R, S, w.smp_emb);
+    PPB_LAUNCH_CHECK();
+  }
+  return PPB_OK;
+}
+
+// Every gradient that reduces dgates over the rows of a step, and every one that follows from d_pstep: d_pstep (an atomic
+// target, zeroed before the call), dW_ih[:, E:], db_ih, db_hh, the type / address embeddings and the sample-embedding layers
+int launch_step_inputs_bwd(const ppb_net* net, const float* arena, float* grad, const ppb_batch* b, const Ws& w,
+                           const float* dgates, cudaStream_t st) {
+  const ppb_net_desc& D = net->desc;
+  const Dims d = dims_of(b);
+  const int H4 = 4 * D.lstm_dim, E = D.obs_dim, S = D.sample_dim, I = net->I;
+  const int C2 = 2 * (D.type_dim + D.addr_dim);
+  // one pass over dgates: step column sums + sample-embedding gradients (S <= 4, 4H <= 2048); otherwise separate kernels
+  const bool one_pass = S <= 4 && H4 <= 2048;
+  int max_rows = 0;
+  for (int s = 0; s < d.NS; ++s) max_rows = b->step_nrows_host[s] > max_rows ? b->step_nrows_host[s] : max_rows;
+  if (one_pass) {
+    // rows per block: enough blocks to fill the SMs twice (a T = 1 minibatch of 256 rows used to be FOUR blocks walking
+    // 64 rows each: 44 us on the side branch that then bounded the step), at most kRedSlab
+    int slab = (d.R + 2 * PPB_NUM_SMS - 1) / (2 * PPB_NUM_SMS);
+    slab = slab < 4 ? 4 : (slab > kRedSlab ? kRedSlab : slab);
+    const dim3 g((max_rows + slab - 1) / slab, d.NS);
+    const float* wt = d.T > 1 ? w.w_smp_t : w.p_step;   // T = 1: no row has a previous site, the pointers are never read
+    if (H4 <= 1024)
+      k_dgates_reduce<4><<<g, 256, 0, st>>>(dgates, wt, w.smp_emb, b->values, b->step_prev_addr, b->step_row0, b->step_nrows,
+                                            b->row_prev, net->d_addrs, H4, S, I, E, w.d_pstep, grad, D.w_ih_off, slab);
+    else
+      k_dgates_reduce<8><<<g, 256, 0, st>>>(dgates, wt, w.smp_emb, b->values, b->step_prev_addr, b->step_row0, b->step_nrows,
+                                            b->row_prev, net->d_addrs, H4, S, I, E, w.d_pstep, grad, D.w_ih_off, slab);
+    PPB_LAUNCH_CHECK();
+  } else {
+    dim3 g((H4 + 31) / 32, d.NS);
+    k_step_colsum<<<g, 256, 0, st>>>(dgates, b->step_row0, b->step_nrows, H4, w.d_pstep);
+    PPB_LAUNCH_CHECK();
+  }
+  {
+    // about half an SM's worth of blocks split the d emb_cat columns (T = 1: one step segment, 5 column blocks); the weight
+    // and bias entries get one thread each
+    const int jbs = (C2 + 31) / 32;
+    int zsplit = PPB_NUM_SMS / 2 / (jbs * d.NS);
+    zsplit = zsplit < 1 ? 1 : (zsplit > 16 ? 16 : zsplit);
+    const int nx = jbs * d.NS * zsplit;
+    const int nw = (int)(((int64_t)H4 * C2 + H4 + 255) / 256);
+    k_pstep_bwd<<<nx + nw, 256, 0, st>>>(w.d_pstep, arena + D.w_ih_off, w.emb_cat, net->d_addrs, net->d_type_off, b->step_addr,
+                                         b->step_prev_addr, d.NS, H4, I, E + S, D.type_dim, D.addr_dim, zsplit, nx, grad,
+                                         D.w_ih_off, D.b_ih_off, D.b_hh_off);
+    PPB_LAUNCH_CHECK();
+  }
+  if (d.T > 1 && !one_pass) {
+    const int slab = 64;
+    k_smp_bwd_seg<<<dim3((max_rows + slab - 1) / slab, d.NS), 128, 0, st>>>(dgates, w.w_smp_t, w.smp_emb, b->values,
+                                                                           b->step_prev_addr, b->step_row0, b->step_nrows,
+                                                                           b->row_prev, net->d_addrs, H4, S, slab, grad);
+    PPB_LAUNCH_CHECK();
+    int rpb = 1024;
+    dim3 g((H4 + 255) / 256, (d.R + rpb - 1) / rpb);
+    k_wsmp_grad<<<g, 256, 0, st>>>(dgates, w.smp_emb, d.R, H4, S, I, E, grad + D.w_ih_off, rpb);
     PPB_LAUNCH_CHECK();
   }
   return PPB_OK;
@@ -1260,6 +1389,116 @@ int simt_head_bias_grad(const ppb_net* net, const ppb_batch* b, const Ws& w, flo
 
 #include "net_tc.inc"
 #include "net_ff.inc"
+
+namespace {
+
+// ---- LSTM network, fp32 SIMT path (precision 2) ------------------------------------------------------------------------
+int simt_loss_forward(ppb_net* net, const float* arena, const ppb_batch* b, void* workspace, float* loss_out,
+                      int32_t* status_out, float* row_lp_out, int want_grad, cudaStream_t st) {
+  PPB_CHECK_ARG(b->row_align == 1, "the SIMT path needs a batch encoded with row_align = 1");
+  const ppb_net_desc& D = net->desc;
+  Dims d = dims_of(b);
+  Ws w = carve(net, d, workspace);
+  const int H = D.lstm_dim, H4 = 4 * H, E = D.obs_dim, S = D.sample_dim, I = net->I;
+
+  // ---- problem lists for all forward GEMM phases -------------------------------------------------
+  Builder bl;
+  obs_fp32_plan_fwd(bl, D, arena, b->obs, d.B, w, w.obs_emb);
+  const int ph_p = (int)bl.phases.size();
+  bl.begin();
+  bl.add(linear_fwd(w.obs_emb, E, arena + D.w_ih_off, I, nullptr, w.p_obs, H4, d.B, H4, E, 0));
+  // recurrent GEMMs: gates[rows of t] = h[rows of t-1 (prefix)] W_hh^T
+  const int ph_rec0 = (int)bl.phases.size();
+  for (int t = 1; t < d.T; ++t) {
+    bl.begin();
+    int r0 = b->row_off_host[t], n = b->row_off_host[t + 1] - r0, rp = b->row_off_host[t - 1];
+    bl.add(linear_fwd(w.h + (int64_t)rp * H, H, arena + D.w_hh_off, H, nullptr, w.gates + (int64_t)r0 * H4, H4, n, H4, H, 0));
+  }
+  int ph_h1, ph_h2;
+  simt_head_fwd(bl, net, arena, b, w, H, ph_h1, ph_h2);
+  int rc = upload_and_get(net, bl, w.problems, w.max_problems / 2, st, 0);
+  if (rc) return rc;
+
+  // ---- launches -----------------------------------------------------------------------------------
+  PPB_CUDA(cudaMemsetAsync(w.loss_acc, 0, 256, st));
+  for (int l = 0; l < ph_p; ++l) { rc = run_phase(bl.phases[l], w.problems, st); if (rc) return rc; }
+  rc = launch_step_inputs_fwd(net, arena, b, w, st); if (rc) return rc;
+  rc = run_phase(bl.phases[ph_p], w.problems, st, &bl); if (rc) return rc;
+  for (int t = 0; t < d.T; ++t) {
+    int r0 = b->row_off_host[t], n = b->row_off_host[t + 1] - r0;
+    if (t > 0) { rc = run_phase(bl.phases[ph_rec0 + t - 1], w.problems, st, &bl); if (rc) return rc; }
+    k_cell_fwd<<<ew_grid((int64_t)n * H), 256, 0, st>>>(w.gates, w.p_obs, w.p_step, w.w_smp_t, w.smp_emb, b->row_step,
+                                                       b->row_prev, b->row_trace, w.c, w.h, HImg(), r0, n, H, S, t);
+    PPB_LAUNCH_CHECK();
+  }
+  return simt_head_nll(net, b, w, bl, ph_h1, ph_h2, loss_out, status_out, row_lp_out, want_grad, st);
+}
+
+int simt_loss_backward(ppb_net* net, const float* arena, float* grad, const ppb_batch* b, void* workspace, float grad_scale,
+                       cudaStream_t st) {
+  PPB_CHECK_ARG(b->step_nrows_host, "missing per-step host arrays");
+  const ppb_net_desc& D = net->desc;
+  Dims d = dims_of(b);
+  Ws w = carve(net, d, workspace);
+  float* dgates = dgates_ptr(w, workspace);
+  const int H = D.lstm_dim, H4 = 4 * H, E = D.obs_dim, I = net->I;
+
+  // d_pstep: atomic target of k_dgates_reduce
+  PPB_CUDA(cudaMemsetAsync(w.d_pstep, 0, (size_t)d.NS * H4 * sizeof(float), st));
+  if (grad_scale != 1.0f) {
+    k_scale<<<ew_grid((int64_t)d.R * net->out_pad), 256, 0, st>>>(w.d_out, (int64_t)d.R * net->out_pad, grad_scale);
+    PPB_LAUNCH_CHECK();
+  }
+
+  Builder bl;
+  const int ph_dhid = 0, ph_hw = 1;
+  simt_head_bwd(bl, net, arena, grad, b, w, H);
+  // BPTT recurrent: dh_rec[prefix rows of t-1] = dgates[rows of t] W_hh
+  const int ph_rec0 = 2;
+  for (int t = d.T - 1; t >= 1; --t) {
+    bl.begin();
+    int r0 = b->row_off_host[t], n = b->row_off_host[t + 1] - r0;
+    bl.add(linear_dx(dgates + (int64_t)r0 * H4, H4, arena + D.w_hh_off, H, w.dh_rec + (int64_t)b->row_off_host[t - 1] * H, H, n, H4, H, 0));
+  }
+  const int ph_lstm_w = (int)bl.phases.size();
+  bl.begin();
+  {
+    // dW_hh += sum_{rows t>=1} dgates[row]^T h[row_prev[row]]
+    int r1 = b->row_off_host[1 < d.T ? 1 : d.T];
+    int n1 = d.R - r1;
+    if (n1 > 0) {
+      Problem p = linear_dw(dgates + (int64_t)r1 * H4, H4, w.h, H, grad + D.w_hh_off, H, n1, H4, H);
+      p.kb_gather = b->row_prev + r1;  // h row of the previous step
+      bl.add(p);
+    }
+    // dW_ih[:, :E] += d_pobs^T obs_emb ; d obs_emb = d_pobs W_ih[:, :E]
+    bl.add(linear_dw(w.d_pobs, H4, w.obs_emb, E, grad + D.w_ih_off, I, d.B, H4, E));
+    bl.add(linear_dx(w.d_pobs, H4, arena + D.w_ih_off, I, w.d_obs_emb, E, d.B, H4, E, 0));
+  }
+  const int ph_obs = obs_fp32_plan_bwd(bl, D, arena, grad, b->obs, d.B, w);
+  Problem* dprobs = w.problems + w.max_problems / 2;
+  int rc = upload_and_get(net, bl, dprobs, w.max_problems / 2, st, 1);
+  if (rc) return rc;
+
+  // ---- launches -----------------------------------------------------------------------------------
+  rc = run_phase(bl.phases[ph_dhid], dprobs, st); if (rc) return rc;
+  rc = run_phase(bl.phases[ph_hw], dprobs, st); if (rc) return rc;
+  rc = launch_head_bias_grad(net, b, w, grad, st); if (rc) return rc;
+  // BPTT
+  for (int t = d.T - 1; t >= 0; --t) {
+    int r0 = b->row_off_host[t], n = b->row_off_host[t + 1] - r0;
+    int n_next = (t + 1 < d.T) ? b->row_off_host[t + 2] - b->row_off_host[t + 1] : 0;
+    if (n_next > 0) { rc = run_phase(bl.phases[ph_rec0 + (d.T - 2 - t)], dprobs, st, &bl); if (rc) return rc; }
+    k_cell_bwd<false><<<ew_grid((int64_t)n * H), 256, 0, st>>>(w.gates, w.c, w.dh, w.dh_rec, w.dc, dgates, w.d_pobs, b->row_prev,
+                                                       b->row_next, b->row_trace, HImg(), r0, n, H, t, HImg());
+    PPB_LAUNCH_CHECK();
+  }
+  rc = launch_step_inputs_bwd(net, arena, grad, b, w, dgates, st); if (rc) return rc;
+  rc = run_phase(bl.phases[ph_lstm_w], dprobs, st, &bl); if (rc) return rc;
+  return obs_fp32_bwd(bl, ph_obs, dprobs, D, grad, d.B, w, st);
+}
+
+}  // namespace
 
 // =====================================================================================================
 extern "C" {
@@ -1363,63 +1602,14 @@ int ppb_ic_loss_forward(ppb_net* net, const float* arena, const ppb_batch* b, vo
   PPB_CHECK_ARG(arena && workspace, "null arena/workspace");
   PPB_CHECK_ARG(!net->addrs.empty(), "address tables not set");
   PPB_CHECK_ARG(precision >= 0 && precision <= 2, "unknown precision mode");
-  const ppb_net_desc& D = net->desc;
   Dims d = dims_of(b);
   PPB_CHECK_ARG(workspace_bytes >= ppb_ic_workspace_bytes(net, d.B, d.R, d.T, d.NS, d.G), "workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
-  if (D.network_type == PPB_NET_FEEDFORWARD)
+  if (net->desc.network_type == PPB_NET_FEEDFORWARD)
     return ff_loss_forward(net, arena, b, workspace, precision, loss_out, status_out, row_lp_out, want_grad, st);
   if (precision != PPB_PREC_FP32_SIMT)
     return tc_loss_forward(net, arena, b, workspace, precision, loss_out, status_out, row_lp_out, want_grad, st);
-  PPB_CHECK_ARG(b->row_align == 1, "the SIMT path needs a batch encoded with row_align = 1");
-  Ws w = carve(net, d, workspace);
-  const int H = D.lstm_dim, H4 = 4 * H, E = D.obs_dim, S = D.sample_dim, I = net->I;
-  const int C2 = 2 * (D.type_dim + D.addr_dim);
-
-  // ---- problem lists for all forward GEMM phases -------------------------------------------------
-  Builder bl;
-  obs_fp32_plan_fwd(bl, D, arena, b->obs, d.B, w, w.obs_emb);
-  const int ph_obs0 = 0;
-  const int ph_p = (int)bl.phases.size();
-  bl.begin();
-  bl.add(linear_fwd(w.obs_emb, E, arena + D.w_ih_off, I, nullptr, w.p_obs, H4, d.B, H4, E, 0));
-  bl.add(linear_fwd(w.emb_cat, C2, arena + D.w_ih_off + E + S, I, arena + D.b_ih_off, w.p_step, H4, d.NS, H4, C2, 0));
-  // recurrent GEMMs: gates[rows of t] = h[rows of t-1 (prefix)] W_hh^T
-  const int ph_rec0 = (int)bl.phases.size();
-  for (int t = 1; t < d.T; ++t) {
-    bl.begin();
-    int r0 = b->row_off_host[t], n = b->row_off_host[t + 1] - r0, rp = b->row_off_host[t - 1];
-    bl.add(linear_fwd(w.h + (int64_t)rp * H, H, arena + D.w_hh_off, H, nullptr, w.gates + (int64_t)r0 * H4, H4, n, H4, H, 0));
-  }
-  int ph_h1, ph_h2;
-  simt_head_fwd(bl, net, arena, b, w, H, ph_h1, ph_h2);
-  rc = upload_and_get(net, bl, w.problems, w.max_problems / 2, st, 0);
-  if (rc) return rc;
-
-  // ---- launches -----------------------------------------------------------------------------------
-  PPB_CUDA(cudaMemsetAsync(w.loss_acc, 0, 256, st));
-  for (int l = ph_obs0; l < ph_p; ++l) { rc = run_phase(bl.phases[l], w.problems, st); if (rc) return rc; }
-  k_step_embed<<<ew_grid((int64_t)d.NS * C2), 256, 0, st>>>(arena, net->d_addrs, net->d_type_off, b->step_addr,
-                                                            b->step_prev_addr, d.NS, D.type_dim, D.addr_dim, w.emb_cat);
-  PPB_LAUNCH_CHECK();
-  k_wsmp_transpose<<<ew_grid(S * H4), 256, 0, st>>>(arena + D.w_ih_off, I, E, S, H4, w.w_smp_t);
-  PPB_LAUNCH_CHECK();
-  k_smp_embed<<<ew_grid((int64_t)d.R * S), 256, 0, st>>>(arena, net->d_addrs, b->row_step, b->step_prev_addr,
-                                                         b->row_prev, b->values, d.R, S, w.smp_emb);
-  PPB_LAUNCH_CHECK();
-  rc = run_phase(bl.phases[ph_p], w.problems, st, &bl);
-  if (rc) return rc;
-  // b_hh joins the step projection (P_step already has b_ih): add once with a scaled-axpy kernel
-  k_add_row_bias<<<ew_grid((int64_t)d.NS * H4), 256, 0, st>>>(w.p_step, arena + D.b_hh_off, (int64_t)d.NS * H4, H4);
-  PPB_LAUNCH_CHECK();
-  for (int t = 0; t < d.T; ++t) {
-    int r0 = b->row_off_host[t], n = b->row_off_host[t + 1] - r0;
-    if (t > 0) { rc = run_phase(bl.phases[ph_rec0 + t - 1], w.problems, st, &bl); if (rc) return rc; }
-    k_cell_fwd<<<ew_grid((int64_t)n * H), 256, 0, st>>>(w.gates, w.p_obs, w.p_step, w.w_smp_t, w.smp_emb, b->row_step,
-                                                       b->row_prev, b->row_trace, w.c, w.h, HImg(), r0, n, H, S, t);
-    PPB_LAUNCH_CHECK();
-  }
-  return simt_head_nll(net, b, w, bl, ph_h1, ph_h2, loss_out, status_out, row_lp_out, want_grad, st);
+  return simt_loss_forward(net, arena, b, workspace, loss_out, status_out, row_lp_out, want_grad, st);
 }
 
 int ppb_ic_loss_backward(ppb_net* net, const float* arena, float* grad, const ppb_batch* b, void* workspace,
@@ -1427,89 +1617,13 @@ int ppb_ic_loss_backward(ppb_net* net, const float* arena, float* grad, const pp
   int rc = check_batch(net, b);
   if (rc) return rc;
   PPB_CHECK_ARG(arena && grad && workspace, "null arena/grad/workspace");
-  const ppb_net_desc& D = net->desc;
   Dims d = dims_of(b);
   PPB_CHECK_ARG(workspace_bytes >= ppb_ic_workspace_bytes(net, d.B, d.R, d.T, d.NS, d.G), "workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
-  if (D.network_type == PPB_NET_FEEDFORWARD) return ff_loss_backward(net, arena, grad, b, workspace, precision, grad_scale, st);
+  if (net->desc.network_type == PPB_NET_FEEDFORWARD)
+    return ff_loss_backward(net, arena, grad, b, workspace, precision, grad_scale, st);
   if (precision != PPB_PREC_FP32_SIMT) return tc_loss_backward(net, arena, grad, b, workspace, precision, grad_scale, st);
-  Ws w = carve(net, d, workspace);
-  float* dgates = dgates_ptr(w, workspace);
-  const int H = D.lstm_dim, H4 = 4 * H, E = D.obs_dim, S = D.sample_dim, I = net->I;
-  const int C2 = 2 * (D.type_dim + D.addr_dim);
-
-  if (grad_scale != 1.0f) {
-    k_scale<<<ew_grid((int64_t)d.R * net->out_pad), 256, 0, st>>>(w.d_out, (int64_t)d.R * net->out_pad, grad_scale);
-    PPB_LAUNCH_CHECK();
-  }
-
-  Builder bl;
-  const int ph_dhid = 0, ph_hw = 1;
-  simt_head_bwd(bl, net, arena, grad, b, w, H);
-  // BPTT recurrent: dh_rec[prefix rows of t-1] = dgates[rows of t] W_hh
-  const int ph_rec0 = 2;
-  for (int t = d.T - 1; t >= 1; --t) {
-    bl.begin();
-    int r0 = b->row_off_host[t], n = b->row_off_host[t + 1] - r0;
-    bl.add(linear_dx(dgates + (int64_t)r0 * H4, H4, arena + D.w_hh_off, H, w.dh_rec + (int64_t)b->row_off_host[t - 1] * H, H, n, H4, H, 0));
-  }
-  const int ph_lstm_w = (int)bl.phases.size();
-  bl.begin();
-  {
-    // dW_hh += sum_{rows t>=1} dgates[row]^T h[row_prev[row]]
-    int r1 = b->row_off_host[1 < d.T ? 1 : d.T];
-    int n1 = d.R - r1;
-    if (n1 > 0) {
-      Problem p = linear_dw(dgates + (int64_t)r1 * H4, H4, w.h, H, grad + D.w_hh_off, H, n1, H4, H);
-      p.kb_gather = b->row_prev + r1;  // h row of the previous step
-      bl.add(p);
-    }
-    // dW_ih[:, :E] += d_pobs^T obs_emb ; dW_ih[:, E+S:] += d_pstep^T emb_cat
-    bl.add(linear_dw(w.d_pobs, H4, w.obs_emb, E, grad + D.w_ih_off, I, d.B, H4, E));
-    bl.add(linear_dw(w.d_pstep, H4, w.emb_cat, C2, grad + D.w_ih_off + E + S, I, d.NS, H4, C2));
-    // d obs_emb = d_pobs W_ih[:, :E] ; d emb_cat = d_pstep W_ih[:, E+S:]
-    bl.add(linear_dx(w.d_pobs, H4, arena + D.w_ih_off, I, w.d_obs_emb, E, d.B, H4, E, 0));
-    bl.add(linear_dx(w.d_pstep, H4, arena + D.w_ih_off + E + S, I, w.d_embcat, C2, d.NS, H4, C2, 0));
-  }
-  const int ph_obs = obs_fp32_plan_bwd(bl, D, arena, grad, b->obs, d.B, w);
-  Problem* dprobs = w.problems + w.max_problems / 2;
-  rc = upload_and_get(net, bl, dprobs, w.max_problems / 2, st, 1);
-  if (rc) return rc;
-
-  // ---- launches -----------------------------------------------------------------------------------
-  rc = run_phase(bl.phases[ph_dhid], dprobs, st); if (rc) return rc;
-  rc = run_phase(bl.phases[ph_hw], dprobs, st); if (rc) return rc;
-  rc = simt_head_bias_grad(net, b, w, grad, st); if (rc) return rc;
-  // BPTT
-  for (int t = d.T - 1; t >= 0; --t) {
-    int r0 = b->row_off_host[t], n = b->row_off_host[t + 1] - r0;
-    int n_next = (t + 1 < d.T) ? b->row_off_host[t + 2] - b->row_off_host[t + 1] : 0;
-    if (n_next > 0) { rc = run_phase(bl.phases[ph_rec0 + (d.T - 2 - t)], dprobs, st, &bl); if (rc) return rc; }
-    k_cell_bwd<false><<<ew_grid((int64_t)n * H), 256, 0, st>>>(w.gates, w.c, w.dh, w.dh_rec, w.dc, dgates, w.d_pobs, b->row_prev,
-                                                       b->row_next, b->row_trace, HImg(), r0, n, H, t, HImg());
-    PPB_LAUNCH_CHECK();
-  }
-  {
-    dim3 g((H4 + 31) / 32, d.NS);
-    k_step_colsum<<<g, 256, 0, st>>>(dgates, b->step_row0, b->step_nrows, H4, w.d_pstep);
-    PPB_LAUNCH_CHECK();
-  }
-  rc = run_phase(bl.phases[ph_lstm_w], dprobs, st, &bl); if (rc) return rc;
-  k_bias_grad<<<(H4 + 255) / 256, 256, 0, st>>>(w.d_pstep, d.NS, H4, grad + D.b_ih_off, grad + D.b_hh_off);
-  PPB_LAUNCH_CHECK();
-  k_embed_scatter<<<ew_grid((int64_t)d.NS * C2), 256, 0, st>>>(w.d_embcat, net->d_addrs, net->d_type_off, b->step_addr,
-                                                               b->step_prev_addr, d.NS, D.type_dim, D.addr_dim, grad);
-  PPB_LAUNCH_CHECK();
-  if (d.T > 1) {
-    k_smp_bwd<<<ew_grid((int64_t)d.R * 32, 128), 128, 0, st>>>(dgates, w.w_smp_t, w.smp_emb, b->values, b->row_step,
-                                                              b->step_prev_addr, b->row_prev, net->d_addrs, d.R, H4, S, grad);
-    PPB_LAUNCH_CHECK();
-    int rpb = 256;
-    dim3 g((H4 + 255) / 256, (d.R + rpb - 1) / rpb);
-    k_wsmp_grad<<<g, 256, 0, st>>>(dgates, w.smp_emb, d.R, H4, S, I, E, grad + D.w_ih_off, rpb);
-    PPB_LAUNCH_CHECK();
-  }
-  return obs_fp32_bwd(bl, ph_obs, dprobs, D, grad, d.B, w, st);
+  return simt_loss_backward(net, arena, grad, b, workspace, grad_scale, st);
 }
 
 }  // extern "C"
@@ -1657,16 +1771,7 @@ __global__ void k_smp_embed_infer(const float* __restrict__ arena, ppb_addr_desc
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n * S; e += (int64_t)gridDim.x * blockDim.x) {
     int64_t i = e / S;
     int j = (int)(e % S);
-    float x = value[i];
-    const float* W = arena + a.smp_w_off + (int64_t)j * a.smp_in;
-    float pre = arena[a.smp_b_off + j];
-    if (a.family == PPB_FAMILY_CATEGORICAL) {
-      int cidx = (int)x;
-      if (cidx >= 0 && cidx < a.smp_in) pre += W[cidx];
-    } else {
-      pre += W[0] * x;
-    }
-    smp_emb[e] = fmaxf(pre, 0.0f);
+    smp_emb[e] = fmaxf(smp_embed_pre(arena, a, value[i], j), 0.0f);
   }
 }
 
@@ -1674,14 +1779,11 @@ __global__ void k_step_row_infer(const float* __restrict__ arena, ppb_addr_desc 
                                  const int64_t* __restrict__ type_off, int td, int ad, float* __restrict__ row) {
   int C2 = 2 * (td + ad);
   for (int j = threadIdx.x; j < C2; j += blockDim.x) {
-    bool is_prev = j < td + ad;
-    int jj = is_prev ? j : j - (td + ad);
-    float v = 0.0f;
-    if (!is_prev || has_prev) {
-      const ppb_addr_desc& a = is_prev ? prev : cur;
-      v = jj < td ? arena[type_off[a.type_id] + jj] : arena[a.addr_emb_off + (jj - td)];
-    }
-    row[j] = v;
+    const int64_t o = step_embed_off(type_off, td, ad, j, [&](bool is_prev, const ppb_addr_desc*& a) {
+      a = is_prev ? &prev : &cur;
+      return !is_prev || has_prev;
+    });
+    row[j] = o >= 0 ? arena[o] : 0.0f;
   }
 }
 

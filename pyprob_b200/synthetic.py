@@ -23,7 +23,7 @@ class _ExampleTrace:
 
 
 def build_network(observe_embeddings, observe_in_dims, addresses, lstm_dim=512, mixture_components=10, precision=0,
-                  seed=0, inference_network=InferenceNetwork.LSTM):
+                  seed=0, inference_network=InferenceNetwork.LSTM, sample_embedding_dim=4):
     """addresses: list of (address, distribution name, num_categories) in address-id order."""
     torch.manual_seed(seed)
     if inference_network == InferenceNetwork.FEEDFORWARD:
@@ -31,6 +31,7 @@ def build_network(observe_embeddings, observe_in_dims, addresses, lstm_dim=512, 
                                           proposal_mixture_components=mixture_components, precision=precision)
     else:
         net = InferenceNetworkLSTM(model=None, observe_embeddings=observe_embeddings, lstm_dim=lstm_dim,
+                                   sample_embedding_dim=sample_embedding_dim,
                                    proposal_mixture_components=mixture_components, precision=precision)
     shapes = {name: (d,) if d > 1 else () for name, d in zip(observe_embeddings.keys(), observe_in_dims)}
     net._ensure_initialized(_ExampleTrace(shapes))
