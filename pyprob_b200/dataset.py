@@ -7,7 +7,7 @@
 import numpy as np
 import torch
 
-from .distributions import Categorical, Normal, Uniform, set_shard_first_index
+from .distributions import Categorical, set_shard_first_index
 from .encoding import EncodedBatch, SubBatch
 from .util import PriorInflation, TraceMode
 
@@ -63,13 +63,8 @@ class TraceBatch:
                     return None
                 ids.append(net._addresses[s.address]['id'])
                 vc.append(push(s.value))
-                d = s.distribution
-                if isinstance(d, Normal):
-                    p0c.append(param(d.loc)); p1c.append(param(d.scale))
-                elif isinstance(d, Uniform):
-                    p0c.append(param(d.low)); p1c.append(param(d.high))
-                else:
-                    p0c.append(-1); p1c.append(-1)
+                p0, p1 = s.distribution._prior_params()
+                p0c.append(-1 if p0 is None else param(p0)); p1c.append(-1 if p1 is None else param(p1))
             plan.append((ids, vc, p0c, p1c, idx))
         ncols = len(cols)
         host = torch.cat([torch.stack(cols, dim=0), obs_mat.t()], dim=0).cpu().numpy()  # one device->host copy
@@ -106,12 +101,9 @@ class TraceBatch:
                 families.append(d.name)
                 cats.append(d.num_categories if isinstance(d, Categorical) else 0)
                 vals.append(host(s.value)[sel])
-                if isinstance(d, Normal):
-                    p0.append(host(d.loc)[sel]); p1.append(host(d.scale)[sel])
-                elif isinstance(d, Uniform):
-                    p0.append(host(d.low)[sel]); p1.append(host(d.high)[sel])
-                else:
-                    p0.append(zeros[sel]); p1.append(zeros[sel])
+                q0, q1 = d._prior_params()
+                p0.append((zeros if q0 is None else host(q0))[sel])
+                p1.append((zeros if q1 is None else host(q1))[sel])
             subs.append({'addresses': addresses, 'families': families, 'num_categories': cats,
                          'values': np.stack(vals, 0), 'prior0': np.stack(p0, 0), 'prior1': np.stack(p1, 0),
                          'obs': obs[sel]})

@@ -258,6 +258,11 @@ class Distribution:
     def stddev(self):
         return self.variance ** 0.5 if torch.is_tensor(self.variance) else math.sqrt(self.variance)
 
+    def _prior_params(self):
+        """The prior parameters a proposal head takes as inputs: (loc, scale) for Normal, (low, high) for Uniform,
+        (None, None) for the other families."""
+        return None, None
+
     def _seed_args(self):
         return util._seed, util.next_draw_offset(), _shard_first_index
 
@@ -295,6 +300,9 @@ class Normal(_ElementWise):
     variance = property(lambda self: self.scale ** 2)
     stddev = property(lambda self: self.scale)
 
+    def _prior_params(self):
+        return self.loc, self.scale
+
     def __repr__(self):
         return 'Normal({}, {})'.format(self.loc, self.scale)
 
@@ -306,6 +314,9 @@ class Uniform(_ElementWise):
 
     mean = property(lambda self: (self.low + self.high) / 2)
     variance = property(lambda self: (self.high - self.low) ** 2 / 12)
+
+    def _prior_params(self):
+        return self.low, self.high
 
     def __repr__(self):
         return 'Uniform(low={}, high={})'.format(self.low, self.high)

@@ -99,8 +99,8 @@ class _LossFunction(torch.autograd.Function):
 class InferenceNetwork(nn.Module):
     """What does not depend on the network type (reference pyprob/nn/inference_network.py): the parameter arena, the
     observation layers, the loss call, the optimisers and the training loop, data-parallel training, checkpoints,
-    workspaces and `_infer_init`.  Subclasses add the proposal layers of an address (`_add_address`), the native
-    network description (`_fill_net_desc`, `_fill_addr_desc`), the infer step and `_segment_presence`."""
+    workspaces, `_infer_init` and the infer step.  Subclasses add the proposal layers of an address (`_add_address`),
+    the native network description (`_fill_net_desc`, `_fill_addr_desc`) and `_segment_presence`."""
 
     def __init__(self, model=None, observe_embeddings={}, proposal_mixture_components=10, precision=0,
                  network_type=''):
@@ -174,7 +174,6 @@ class InferenceNetwork(nn.Module):
         self._image_host = None
         self._loss_buf = None
         # inference state
-        self._infer_observe = None
         self._infer_observe_embedding = None
 
     # ------------------------------------------------------------------------------------------------
@@ -281,7 +280,8 @@ class InferenceNetwork(nn.Module):
         self._rebind()
 
     def _proposal_layers(self, address, family, num_categories, in_dim):
-        """The proposal head of an address (proposal_*.py: EmbeddingFeedForward(in_dim -> out, 2 layers)) -> its info."""
+        """The proposal head of an address (proposal_*.py: EmbeddingFeedForward(in_dim -> out, 2 layers)) -> its info:
+        the head's widths and `smp_in`, the width of the address's value as a sample-embedding input."""
         K = self._proposal_mixture_components
         # proposal_categorical_categorical.py: C logits; proposal_bernoulli_bernoulli.py: one logit; mixtures: 3K
         out = num_categories if family == FAMILY_CATEGORICAL else 1 if family == FAMILY_BERNOULLI else 3 * K
@@ -289,7 +289,7 @@ class InferenceNetwork(nn.Module):
         p = '_layers_proposal.{}._ff._layers'.format(address)
         self._linear(p + '.0', in_dim, hidden)
         self._linear(p + '.1', hidden, out)
-        return dict(head_hidden=hidden, head_out=out)
+        return dict(head_hidden=hidden, head_out=out, smp_in=num_categories if family == FAMILY_CATEGORICAL else 1)
 
     def _ensure_initialized(self, example_trace):
         if not self._layers_initialized:
@@ -845,7 +845,6 @@ class InferenceNetwork(nn.Module):
     def _infer_init(self, observe=None):
         """Embed the (single) observation once; `observe` maps names to values."""
         self._sync_native()
-        self._infer_observe = observe
         vals = []
         for name, in_dim in zip(self._observe_names, self._observe_in_dims):
             v = torch.as_tensor(observe[name], dtype=torch.float32).reshape(-1)
@@ -867,6 +866,48 @@ class InferenceNetwork(nn.Module):
             cache = {info['id']: a for a, info in self._addresses.items()}
             self._by_id_cache = cache
         return cache
+
+    def _infer_step_lanes(self, address, prior0, prior1, m, prev_address=None, prev_value=None, h=None, c=None):
+        """One proposal step for m particles at `address`.  The LSTM passes the site they came from (`prev_address`,
+        None: first controlled site, with values `prev_value` [m]) and their state rows `h`, `c` ([m, H] contiguous,
+        updated in place); a feed-forward head reads the shared observation embedding alone.  Returns the proposal
+        parameters [m, head_out]: means|stddevs|probs [m, 3K], [m, C] or [m, 1] (Bernoulli probs)."""
+        info = self._addresses[address]
+        params = torch.empty(m, info['head_out'], dtype=torch.float32, device='cuda')
+        need = self._infer_workspace(m)
+
+        def par(x):
+            if x is None:
+                return None, 0
+            t = ops._f32(x, 'cuda').reshape(-1)      # python scalars: cached device constants (no host->device copy)
+            return t, (0 if t.numel() == 1 else 1)
+        p0, s0 = par(prior0)
+        p1, s1 = par(prior1)
+        pv = None if prev_value is None else prev_value.to(dtype=torch.float32).contiguous()
+        call('ppb_ic_infer_step', self._handle, ptr(self._arena.data), ptr(self._infer_observe_embedding), 0,
+             -1 if prev_address is None else self._addresses[prev_address]['id'], ptr(pv), info['id'],
+             ptr(p0), s0, ptr(p1), s1, ptr(h), ptr(c), ptr(params), m, ptr(self._infer_ws), need, self._precision,
+             stream())
+        return params
+
+    def _infer_step_batched(self, address, prev_address, prev_value, prior0, prior1, n):
+        """Proposal parameters for n particles in lock-step at `address`, all coming from `prev_address` with values
+        `prev_value`.  The LSTM keeps its state from the previous call, reset when `prev_address` is None or n changes;
+        the feed-forward network ignores the previous site.
+
+        Returns a [n, head_out] tensor, or None if the address (LSTM: or the previous address) is unknown (the caller
+        then falls back to the prior, as the reference does with a warning)."""
+        lstm = isinstance(self, InferenceNetworkLSTM)
+        unknown_prev = lstm and prev_address is not None and prev_address not in self._addresses
+        if address not in self._addresses or unknown_prev:
+            warnings.warn('Address unknown by inference network: {}'.format(address))
+            return None
+        if not lstm:
+            return self._infer_step_lanes(address, prior0, prior1, n)
+        if prev_address is None or self._infer_state is None or self._infer_state[0].size(0) != n:
+            self._infer_state = (torch.zeros(n, self._lstm_dim, device='cuda'),
+                                 torch.zeros(n, self._lstm_dim, device='cuda'))
+        return self._infer_step_lanes(address, prior0, prior1, n, prev_address, prev_value, *self._infer_state)
 
 
 class InferenceNetworkLSTM(InferenceNetwork):
@@ -911,10 +952,10 @@ class InferenceNetworkLSTM(InferenceNetwork):
                         torch.zeros(self._distribution_type_embedding_dim).normal_())
             self._types[dist_name] = len(self._types)
         head = self._proposal_layers(address, family, num_categories, self._lstm_dim)
-        smp_in = num_categories if family == FAMILY_CATEGORICAL else 1
-        self._linear('_layers_sample_embedding.{}._layers.0'.format(address), smp_in, self._sample_embedding_dim)
+        self._linear('_layers_sample_embedding.{}._layers.0'.format(address), head['smp_in'],
+                     self._sample_embedding_dim)
         self._addresses[address] = dict(id=len(self._addresses), family=family, num_categories=num_categories,
-                                        smp_in=smp_in, type=dist_name, **head)
+                                        type=dist_name, **head)
         self._head_iterations[address] = 0
 
     def _segment_presence(self, enc, force=False):
@@ -944,62 +985,6 @@ class InferenceNetworkLSTM(InferenceNetwork):
                 a = name[len('_layers_sample_embedding.'):name.index('._layers.')]
                 present[k] = int(self._addresses[a]['id'] in prev)
         return present
-
-    def _infer_step_lanes(self, address, prev_address, prev_value, prior0, prior1, h, c):
-        """One proposal step for the particles whose LSTM state rows are `h`, `c` ([m, H] contiguous, updated in place):
-        all m particles sit at `address` and came from `prev_address` (None: first controlled site) with values
-        `prev_value` [m].  Returns the proposal parameters [m, 3K] (means|stddevs|probs), [m, C] or [m, 1] (Bernoulli
-        probs)."""
-        info = self._addresses[address]
-        m = h.size(0)
-        width = info['head_out'] if info['family'] != FAMILY_CATEGORICAL else info['num_categories']
-        params = torch.empty(m, width, dtype=torch.float32, device='cuda')
-        need = self._infer_workspace(m)
-
-        def par(x):
-            if x is None:
-                return None, 0, None
-            t = ops._f32(x, 'cuda').reshape(-1)      # python scalars: cached device constants (no host->device copy)
-            return t, (0 if t.numel() == 1 else 1), t
-        p0, s0, k0 = par(prior0)
-        p1, s1, k1 = par(prior1)
-        pv = None if prev_value is None else prev_value.to(dtype=torch.float32).contiguous()
-        call('ppb_ic_infer_step', self._handle, ptr(self._arena.data), ptr(self._infer_observe_embedding), 0,
-             -1 if prev_address is None else self._addresses[prev_address]['id'], ptr(pv), info['id'],
-             ptr(p0), s0, ptr(p1), s1, ptr(h), ptr(c), ptr(params), m, ptr(self._infer_ws), need, self._precision,
-             stream())
-        return params
-
-    def _infer_step_batched(self, address, prev_address, prev_value, prior0, prior1, n):
-        """Proposal parameters for n particles in lock-step at `address`.
-
-        Returns a [n, 3K] (means|stddevs|probs), [n, C] or [n, 1] (Bernoulli probs) tensor, or None if the address is unknown
-        (the caller then falls back to the prior, as the reference does with a warning)."""
-        if address not in self._addresses or (prev_address is not None and prev_address not in self._addresses):
-            warnings.warn('Address unknown by inference network: {}'.format(address))
-            return None
-        info = self._addresses[address]
-        H = self._lstm_dim
-        if prev_address is None or self._infer_state is None or self._infer_state[0].size(0) != n:
-            self._infer_state = (torch.zeros(n, H, device='cuda'), torch.zeros(n, H, device='cuda'))
-        h, c = self._infer_state
-        width = info['head_out'] if info['family'] != FAMILY_CATEGORICAL else info['num_categories']
-        params = torch.empty(n, width, dtype=torch.float32, device='cuda')
-        need = self._infer_workspace(n)
-
-        def par(x):
-            if x is None:
-                return None, 0, None
-            t = torch.as_tensor(x, dtype=torch.float32, device='cuda').reshape(-1)
-            return t, (0 if t.numel() == 1 else 1), t
-        p0, s0, k0 = par(prior0)
-        p1, s1, k1 = par(prior1)
-        pv = None if prev_value is None else prev_value.to(dtype=torch.float32).contiguous()
-        call('ppb_ic_infer_step', self._handle, ptr(self._arena.data), ptr(self._infer_observe_embedding), 0,
-             -1 if prev_address is None else self._addresses[prev_address]['id'], ptr(pv), info['id'],
-             ptr(p0), s0, ptr(p1), s1, ptr(h), ptr(c), ptr(params), n, ptr(self._infer_ws), need, self._precision,
-             stream())
-        return params
 
     def _fill_net_desc(self, nd):
         nd.network_type = NET_LSTM
@@ -1035,8 +1020,7 @@ class InferenceNetworkFeedForward(InferenceNetwork):
         family = _FAMILY_OF[dist_name]
         head = self._proposal_layers(address, family, num_categories, self._observe_embedding_dim)
         self._addresses[address] = dict(id=len(self._addresses), family=family, num_categories=num_categories,
-                                        smp_in=1 if family != FAMILY_CATEGORICAL else num_categories, type=dist_name,
-                                        **head)
+                                        type=dist_name, **head)
         self._head_iterations[address] = 0
 
     def _fill_net_desc(self, nd):
@@ -1057,31 +1041,3 @@ class InferenceNetworkFeedForward(InferenceNetwork):
                 a = name[len('_layers_proposal.'):name.index('._ff._layers.')]
                 present[k] = int(self._addresses[a]['id'] in cur)
         return present
-
-    def _infer_step_lanes(self, address, prior0, prior1, m):
-        """Proposal parameters at `address` for m particles (_infer_step, :53-66): the head runs once on the shared
-        observation embedding; only the priors differ per particle.  [m, 3K] (means|stddevs|probs), [m, C] or [m, 1]."""
-        info = self._addresses[address]
-        width = info['head_out'] if info['family'] != FAMILY_CATEGORICAL else info['num_categories']
-        params = torch.empty(m, width, dtype=torch.float32, device='cuda')
-        need = self._infer_workspace(m)
-
-        def par(x):
-            if x is None:
-                return None, 0
-            t = ops._f32(x, 'cuda').reshape(-1)      # python scalars: cached device constants (no host->device copy)
-            return t, (0 if t.numel() == 1 else 1)
-        p0, s0 = par(prior0)
-        p1, s1 = par(prior1)
-        call('ppb_ic_infer_step', self._handle, ptr(self._arena.data), ptr(self._infer_observe_embedding), 0, -1, None,
-             info['id'], ptr(p0), s0, ptr(p1), s1, None, None, ptr(params), m, ptr(self._infer_ws), need,
-             self._precision, stream())
-        return params
-
-    def _infer_step_batched(self, address, prev_address, prev_value, prior0, prior1, n):
-        """As InferenceNetworkLSTM._infer_step_batched; the previous site plays no part.  None if the address is unknown
-        (the caller then falls back to the prior)."""
-        if address not in self._addresses:
-            warnings.warn('Address unknown by inference network: {}'.format(address))
-            return None
-        return self._infer_step_lanes(address, prior0, prior1, n)

@@ -26,14 +26,12 @@ _likelihood_importance = 1.0
 _current_trace = None
 _root_function_name = None
 _network = None
-_previous_site = None
 _observed = {}
 _mask = None            # bool [n] of lanes executing the current statement, None = all
 _mask_idx = None        # indices of the lanes of _mask (computed once per while_loop iteration), or None
 _mask_parent = None     # the mask this one was narrowed from (while_loop: the previous iteration's mask)
 _trace_start = None
 _target_cache = {}
-_NO_MASK_YET = object()
 _mcmc = None            # the mcmc.Chains whose candidate traces this execution writes (LMH / RMH), or None
 
 
@@ -131,14 +129,6 @@ def _accumulate(trace, fn):
         trace.log_w.add_(term.masked_fill_(~_mask, 0.0))   # masked-out lanes may hold junk (even NaN): dropped
 
 
-def _prior_params(distribution):
-    if isinstance(distribution, Normal):
-        return distribution.loc, distribution.scale
-    if isinstance(distribution, Uniform):
-        return distribution.low, distribution.high
-    return None, None
-
-
 # ---- public statements ----------------------------------------------------------------------------------------
 def tag(value, name=None, address=None):
     if _current_trace is None:
@@ -181,7 +171,6 @@ def observe(distribution, value=None, name=None, address=None):
 
 
 def sample(distribution, name=None, address=None, control=True):
-    global _previous_site
     trace = _current_trace
     if trace is None:
         return distribution.sample()
@@ -218,10 +207,7 @@ def sample(distribution, name=None, address=None, control=True):
                     distribution.score_into(value, acc, 1.0)
                     acc.sub_(q_lp.double())
                 _accumulate(trace, fn)
-    site = Site(distribution, value, base, addr, instance, control=control, name=name, mask=_mask)
-    trace.add(site)
-    if use_network:
-        _previous_site = site
+    trace.add(Site(distribution, value, base, addr, instance, control=control, name=name, mask=_mask))
     return value
 
 
@@ -231,46 +217,45 @@ def _lanes(x, idx):
 
 
 def _sample_from_proposal(trace, distribution, addr, n):
-    """IC branch (state.py:203-219): value ~ q(.|LSTM state); weight += log p(value) - log q(value).
+    """IC branch (state.py:203-219): value ~ q(.|network state); weight += log p(value) - log q(value).
 
     The proposal network only runs for the particles that execute this statement (the lanes of the current mask), packed
-    densely, so a loop whose lanes drop out costs what its live lanes cost.  Every lane keeps its own LSTM state and its
-    own previous site (address id + value): lanes that reached this statement from different sites are stepped in
-    separate groups, like the per-trace `_current_trace_previous_variable` of the reference (state.py:212)."""
+    densely, so a loop whose lanes drop out costs what its live lanes cost.  Under the LSTM every lane keeps its own
+    LSTM state and its own previous site (address id + value): lanes that reached this statement from different sites
+    are stepped in separate groups, like the per-trace `_current_trace_previous_variable` of the reference
+    (state.py:212).  A feed-forward network has neither (inference_network_feedforward.py:53-66): its lanes are one
+    group."""
     net = _network
     K = net._proposal_mixture_components
-    if isinstance(net, InferenceNetworkFeedForward):
-        return _propose_and_weigh(trace, distribution, n, *_feedforward_params(net, distribution, addr, n, K))
-    H = net._lstm_dim
-    st = trace.ic_state
-    if st is None:
-        st = trace.ic_state = {'h': torch.zeros(n, H, device='cuda'), 'c': torch.zeros(n, H, device='cuda'),
-                               'prev_id': torch.full((n,), -1, dtype=torch.int64, device='cuda'),
-                               'prev_value': torch.zeros(n, device='cuda'),
-                               'uniform_prev': -1}    # host copy of prev_id when all lanes are known to share it
+    st = None
+    if not isinstance(net, InferenceNetworkFeedForward):
+        H = net._lstm_dim
+        st = trace.ic_state
+        if st is None:
+            st = trace.ic_state = {'h': torch.zeros(n, H, device='cuda'), 'c': torch.zeros(n, H, device='cuda'),
+                                   'prev_id': torch.full((n,), -1, dtype=torch.int64, device='cuda'),
+                                   'prev_value': torch.zeros(n, device='cuda'),
+                                   'uniform_prev': -1}    # host copy of prev_id when all lanes are known to share it
     known = addr in net._addresses
     if not known:
         warnings.warn('Address unknown by inference network: {}'.format(addr))
     idx = None if _mask is None else (_mask_idx if _mask_idx is not None else torch.nonzero(_mask).view(-1))
     if idx is not None and idx.numel() == 0:     # nobody executes the statement: nothing to propose, nothing to weigh
         return distribution.sample(n)
-    p0, p1 = _prior_params(distribution)
+    p0, p1 = distribution._prior_params()
     # group the executing lanes by the site they came from.  Known on the host without a device round trip when every lane
     # shares its previous site, or when this mask is (a narrowing of) the mask of the previous proposal site: then all of its
     # lanes executed that site last.
-    last_mask = st.get('last_mask', _NO_MASK_YET)
-    if idx is None and st['uniform_prev'] is not None:
+    if st is None:
+        groups = [(-1, None)]
+    elif st['uniform_prev'] is not None:
         groups = [(st['uniform_prev'], None)]
-    elif idx is not None and st['uniform_prev'] is not None:
-        groups = [(st['uniform_prev'], None)]
-    elif idx is not None and last_mask is not _NO_MASK_YET and (_mask is last_mask or _mask_parent is last_mask):
+    elif idx is not None and 'last_mask' in st and (_mask is st['last_mask'] or _mask_parent is st['last_mask']):
         groups = [(st['last_id'], None)]
     else:
         ids = st['prev_id'] if idx is None else st['prev_id'][idx]
         uniq = torch.unique(ids).tolist()
         groups = [(u, None if len(uniq) == 1 else (ids == u)) for u in uniq]
-    is_cat = isinstance(distribution, Categorical)
-    width = distribution.num_categories if is_cat else 1 if isinstance(distribution, Bernoulli) else 3 * K
     params = None
     covered = True        # every executing lane got a proposal from the network
     by_id = net._address_by_id()
@@ -279,24 +264,30 @@ def _sample_from_proposal(trace, distribution, addr, n):
             covered = False
             continue
         lanes = idx if sel is None else (torch.nonzero(sel).view(-1) if idx is None else idx[sel])
-        if lanes is None:
-            h, c = st['h'], st['c']
-            pv = st['prev_value']
+        args = (addr, _lanes(p0, lanes), _lanes(p1, lanes), n if lanes is None else lanes.numel())
+        if st is None:
+            out = net._infer_step_lanes(*args)
         else:
-            h, c = st['h'][lanes], st['c'][lanes]
-            pv = st['prev_value'][lanes]
-        out = net._infer_step_lanes(addr, None if pid < 0 else by_id[pid], None if pid < 0 else pv, _lanes(p0, lanes),
-                                    _lanes(p1, lanes), h, c)
+            if lanes is None:
+                h, c = st['h'], st['c']
+                pv = st['prev_value']
+            else:
+                h, c = st['h'][lanes], st['c'][lanes]
+                pv = st['prev_value'][lanes]
+            out = net._infer_step_lanes(*args, None if pid < 0 else by_id[pid], None if pid < 0 else pv, h, c)
+            if lanes is not None:
+                st['h'].index_copy_(0, lanes, h)
+                st['c'].index_copy_(0, lanes, c)
         if lanes is None:
             params = out
         else:
-            st['h'].index_copy_(0, lanes, h)
-            st['c'].index_copy_(0, lanes, c)
             if params is None:
-                params = _default_params(distribution, n, K, width)
+                params = _default_params(distribution, n, K, out.size(1))
             params.index_copy_(0, lanes, out)
     has = None
-    if not covered:   # lanes whose previous / current address the network does not know fall back to the prior
+    # lanes whose previous / current address the network does not know fall back to the prior (feed-forward: one group,
+    # so a site is covered entirely or not at all)
+    if not covered and st is not None:
         has = torch.zeros(n, dtype=torch.bool, device='cuda')
         for pid, sel in groups:
             if known and pid != -2 and (pid < 0 or pid in by_id):
@@ -306,6 +297,8 @@ def _sample_from_proposal(trace, distribution, addr, n):
                 else:
                     has[lanes] = True
     value = _propose_and_weigh(trace, distribution, n, params, has)
+    if st is None:
+        return value
     # this site becomes the previous site of the lanes that executed it
     new_id = net._addresses[addr]['id'] if known else -2
     if idx is None:
@@ -318,26 +311,6 @@ def _sample_from_proposal(trace, distribution, addr, n):
         st['uniform_prev'] = None
     st['last_mask'], st['last_id'] = _mask, new_id
     return value
-
-
-def _feedforward_params(net, distribution, addr, n, K):
-    """Feed-forward network (inference_network_feedforward.py:53-66): no LSTM state and no previous site, so the lanes
-    that execute this statement are proposed for in ONE call.  -> (params [n, width] or None, None)."""
-    idx = None if _mask is None else (_mask_idx if _mask_idx is not None else torch.nonzero(_mask).view(-1))
-    if addr not in net._addresses:
-        warnings.warn('Address unknown by inference network: {}'.format(addr))
-        return None, None
-    if idx is not None and idx.numel() == 0:
-        return None, None
-    p0, p1 = _prior_params(distribution)
-    out = net._infer_step_lanes(addr, _lanes(p0, idx), _lanes(p1, idx), n if idx is None else idx.numel())
-    if idx is None:
-        return out, None
-    is_cat = isinstance(distribution, Categorical)
-    width = distribution.num_categories if is_cat else 1 if isinstance(distribution, Bernoulli) else 3 * K
-    params = _default_params(distribution, n, K, width)
-    params.index_copy_(0, idx, out)
-    return params, None
 
 
 def _propose_and_weigh(trace, distribution, n, params, has):
@@ -451,15 +424,12 @@ def _init_traces(func, trace_mode=TraceMode.PRIOR, prior_inflation=PriorInflatio
 
 
 def _begin_trace(n):
-    global _current_trace, _previous_site, _trace_start, _mask
+    global _current_trace, _trace_start, _mask
     _trace_start = time.time()
     _current_trace = BatchedTrace(n)
     if _mcmc is not None:     # the candidate's log_prob_observed accumulates in the chain tables
         _current_trace.log_w = _mcmc.log_w_view(n)
-    _previous_site = None
     _mask = None
-    if _network is not None:
-        _network._infer_state = None
 
 
 def _end_trace(result):

@@ -1,5 +1,6 @@
-"""The CUDA per-site proposal step (ppb_ic_infer_step through InferenceNetworkLSTM._infer_step_batched) against the
-UNMODIFIED reference's _infer_step on real reference traces (tests/golden/infer_golden.npz)."""
+"""The CUDA per-site proposal step (ppb_ic_infer_step through InferenceNetwork._infer_step_lanes, the call the IC engine
+makes, driven by _infer_step_batched) against the UNMODIFIED reference's _infer_step on real reference traces
+(tests/golden/infer_golden.npz)."""
 import numpy as np
 import pytest
 import torch
