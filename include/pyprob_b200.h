@@ -439,6 +439,10 @@ int64_t ppb_ic_infer_workspace_bytes(const ppb_net* net, int64_t n);
  * ppb_ic_loss_forward and ppb_ic_embed_observe; call it if the arena was modified by other means before
  * ppb_ic_infer_step). */
 int ppb_net_refresh_weights(ppb_net* net, const float* arena, void* stream);
+/* The loss and infer calls keep their problem and chunk lists in the caller's workspace and do not send a list again
+ * while the same content already lives at the same address.  A caller that writes a workspace between two calls of one
+ * net, or hands the net memory that held another workspace, calls this first: the next calls upload every list. */
+int ppb_net_forget_uploads(ppb_net* net);
 
 /* ------------------------------------------------------------------------------------------------
  * 5. Host-buffer convenience entry (the end-to-end call bench.py times as `e2e`)

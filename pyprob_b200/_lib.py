@@ -69,6 +69,7 @@ _SIGNATURES = {
     'ppb_ic_embed_observe': [C.c_void_p, c_f, c_f, c_f, c_i64, c_f, c_i64, c_f],
     'ppb_ic_infer_workspace_bytes': [C.c_void_p, c_i64],
     'ppb_net_refresh_weights': [C.c_void_p, c_f, c_f],
+    'ppb_net_forget_uploads': [C.c_void_p],
     'ppb_ic_train_step_host': [C.c_void_p, c_f, c_f, c_f, c_f, c_i64, C.c_void_p, c_i64, c_f, c_f, c_i64, c_int,
                                c_flt, c_flt, c_flt, c_flt, c_flt, c_i64, C.c_void_p, C.c_void_p, c_f],
     'ppb_packed_floats': [c_i64, c_i64],

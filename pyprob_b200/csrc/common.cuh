@@ -122,8 +122,10 @@ __device__ __forceinline__ float ppb_normal_lp(float v, float mu, float sigma) {
 
 // LSTM cell activations, branch-free (the libm forms carry a slow-path branch each — division, tanhf's range split — which cut
 // the epilogue of the fused LSTM kernels into one basic block per gate and kept the loads of different rows from overlapping;
-// they were also a third of its instructions).  EX2 / RCP approximations: sigmoid within 3e-7 relative; tanh within 4e-7
-// relative (odd Taylor polynomial to x^9 below 0.25, 1 - 2 / (1 + exp(2|x|)) above).  Every cell kernel, fused or not,
+// they were also a third of its instructions).  EX2 / RCP approximations, measured against fp64 on an H100: sigmoid within
+// 1.5e-7 relative for x >= -1; below, x * log2(e) is rounded to fp32 before ex2, so the relative error grows with |x|
+// (1.7e-6 at x = -25, 3.8e-6 at x = -84), and below x = -87.3 the result is flushed to zero.  tanh within 3.7e-7 relative
+// (odd Taylor polynomial to x^9 below 0.25, 1 - 2 / (1 + exp(2|x|)) above, worst just above 0.25).  Every cell kernel, fused or not,
 // forward or backward, goes through these two, so all variants agree to the last bit of the activation.
 __device__ __forceinline__ float ppb_cell_sigmoid(float x) {
   float e, r;

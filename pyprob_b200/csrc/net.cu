@@ -61,6 +61,8 @@ struct ppb_net {
   // which also makes a repeated step capturable in a CUDA graph (no host->device copy inside the capture)
   uint64_t slot_hash[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
   const void* slot_dev[10] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  uint64_t ws_layout = 0;      // workspace address, batch dims and precision of the last loss call (forget_on_new_layout)
+  uint64_t infer_layout = 0;   // workspace address, particle count and entry of the last inference call
   void* h_blob[2] = {nullptr, nullptr};
   cudaEvent_t ev_blob[2] = {nullptr, nullptr};
   size_t blob_cap = 0;
@@ -1594,6 +1596,18 @@ int64_t ppb_ic_workspace_bytes(const ppb_net* net, int32_t n_traces, int32_t n_r
   return simt_region_bytes(net, d) + carve_tc(net, d, nullptr).total_bytes + 1024;
 }
 
+// The workspace regions move with the batch dims (carve, carve_tc; carve_infer with n), so a call with another layout may
+// write its buffers over a list an earlier call uploaded (a no-grad forward of a larger batch over the last step's backward
+// lists, _infer_init's embedding over the infer step's list): when the workspace address or the layout key changes, the
+// lists of slots [first, last] are sent again.  Slot 7 (the fused LSTM step list) lives in memory the net owns.
+static void forget_on_new_layout(ppb_net* net, uint64_t& last_key, const void* key, size_t key_bytes, const void* workspace,
+                                 int first, int last) {
+  const uint64_t h = fnv1a(&workspace, sizeof(workspace), fnv1a(key, key_bytes));
+  if (h == last_key) return;
+  for (int i = first; i <= last; ++i) net->slot_hash[i] = 0;
+  last_key = h;
+}
+
 int ppb_ic_loss_forward(ppb_net* net, const float* arena, const ppb_batch* b, void* workspace,
                         int64_t workspace_bytes, int precision, float* loss_out, int32_t* status_out,
                         float* row_lp_out, int want_grad, void* stream) {
@@ -1604,6 +1618,10 @@ int ppb_ic_loss_forward(ppb_net* net, const float* arena, const ppb_batch* b, vo
   PPB_CHECK_ARG(precision >= 0 && precision <= 2, "unknown precision mode");
   Dims d = dims_of(b);
   PPB_CHECK_ARG(workspace_bytes >= ppb_ic_workspace_bytes(net, d.B, d.R, d.T, d.NS, d.G), "workspace too small");
+  {
+    const int key[6] = {d.B, d.R, d.T, d.NS, d.G, precision};
+    forget_on_new_layout(net, net->ws_layout, key, sizeof(key), workspace, 0, 4);
+  }
   cudaStream_t st = (cudaStream_t)stream;
   if (net->desc.network_type == PPB_NET_FEEDFORWARD)
     return ff_loss_forward(net, arena, b, workspace, precision, loss_out, status_out, row_lp_out, want_grad, st);
@@ -1619,6 +1637,10 @@ int ppb_ic_loss_backward(ppb_net* net, const float* arena, float* grad, const pp
   PPB_CHECK_ARG(arena && grad && workspace, "null arena/grad/workspace");
   Dims d = dims_of(b);
   PPB_CHECK_ARG(workspace_bytes >= ppb_ic_workspace_bytes(net, d.B, d.R, d.T, d.NS, d.G), "workspace too small");
+  {
+    const int key[6] = {d.B, d.R, d.T, d.NS, d.G, precision};
+    forget_on_new_layout(net, net->ws_layout, key, sizeof(key), workspace, 0, 4);
+  }
   cudaStream_t st = (cudaStream_t)stream;
   if (net->desc.network_type == PPB_NET_FEEDFORWARD)
     return ff_loss_backward(net, arena, grad, b, workspace, precision, grad_scale, st);
@@ -1972,6 +1994,12 @@ int ppb_adam_step_dev(float* arena, const float* grad, float* exp_avg, float* ex
   return PPB_OK;
 }
 
+int ppb_net_forget_uploads(ppb_net* net) {
+  PPB_CHECK_ARG(net, "bad arguments");
+  for (int i = 0; i < (int)(sizeof(net->slot_hash) / sizeof(net->slot_hash[0])); ++i) net->slot_hash[i] = 0;
+  return PPB_OK;
+}
+
 int ppb_net_refresh_weights(ppb_net* net, const float* arena, void* stream) {
   PPB_CHECK_ARG(net && arena && net->wimg, "bad arguments (tables not set?)");
   k_pack_table<<<dim3(net->pack_tiles, 8), 256, 0, (cudaStream_t)stream>>>(arena, net->d_pack, (int)net->pack.size(), net->wimg);
@@ -1988,6 +2016,10 @@ int ppb_ic_embed_observe(ppb_net* net, const float* arena, const float* obs, flo
                          void* workspace, int64_t workspace_bytes, void* stream) {
   PPB_CHECK_ARG(net && arena && obs && obs_emb_out && workspace && n > 0, "bad arguments");
   PPB_CHECK_ARG(workspace_bytes >= ppb_ic_infer_workspace_bytes(net, n), "workspace too small");
+  {
+    const int64_t key[2] = {n, 0};
+    forget_on_new_layout(net, net->infer_layout, key, sizeof(key), workspace, 5, 6);
+  }
   cudaStream_t st = (cudaStream_t)stream;
   InferWs w = carve_infer(net, n, workspace);
   if (net->wimg) {  // inference starts here (_infer_init): bring the tensor-core weight images up to date
@@ -2010,6 +2042,10 @@ int ppb_ic_infer_step(ppb_net* net, const float* arena, const float* obs_emb, in
   PPB_CHECK_ARG(net && arena && obs_emb && (ff || (h && c)) && params_out && workspace && n > 0, "bad arguments");
   PPB_CHECK_ARG(cur_addr >= 0 && cur_addr < (int)net->addrs.size(), "unknown current address");
   PPB_CHECK_ARG(workspace_bytes >= ppb_ic_infer_workspace_bytes(net, n), "workspace too small");
+  {
+    const int64_t key[2] = {n, 1};
+    forget_on_new_layout(net, net->infer_layout, key, sizeof(key), workspace, 5, 6);
+  }
   if (ff) {
     if (obs_emb_row_stride != 0) {
       ppb_set_error("ppb_ic_infer_step: per-particle observation embeddings are not supported yet (stride must be 0)");

@@ -406,6 +406,8 @@ class InferenceNetwork(nn.Module):
                          enc.n_groups) + 512
         if self._workspace is None or self._workspace.numel() < need:
             self._workspace = torch.empty(int(need * 1.25), dtype=torch.uint8, device='cuda')
+            # the allocator may hand back the old address with other content: the cached lists must be sent again
+            call('ppb_net_forget_uploads', self._handle)
         if self._loss_buf is None:
             self._loss_buf = torch.zeros(4, dtype=torch.float32, device='cuda')
         return need
@@ -840,6 +842,7 @@ class InferenceNetwork(nn.Module):
         ws = getattr(self, '_infer_ws', None)
         if ws is None or ws.numel() < need:
             self._infer_ws = torch.empty(int(need), dtype=torch.uint8, device='cuda')
+            call('ppb_net_forget_uploads', self._handle)
         return need
 
     def _infer_init(self, observe=None):

@@ -75,13 +75,14 @@ def window(family, p0, p1):
 
 
 def proposal(family, x, K, p0, p1):
-    """x [n] (one row, any dtype) -> (means, stddevs, probs) of a mixture head, (probs,) of a Categorical or Bernoulli
-    head: the tensors the reference's proposal layer hands to its distribution."""
+    """x [n] (one row, any dtype) or [rows, n] -> (means, stddevs, probs) of a mixture head, (probs,) of a Categorical or
+    Bernoulli head: the tensors the reference's proposal layer hands to its distribution.  With rows, p0 and p1 are
+    [rows, 1] (or scalars)."""
     if family == 'Categorical':
-        return (torch.softmax(x, dim=0) + 1e-8,)
+        return (torch.softmax(x, dim=-1) + 1e-8,)
     if family == 'Bernoulli':
         return (torch.sigmoid(x) + 1e-8,)
-    means, stddevs, coeffs = x[:K], x[K:2 * K], torch.softmax(x[2 * K:3 * K], dim=0)
+    means, stddevs, coeffs = x[..., :K], x[..., K:2 * K], torch.softmax(x[..., 2 * K:3 * K], dim=-1)
     if family == 'Normal':
         return p0 + means * p1, torch.exp(stddevs) * p1, coeffs
     if family == 'Uniform':
