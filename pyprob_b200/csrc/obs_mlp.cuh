@@ -165,6 +165,11 @@ __device__ __forceinline__ void layer_fwd(const Plan& P, const Layer& L, const f
 // grid = ceil(B / traces_per_cta); every CTA walks its traces in chunks of kMT
 __global__ void __launch_bounds__(kThreads) k_fwd(const __grid_constant__ Plan P, const float* __restrict__ arena, int B,
                                                   int traces_per_cta) {
+  // Launched with PDL: its CTAs are placed while the predecessor drains, ahead of the side-stream kernels that start beside
+  // it.  It waits before its first read AND before it lets its own dependents launch, so every later kernel of the step
+  // starts after whatever ran before this one (the optimiser that wrote the weights) has finished: kernels further down the
+  // chain may read the weights before their own wait (k_bwd does).
+  ppb_pdl_wait();
   ppb_pdl_trigger();   // the P_obs GEMM that follows is launched with the PDL attribute: its prologue overlaps this kernel
   extern __shared__ __align__(16) float smem[];
   const int n_layers = P.n_layers, A = P.A;
@@ -247,16 +252,19 @@ __global__ void __launch_bounds__(kThreads) k_bwd(const __grid_constant__ Plan P
   float* act = smem + P.w_floats;
   float* dz = act + kMT * A;
   float* part = dz + kMT * Dz;
-  // Staged before the wait: the weights and the forward activations are not written by any kernel of the backward pass.
-  // The first layer of a chain never propagates further down: it is not staged.
+  // Staged before the wait: the weights (arena).  Only the optimiser writes them, and no kernel of a training step can
+  // start before the previous step's optimiser has finished: k_fwd waits before it lets its dependents launch.  The
+  // first layer of a chain never propagates further down: it is not staged.
   for (int i = 0; i < n_layers; ++i)
     if (P.L[i].dxoff >= 0) stage_layer(smem, arena, P.L[i]);
   for (int i = threadIdx.x; i < part_floats; i += kThreads) part[i] = 0.f;
+  // Everything else after it: the forward activations and the embedding are written by k_fwd of this same step, which a
+  // chain of programmatic edges does not order before this point (each kernel of the chain triggers before its own wait)
+  ppb_pdl_wait();
   const int t_begin = blockIdx.x * traces_per_cta;
   const int t_end = min(B, t_begin + traces_per_cta);
   const int zoff = P.L[n_layers - 1].dzoff, eoff = P.L[n_layers - 1].yoff;
   const float* emb = P.L[n_layers - 1].y;
-  bool waited = false;
   for (int c0 = t_begin; c0 < t_end; c0 += kMT) {
     const int nt = min(kMT, t_end - c0);
     for (int i = 0; i < n_layers; ++i) {   // every layer's input, and the embedding
@@ -264,7 +272,6 @@ __global__ void __launch_bounds__(kThreads) k_bwd(const __grid_constant__ Plan P
       load_rows(act + L.xoff, A, L.x, L.ldx, c0, nt, L.in_dim);
     }
     load_rows(act + eoff, A, emb, E, c0, nt, E);
-    if (!waited) { ppb_pdl_wait(); waited = true; }
     load_rows(dz + zoff, Dz, d_emb, E, c0, nt, E);
     cp_async_wait_all();
     __syncthreads();
@@ -282,7 +289,7 @@ __global__ void __launch_bounds__(kThreads) k_bwd(const __grid_constant__ Plan P
     for (int i = 0; i < n_layers; ++i) layer_partial(P, P.L[i], act, dz, part, nt);
     __syncthreads();
   }
-  if (!waited) { ppb_pdl_wait(); cp_async_wait_all(); }   // no copy may stay in flight past the exit
+  cp_async_wait_all();   // a CTA without traces still has its staging copies in flight: none may stay past the exit
   // cluster reduction: rank r sums entries r*256 + tid (stride kCluster*256) over the cluster and adds them to the arena
   tcc::cluster_sync_all();
   const uint32_t rank = tcc::cluster_ctarank();
