@@ -353,18 +353,36 @@ int ppb_ic_loss_backward(ppb_net* net, const float* arena, float* grad_arena,
                          const ppb_batch* batch_host_struct, void* workspace, int64_t workspace_bytes,
                          int precision, float grad_scale, void* stream);
 
-/* Fused flat-arena Adam (torch.optim.Adam semantics: pyprob/nn/inference_network.py:348, :496).
- * step is the 1-based step count after increment; grad_scale multiplies the gradient first
- * (1/world for data-parallel averaging, inference_network.py:324-325). */
-int ppb_adam_step(float* arena, const float* grad, float* exp_avg, float* exp_avg_sq, int64_t n,
-                  float lr, float beta1, float beta2, float eps, float weight_decay, int64_t step,
-                  float grad_scale, void* stream);
+/* Slots of the device hyper-parameter vector (float) read by the optimiser steps.  The Adam steps
+ * (ppb_adam_step_dev, ppb_dp_adam_step) read the first PPB_HYPER_ADAM_COUNT; the segmented step
+ * (ppb_optimizer_step_segmented) reads all PPB_HYPER_COUNT. */
+enum {
+  PPB_HYPER_LR = 0,
+  PPB_HYPER_BETA1,
+  PPB_HYPER_BETA2,
+  PPB_HYPER_EPS,
+  PPB_HYPER_WEIGHT_DECAY,
+  PPB_HYPER_GRAD_SCALE,      /* multiplies the gradient first (1/world for data-parallel averaging, :324-325) */
+  PPB_HYPER_ADAM_COUNT,
+  PPB_HYPER_MOMENTUM = PPB_HYPER_ADAM_COUNT,
+  PPB_HYPER_LARC_TRUST,      /* LARC trust coefficient (0.002) */
+  PPB_HYPER_LARC_EPS,        /* LARC eps (1e-8) */
+  PPB_HYPER_LARC_EPSILON,    /* LARC epsilon (1/16000) */
+  PPB_HYPER_COUNT
+};
 
-/* Same update with the step counter and hyper-parameters in device memory, so that a whole training step
- * (forward, backward, optimiser) can be captured once in a CUDA graph and replayed.
- *   hyper_dev: float[6] = lr, beta1, beta2, eps, weight_decay, grad_scale
- *   state_dev: 16 bytes, zero-initialised: int64 step counter (incremented by the call), float bc1 of the last step,
- *              uint32 scratch (finished-block count, zero between calls) */
+/* Adam state block (16 bytes of device memory, zero-initialised), shared by ppb_adam_step_dev and
+ * ppb_dp_adam_step:
+ *   byte 0   int64   step counter: the number of steps taken; each call advances it by one
+ *   byte 8   float   1 - beta1^t of the last step (written, read by nothing in this library)
+ *   byte 12  uint32  finished-block count of ppb_adam_step_dev: zero between calls
+ * A caller that resumes from a checkpoint writes its step count at byte 0. */
+
+/* Fused flat-arena Adam (torch.optim.Adam semantics: pyprob/nn/inference_network.py:348, :496) with the step
+ * counter and hyper-parameters in device memory, so that a whole training step (forward, backward, optimiser) can be
+ * captured once in a CUDA graph and replayed.  Any alignment of the four arrays is accepted.
+ *   hyper_dev: float[PPB_HYPER_ADAM_COUNT]
+ *   state_dev: the Adam state block */
 int ppb_adam_step_dev(float* arena, const float* grad, float* exp_avg, float* exp_avg_sq, int64_t n,
                       const float* hyper_dev, void* state_dev, void* stream);
 
@@ -378,8 +396,7 @@ int ppb_adam_step_dev(float* arena, const float* grad, float* exp_avg, float* ex
  *   present         int32[n_segs] device: 1 if the segment received a gradient this step
  *   seg_steps       int64[n_segs] device: per-segment step counts (incremented for present segments)
  *   state0/state1   Adam: exp_avg / exp_avg_sq;  SGD: momentum buffer / unused (may be NULL)
- *   hyper_dev       float[10] device: lr, beta1, beta2, eps, weight_decay, grad_scale, momentum,
- *                   larc trust coefficient (0.002), larc eps (1e-8), larc epsilon (1/16000)
+ *   hyper_dev       float[PPB_HYPER_COUNT] device
  *   scratch         ppb_optimizer_scratch_bytes(n_segs) bytes of device memory
  * Graph-capturable (all step-dependent state lives in device memory). */
 int64_t ppb_optimizer_scratch_bytes(int32_t n_segs);
@@ -402,7 +419,8 @@ int ppb_optimizer_step_segmented(float* arena, const float* grad, float* state0,
  * exp_avg_sq are local, only the slice is touched) -> the updated parameters are stored into every peer's
  * arena (all-gather by peer stores) -> cross-rank barrier.  The n_extra scalars are summed by rank 0 and
  * written back to every rank's gradient tail.  Replicas stay bit-identical: every element is reduced by
- * exactly one rank.  hyper_dev/state_dev as for ppb_adam_step_dev (grad_scale = 1/world). The call is
+ * exactly one rank.  hyper_dev/state_dev as for ppb_adam_step_dev (grad_scale = 1/world); the step leaves
+ * byte 12 of the state block untouched.  The call is
  * CUDA-graph capturable; all ranks must issue it the same number of times. */
 int ppb_dp_alloc(int64_t bytes, void** ptr_out, void* ipc_handle_out /* 64 bytes */);
 int ppb_dp_open(const void* ipc_handle /* 64 bytes, from another process */, void** ptr_out);
@@ -452,7 +470,8 @@ int ppb_net_forget_uploads(ppb_net* net);
  *    The call returns when the step has finished (loss_host / status_host are valid).  After the first call
  *    with a given batch STRUCTURE the whole step — including both copies, staged through an internal pinned
  *    buffer, so batch_image_host need not be pinned — replays from one CUDA graph (PPB_HOST_STEP_GRAPH=0:
- *    plain stream launches).
+ *    the same launches, issued without capture).  Adam runs as ppb_adam_step_dev on a state block the net owns;
+ *    `step` is the 1-based count after this step, and the block's counter is rewritten when it disagrees.
  * ---------------------------------------------------------------------------------------------- */
 int ppb_ic_train_step_host(ppb_net* net, float* arena, float* grad_arena, float* exp_avg,
                            float* exp_avg_sq, int64_t arena_floats, const void* batch_image_host,

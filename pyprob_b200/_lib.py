@@ -54,7 +54,6 @@ _SIGNATURES = {
     'ppb_sizeof': [c_int],
     'ppb_ic_loss_forward': [C.c_void_p, c_f, C.c_void_p, c_f, c_i64, c_int, c_f, c_f, c_f, c_int, c_f],
     'ppb_ic_loss_backward': [C.c_void_p, c_f, c_f, C.c_void_p, c_f, c_i64, c_int, c_flt, c_f],
-    'ppb_adam_step': [c_f, c_f, c_f, c_f, c_i64, c_flt, c_flt, c_flt, c_flt, c_flt, c_i64, c_flt, c_f],
     'ppb_adam_step_dev': [c_f, c_f, c_f, c_f, c_i64, c_f, c_f, c_f],
     'ppb_optimizer_scratch_bytes': [c_i32],
     'ppb_optimizer_step_segmented': [c_f, c_f, c_f, c_f, c_i64, c_f, c_i32, c_f, c_f, c_f, c_i64, c_int, c_f, c_f],

@@ -93,8 +93,16 @@ static inline int ppb_grid_for(int64_t n, int threads, int items_per_thread, int
   return (int)blocks;
 }
 
-// One Adam update (torch.optim.Adam without amsgrad) with every rounding spelled out, so that the plain, the
-// device-state and the data-parallel fused optimiser kernels produce the same bits:
+// Bias corrections of Adam step t (1-based) from the betas of a device hyper vector (PPB_HYPER_* slots), computed in
+// double and rounded once to fp32: bc1 = 1 - b1^t (the update's step is lr / bc1) and bc2_sqrt = sqrt(1 - b2^t).
+// beta2 is read after the first pow(), so that it does not hold a register across it.
+__device__ __forceinline__ void ppb_adam_bias_corrections(const float* hyper, long long t, float& bc1, float& bc2_sqrt) {
+  bc1 = (float)(1.0 - pow((double)hyper[PPB_HYPER_BETA1], (double)t));
+  bc2_sqrt = (float)sqrt(1.0 - pow((double)hyper[PPB_HYPER_BETA2], (double)t));
+}
+
+// One Adam update (torch.optim.Adam without amsgrad) with every rounding spelled out, so that the flat, the
+// segmented and the data-parallel fused optimiser kernels produce the same bits:
 //   g' = g*gscale + wd*p;  m = b1 m + (1-b1) g';  v = b2 v + (1-b2) g'^2;  p -= step * m / (sqrt(v)/bc2_sqrt + eps)
 __device__ __forceinline__ void ppb_adam_update(float& p, float g, float& m, float& v, float b1, float b2, float eps,
                                                 float wd, float gscale, float step, float bc2_sqrt) {

@@ -85,9 +85,7 @@ __global__ void __launch_bounds__(256) k_dp_adam(Peers P, int world, int rank, f
   __shared__ int s_last;
   if (threadIdx.x == 0) {
     s_epoch = my[kFlagEpoch] + 1u;  // written only by the last block of the previous launch
-    long long t = *step_ctr + 1;
-    s_bc[0] = (float)(1.0 - pow((double)hyper[1], (double)t));
-    s_bc[1] = (float)sqrt(1.0 - pow((double)hyper[2], (double)t));
+    ppb_adam_bias_corrections(hyper, *step_ctr + 1, s_bc[0], s_bc[1]);
   }
   __syncthreads();
   const uint32_t epoch = s_epoch;
@@ -100,7 +98,8 @@ __global__ void __launch_bounds__(256) k_dp_adam(Peers P, int world, int rank, f
   __syncthreads();
   if (blockIdx.x == 0 && threadIdx.x == 0) my[kFlagTrace + 1] = (uint32_t)now_ns();
 
-  const float lr = hyper[0], b1 = hyper[1], b2 = hyper[2], eps = hyper[3], wd = hyper[4], gscale = hyper[5];
+  const float lr = hyper[PPB_HYPER_LR], b1 = hyper[PPB_HYPER_BETA1], b2 = hyper[PPB_HYPER_BETA2];
+  const float eps = hyper[PPB_HYPER_EPS], wd = hyper[PPB_HYPER_WEIGHT_DECAY], gscale = hyper[PPB_HYPER_GRAD_SCALE];
   const float step = lr / s_bc[0], bc2_sqrt = s_bc[1];
 
   // ---- this rank's slice: [lo, hi), boundaries on float4
@@ -168,7 +167,7 @@ __global__ void __launch_bounds__(256) k_dp_adam(Peers P, int world, int rank, f
       my[kFlagDone] = 0u;
       my[kFlagEpoch] = epoch;
       *step_ctr = *step_ctr + 1;
-      bc_out[0] = s_bc[0];   // (byte 12 of the state block is scratch of ppb_adam_step_dev: left untouched)
+      bc_out[0] = s_bc[0];   // byte 8 of the Adam state block (include/pyprob_b200.h); byte 12 is left untouched
     }
   }
 }

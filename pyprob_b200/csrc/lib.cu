@@ -32,7 +32,7 @@ extern "C" {
 
 const char* ppb_last_error(void) { return g_err; }
 
-int ppb_version(void) { return 101; }
+int ppb_version(void) { return 102; }
 
 int64_t ppb_launch_count(void) { return (int64_t)g_ppb_launches; }
 

@@ -94,9 +94,9 @@ struct ppb_net {
   cudaGraphExec_t host_exec = nullptr;
   uint64_t host_key = 0;
   int host_seen = 0;
-  float* host_hyper_dev = nullptr;  // [6] lr, b1, b2, eps, wd, grad_scale
-  void* host_state_dev = nullptr;   // 16 B Adam state (ppb_adam_step_dev)
-  float host_hyper[6] = {0, 0, 0, 0, 0, 0};
+  float* host_hyper_dev = nullptr;  // [PPB_HYPER_ADAM_COUNT] (include/pyprob_b200.h)
+  void* host_state_dev = nullptr;   // Adam state block (include/pyprob_b200.h)
+  float host_hyper[PPB_HYPER_ADAM_COUNT] = {0, 0, 0, 0, 0, 0};
   int64_t host_step_dev = -1;       // value of the device step counter
   char* host_pin = nullptr;         // pinned staging: [image bytes | 8 B loss + status]; both copies are nodes of the step graph
   int64_t host_pin_cap = 0;
@@ -1655,38 +1655,9 @@ int ppb_ic_loss_backward(ppb_net* net, const float* arena, float* grad, const pp
 // =====================================================================================================
 namespace {
 
-__global__ void __launch_bounds__(256) k_adam(float* __restrict__ p, const float* __restrict__ g,
-                                               float* __restrict__ m, float* __restrict__ v, int64_t n, float lr,
-                                               float b1, float b2, float eps, float wd, float bc1, float bc2_sqrt,
-                                               float gscale) {
-  ppb_pdl_trigger();
-  ppb_pdl_wait();
-  // torch.optim.Adam (no amsgrad): g += wd*p; m = b1 m + (1-b1) g; v = b2 v + (1-b2) g^2;
-  // p -= (lr / bc1) * m / (sqrt(v)/sqrt(bc2) + eps)
-  int64_t n4 = n >> 2;
-  float step = lr / bc1;
-  for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < n4; q += (int64_t)gridDim.x * blockDim.x) {
-    float4 pp = reinterpret_cast<float4*>(p)[q], gg = reinterpret_cast<const float4*>(g)[q];
-    float4 mm = reinterpret_cast<float4*>(m)[q], vv = reinterpret_cast<float4*>(v)[q];
-    float pa[4] = {pp.x, pp.y, pp.z, pp.w}, ga[4] = {gg.x, gg.y, gg.z, gg.w};
-    float ma[4] = {mm.x, mm.y, mm.z, mm.w}, va[4] = {vv.x, vv.y, vv.z, vv.w};
-#pragma unroll
-    for (int j = 0; j < 4; ++j) ppb_adam_update(pa[j], ga[j], ma[j], va[j], b1, b2, eps, wd, gscale, step, bc2_sqrt);
-    reinterpret_cast<float4*>(p)[q] = make_float4(pa[0], pa[1], pa[2], pa[3]);
-    reinterpret_cast<float4*>(m)[q] = make_float4(ma[0], ma[1], ma[2], ma[3]);
-    reinterpret_cast<float4*>(v)[q] = make_float4(va[0], va[1], va[2], va[3]);
-  }
-  for (int64_t i = (n4 << 2) + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n;
-       i += (int64_t)gridDim.x * blockDim.x) {
-    float pi = p[i], mi = m[i], vi = v[i];
-    ppb_adam_update(pi, g[i], mi, vi, b1, b2, eps, wd, gscale, step, bc2_sqrt);
-    m[i] = mi; v[i] = vi; p[i] = pi;
-  }
-}
-
 // Graph-replayable Adam: step counter and hyper-parameters live in device memory.  Every block derives the bias
-// corrections of step t+1 itself; the last block to finish advances the counter (state: int64 step | float bc1 |
-// uint32 finished-block count, zero between launches).
+// corrections of step t+1 itself; the last block to finish advances the counter (the Adam state block of
+// include/pyprob_b200.h).
 __global__ void __launch_bounds__(256) k_adam_dev(float* __restrict__ p, const float* __restrict__ g,
                                                    float* __restrict__ m, float* __restrict__ v, int64_t n, int vec,
                                                    const float* __restrict__ hyper, long long* __restrict__ step_ctr,
@@ -1710,11 +1681,11 @@ __global__ void __launch_bounds__(256) k_adam_dev(float* __restrict__ p, const f
   if (threadIdx.x == 0) {
     long long t = *step_ctr + 1;
     s_t = t;
-    s_bc[0] = (float)(1.0 - pow((double)hyper[1], (double)t));
-    s_bc[1] = (float)sqrt(1.0 - pow((double)hyper[2], (double)t));
+    ppb_adam_bias_corrections(hyper, t, s_bc[0], s_bc[1]);
   }
   __syncthreads();
-  const float lr = hyper[0], b1 = hyper[1], b2 = hyper[2], eps = hyper[3], wd = hyper[4], gscale = hyper[5];
+  const float lr = hyper[PPB_HYPER_LR], b1 = hyper[PPB_HYPER_BETA1], b2 = hyper[PPB_HYPER_BETA2];
+  const float eps = hyper[PPB_HYPER_EPS], wd = hyper[PPB_HYPER_WEIGHT_DECAY], gscale = hyper[PPB_HYPER_GRAD_SCALE];
   const float step = lr / s_bc[0], bc2_sqrt = s_bc[1];
   while (q < n4) {
     // a tensor that has never seen a gradient (g = m = v = 0) and no weight decay: the update is exactly zero — skip
@@ -1969,20 +1940,9 @@ int ppb_batch_from_image(const void* image_host, const void* image_dev, int64_t 
   return PPB_OK;
 }
 
-int ppb_adam_step(float* arena, const float* grad, float* exp_avg, float* exp_avg_sq, int64_t n, float lr, float beta1,
-                  float beta2, float eps, float weight_decay, int64_t step, float grad_scale, void* stream) {
-  PPB_CHECK_ARG(arena && grad && exp_avg && exp_avg_sq && n > 0 && step >= 1, "bad arguments");
-  double bc1 = 1.0 - pow((double)beta1, (double)step), bc2 = 1.0 - pow((double)beta2, (double)step);
-  PPB_CUDA(ppb_launch(k_adam, dim3(ppb_grid_for(n, 256, 4)), dim3(256), 0, (cudaStream_t)stream, 0, 0, arena, grad, exp_avg,
-                      exp_avg_sq, n, lr, beta1, beta2, eps, weight_decay, (float)bc1, (float)sqrt(bc2), grad_scale));
-  PPB_LAUNCH_CHECK();
-  return PPB_OK;
-}
-
 // Graph-replayable Adam: the step counter and the hyper-parameters live in device memory, so a captured
-// training step stays valid while the count advances and the learning rate follows its schedule.
-//   state_dev: 16 bytes: int64 step counter at [0], float bc1 of the last step at byte 8, uint32 scratch at byte 12 (zero)
-//   hyper_dev: float[6] = lr, beta1, beta2, eps, weight_decay, grad_scale
+// training step stays valid while the count advances and the learning rate follows its schedule.  The float4 path
+// needs all four arrays 16-byte aligned; otherwise every element takes the scalar loop.
 int ppb_adam_step_dev(float* arena, const float* grad, float* exp_avg, float* exp_avg_sq, int64_t n,
                       const float* hyper_dev, void* state_dev, void* stream) {
   PPB_CHECK_ARG(arena && grad && exp_avg && exp_avg_sq && hyper_dev && state_dev && n > 0, "bad arguments");
@@ -2189,28 +2149,13 @@ int ppb_ic_train_step_host(ppb_net* net, float* arena, float* grad_arena, float*
   float* loss_dev = (float*)((char*)workspace + need);  // loss scalar + status live after the carved region
   int32_t* status_dev = (int32_t*)(loss_dev + 1);
 
-  if (!net->host_graph || g_prof.on) {
-    PPB_CUDA(cudaMemcpyAsync(batch_image_dev, batch_image_host, batch_image_bytes, cudaMemcpyHostToDevice, st));
-    PPB_CUDA(cudaMemsetAsync(grad_arena, 0, arena_floats * sizeof(float), st));
-    rc = ppb_ic_loss_forward(net, arena, &b, workspace, need, precision, loss_dev, status_dev, nullptr, 1, stream);
-    if (rc) return rc;
-    rc = ppb_ic_loss_backward(net, arena, grad_arena, &b, workspace, need, precision, 1.0f, stream);
-    if (rc) return rc;
-    rc = ppb_adam_step(arena, grad_arena, exp_avg, exp_avg_sq, arena_floats, lr, beta1, beta2, eps, weight_decay, step, 1.0f,
-                       stream);
-    if (rc) return rc;
-    if (loss_host) PPB_CUDA(cudaMemcpyAsync(loss_host, loss_dev, sizeof(float), cudaMemcpyDeviceToHost, st));
-    if (status_host) PPB_CUDA(cudaMemcpyAsync(status_host, status_dev, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-    PPB_CUDA(cudaStreamSynchronize(st));
-    return PPB_OK;
-  }
-
-  // ---- graph-cached variant: the launches of a step depend only on the batch STRUCTURE (host index arrays) and on the
-  // buffers; the first call with a structure runs eagerly (and uploads the problem lists), the second captures the step
-  // into a graph on an internal stream, later calls replay it.  Adam's step count and hyper-parameters live in device memory.
+  // The launches of a step depend only on the batch STRUCTURE (host index arrays) and on the buffers: the first call with a
+  // structure runs eagerly (and uploads the problem lists), the second captures the step into a graph on an internal
+  // stream, later calls replay it.  With PPB_HOST_STEP_GRAPH=0 or kernel profiling on, every call runs eagerly on that
+  // stream.  Adam's step count and hyper-parameters live in device memory.
   if (!net->host_stream) {
     PPB_CUDA(cudaStreamCreateWithFlags(&net->host_stream, cudaStreamNonBlocking));
-    PPB_CUDA(cudaMalloc((void**)&net->host_hyper_dev, 6 * sizeof(float)));
+    PPB_CUDA(cudaMalloc((void**)&net->host_hyper_dev, sizeof(net->host_hyper)));
     PPB_CUDA(cudaMalloc(&net->host_state_dev, 16));
     PPB_CUDA(cudaMemset(net->host_state_dev, 0, 16));
     net->host_step_dev = 0;
@@ -2251,7 +2196,7 @@ int ppb_ic_train_step_host(ppb_net* net, float* arena, float* grad_arena, float*
   rc = stream_after(net, st, hs);
   if (rc) return rc;
   memcpy(pin_img, batch_image_host, (size_t)batch_image_bytes);
-  const float hyper[6] = {lr, beta1, beta2, eps, weight_decay, 1.0f};
+  const float hyper[PPB_HYPER_ADAM_COUNT] = {lr, beta1, beta2, eps, weight_decay, 1.0f};
   if (memcmp(hyper, net->host_hyper, sizeof(hyper)) != 0) {
     memcpy(net->host_hyper, hyper, sizeof(hyper));
     PPB_CUDA(cudaMemcpyAsync(net->host_hyper_dev, net->host_hyper, sizeof(hyper), cudaMemcpyHostToDevice, hs));
@@ -2274,9 +2219,10 @@ int ppb_ic_train_step_host(ppb_net* net, float* arena, float* grad_arena, float*
     PPB_CUDA(cudaMemcpyAsync(pin_res, loss_dev, 8, cudaMemcpyDeviceToHost, q));   // loss (float) + status (int32), adjacent
     return PPB_OK;
   };
-  if (net->host_exec) {
+  const bool use_graph = net->host_graph && !g_prof.on;
+  if (use_graph && net->host_exec) {
     PPB_CUDA(cudaGraphLaunch(net->host_exec, hs));
-  } else if (net->host_seen >= 1) {
+  } else if (use_graph && net->host_seen >= 1) {
     cudaGraph_t graph = nullptr;
     PPB_CUDA(cudaStreamBeginCapture(hs, cudaStreamCaptureModeThreadLocal));
     rc = enqueue(hs);

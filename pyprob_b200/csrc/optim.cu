@@ -8,15 +8,11 @@
 // tensor; here the whole arena is three launches: per-segment norms (LARC only), a per-segment table (step counts,
 // bias corrections, LARC ratios), and one element-wise update.  HBM-bound: 16 B read + 12 B written per parameter
 // (+8 B read for the norms pass under LARC).
-//
-// STATUS: written after the round-1 GPU budget was spent; not yet validated on hardware (tests are opt-in).
 #include "common.cuh"
 
 namespace {
 
 enum { kAdam = 0, kAdamLarc = 1, kSgd = 2, kSgdLarc = 3 };
-// hyper_dev layout
-enum { hLr = 0, hB1, hB2, hEps, hWd, hGscale, hMomentum, hTrust, hLarcEps, hLarcEpsilon, hCount };
 // per-segment table written by k_seg_table
 struct SegEntry {
   float step_size;  // Adam: lr / (1 - b1^t); SGD: lr
@@ -51,7 +47,7 @@ __global__ void __launch_bounds__(256) k_seg_norms(const float* __restrict__ p, 
                                                     const int32_t* __restrict__ seg_of_block,
                                                     const int32_t* __restrict__ present, const float* __restrict__ hyper,
                                                     float* __restrict__ norms /* [2*S] zeroed */) {
-  const float gscale = hyper[hGscale];
+  const float gscale = hyper[PPB_HYPER_GRAD_SCALE];
   const unsigned lane = threadIdx.x & 31;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   const int64_t rounds = (n_blocks + stride - 1) / stride;
@@ -96,14 +92,15 @@ __global__ void k_seg_table(int n_segs, const int32_t* __restrict__ present, lon
                             SegEntry* __restrict__ table) {
   int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n_segs || !present[k]) return;
-  const float lr = hyper[hLr], wd = hyper[hWd];
+  const float lr = hyper[PPB_HYPER_LR], wd = hyper[PPB_HYPER_WEIGHT_DECAY];
   long long t = steps[k] + 1;
   steps[k] = t;
   SegEntry e;
   e.first = (t == 1);
   if (kind == kAdam || kind == kAdamLarc) {
-    e.step_size = lr / (float)(1.0 - pow((double)hyper[hB1], (double)t));
-    e.bc2_sqrt = (float)sqrt(1.0 - pow((double)hyper[hB2], (double)t));
+    float bc1;
+    ppb_adam_bias_corrections(hyper, t, bc1, e.bc2_sqrt);
+    e.step_size = lr / bc1;
   } else {
     e.step_size = lr;
     e.bc2_sqrt = 1.0f;
@@ -112,7 +109,9 @@ __global__ void k_seg_table(int n_segs, const int32_t* __restrict__ present, lon
   if (kind == kAdamLarc || kind == kSgdLarc) {
     // optimizer_larc.py:87-99, clip mode: min(local_lr / lr, 1)
     float pn = sqrtf(norms[2 * k]), gn = sqrtf(norms[2 * k + 1]);
-    float local = (pn != 0.0f && gn != 0.0f) ? hyper[hTrust] * pn / (gn + pn * wd + hyper[hLarcEps]) : hyper[hLarcEpsilon];
+    float local = (pn != 0.0f && gn != 0.0f)
+                      ? hyper[PPB_HYPER_LARC_TRUST] * pn / (gn + pn * wd + hyper[PPB_HYPER_LARC_EPS])
+                      : hyper[PPB_HYPER_LARC_EPSILON];
     e.adaptive = fminf(local / lr, 1.0f);
   }
   table[k] = e;
@@ -124,8 +123,9 @@ __global__ void __launch_bounds__(256) k_seg_update(float* __restrict__ p, const
                                                      const int32_t* __restrict__ present,
                                                      const SegEntry* __restrict__ table,
                                                      const float* __restrict__ hyper, int kind) {
-  const float b1 = hyper[hB1], b2 = hyper[hB2], eps = hyper[hEps], wd = hyper[hWd], gscale = hyper[hGscale];
-  const float momentum = hyper[hMomentum];
+  const float b1 = hyper[PPB_HYPER_BETA1], b2 = hyper[PPB_HYPER_BETA2], eps = hyper[PPB_HYPER_EPS];
+  const float wd = hyper[PPB_HYPER_WEIGHT_DECAY], gscale = hyper[PPB_HYPER_GRAD_SCALE];
+  const float momentum = hyper[PPB_HYPER_MOMENTUM];
   const bool larc = kind == kAdamLarc || kind == kSgdLarc;
   const bool adam = kind == kAdam || kind == kAdamLarc;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_blocks; i += (int64_t)gridDim.x * blockDim.x) {

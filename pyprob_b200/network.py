@@ -9,7 +9,8 @@ pyprob/nn/inference_network_lstm.py:13-27, pyprob/nn/inference_network_feedforwa
   state_dict key names (``parameter_index``), so reference checkpoints load verbatim;
 * ``_loss`` encodes the minibatch into index tensors and calls the C-ABI forward/backward
   (include/pyprob_b200.h section 4) through one ``torch.autograd.Function``;
-* the optimiser is the fused flat-arena Adam kernel (``ppb_adam_step``);
+* the optimiser is the fused flat-arena Adam kernel (``ppb_adam_step_dev``), its step counter and hyper-parameters
+  in device memory;
 * there is no CPU execution path: every method raises without a CUDA device + the native library.
 """
 import ctypes as C
@@ -30,6 +31,7 @@ from .util import InferenceNetwork as InferenceNetworkType  # noqa: F401
 from .util import LearningRateScheduler, ObserveEmbedding, Optimizer
 
 _OPTIMIZER_KIND = {Optimizer.ADAM: 0, Optimizer.ADAM_LARC: 1, Optimizer.SGD: 2, Optimizer.SGD_LARC: 3}
+_HYPER_COUNT = 10   # PPB_HYPER_COUNT: slots of the optimiser's device hyper vector (include/pyprob_b200.h)
 
 FAMILY_NORMAL, FAMILY_UNIFORM, FAMILY_POISSON, FAMILY_CATEGORICAL, FAMILY_BERNOULLI = 0, 1, 2, 3, 4
 _FAMILY_OF = {'Normal': FAMILY_NORMAL, 'Uniform': FAMILY_UNIFORM, 'Poisson': FAMILY_POISSON,
@@ -132,6 +134,10 @@ class InferenceNetwork(nn.Module):
         self._exp_avg_sq = None
         self._peer = None                 # parallel.PeerAdam when training data-parallel over NVLink
         self._seg = None                  # device tables of the segment-aware optimiser step (LARC / SGD / skipping)
+        self._hyper = None                # device hyper vector of every optimiser step (_optimizer_hyper)
+        self._hyper_host = None           # the values it holds
+        self._adam_state = None           # Adam state block of the flat and peer steps (_adam_state_block)
+        self._adam_state_step = None      # the step counter it holds
         self._skip_absent_gradients = False   # True: tensors absent from a minibatch are skipped like .grad None
         # Optimizer.ADAM hands over to the skipping step by itself when the flat kernel would differ from torch.optim
         # (_maybe_switch_to_segmented); PPB_FLAT_ADAM=1 keeps the flat kernel (absent gradient = zeros) throughout
@@ -371,7 +377,8 @@ class InferenceNetwork(nn.Module):
     def __getstate__(self):
         st = self.__dict__.copy()
         for k in ('_handle', '_workspace', '_image_dev', '_image_host', '_loss_buf', '_model',
-                  '_infer_observe_embedding', '_peer', '_peer_hyper', '_peer_state', '_seg', '_last_enc'):
+                  '_infer_observe_embedding', '_peer', '_seg', '_last_enc', '_hyper', '_hyper_host', '_adam_state',
+                  '_adam_state_step'):
             st[k] = None
         if self._peer is not None:   # the arena lives in an NVLink peer block: pickle a private copy
             st['_arena_store'] = self._arena_store.clone()
@@ -499,30 +506,51 @@ class InferenceNetwork(nn.Module):
                      'seg_of_block': torch.from_numpy(seg_of_block).cuda(),
                      'steps': torch.zeros(S, dtype=torch.int64, device='cuda'),
                      'present': torch.ones(S, dtype=torch.int32, device='cuda'),
-                     'scratch': torch.empty(int(scratch), dtype=torch.uint8, device='cuda'),
-                     'hyper': torch.zeros(10, dtype=torch.float32, device='cuda')}
+                     'scratch': torch.empty(int(scratch), dtype=torch.uint8, device='cuda')}
 
     def _segment_names(self):
         return sorted(self.parameter_index, key=lambda k: self.parameter_index[k][0])
 
     def _segmented_optimizer_step(self, grad_scale):
         seg = self._seg
-        b1, b2 = self._adam_betas
         seg['present'].copy_(torch.from_numpy(self._segment_presence(self._last_enc)))
         world, _ = parallel.world_info()
         if world > 1 and self._skip_absent_gradients:
             # a tensor is present if any rank saw it (the reference's presence map, inference_network.py:299-311)
             import torch.distributed as dist
             dist.all_reduce(seg['present'], op=dist.ReduceOp.MAX)
-        seg['hyper'].copy_(torch.tensor([float(self._learning_rate), b1, b2, self._adam_eps,
-                                         float(self._weight_decay or 0.0), float(grad_scale),
-                                         float(self._momentum if self._momentum is not None else 0.9),
-                                         0.002, 1e-8, 1.0 / 16000.0]))
+        hyper = self._optimizer_hyper(grad_scale, (float(self._momentum if self._momentum is not None else 0.9),
+                                                   0.002, 1e-8, 1.0 / 16000.0))
         adam = self._optimizer_type in (Optimizer.ADAM, Optimizer.ADAM_LARC)
         call('ppb_optimizer_step_segmented', ptr(self._arena.data), ptr(self._arena.grad), ptr(self._exp_avg),
              ptr(self._exp_avg_sq) if adam else None, self._arena.numel(), ptr(seg['seg_of_block']), len(seg['names']),
              ptr(seg['present']), ptr(seg['steps']), ptr(seg['scratch']), seg['scratch'].numel(),
-             _OPTIMIZER_KIND[self._optimizer_type], ptr(seg['hyper']), stream())
+             _OPTIMIZER_KIND[self._optimizer_type], ptr(hyper), stream())
+
+    def _optimizer_hyper(self, grad_scale, extra=()):
+        """The device hyper vector of the next optimiser step (PPB_HYPER_* slots): lr, betas, eps, weight decay and
+        grad_scale, then `extra` (the segmented step's momentum and LARC slots).  Uploaded only when the values change."""
+        b1, b2 = self._adam_betas
+        values = (float(self._learning_rate), float(b1), float(b2), float(self._adam_eps),
+                  float(self._weight_decay or 0.0), float(grad_scale)) + tuple(extra)
+        if self._hyper is None:
+            self._hyper = torch.zeros(_HYPER_COUNT, dtype=torch.float32, device=self._arena.device)
+        if values != self._hyper_host:
+            self._hyper[:len(values)].copy_(torch.tensor(values, dtype=torch.float32))
+            self._hyper_host = values
+        return self._hyper
+
+    def _adam_state_block(self):
+        """The Adam state block (include/pyprob_b200.h) for the flat or peer step about to run.  _optimizer_step stays the
+        source of truth (tests assign it, checkpoints load it): the block's counter is rewritten when the host mirror of
+        it differs, and the mirror then counts the step about to run."""
+        if self._adam_state is None:
+            self._adam_state = torch.zeros(2, dtype=torch.int64, device=self._arena.device)
+            self._adam_state_step = 0
+        if self._adam_state_step != self._optimizer_step:
+            self._adam_state[0] = int(self._optimizer_step)
+        self._adam_state_step = self._optimizer_step + 1
+        return self._adam_state
 
     @property
     def _optimizer(self):
@@ -564,14 +592,13 @@ class InferenceNetwork(nn.Module):
 
     def optimizer_step(self, grad_scale=1.0):
         self._maybe_switch_to_segmented()
-        self._optimizer_step += 1
         if self._seg is not None:
             self._segmented_optimizer_step(grad_scale)
-            return
-        b1, b2 = self._adam_betas
-        call('ppb_adam_step', ptr(self._arena.data), ptr(self._arena.grad), ptr(self._exp_avg), ptr(self._exp_avg_sq),
-             self._arena.numel(), float(self._learning_rate), b1, b2, self._adam_eps, float(self._weight_decay or 0.0),
-             self._optimizer_step, float(grad_scale), stream())
+        else:
+            call('ppb_adam_step_dev', ptr(self._arena.data), ptr(self._arena.grad), ptr(self._exp_avg),
+                 ptr(self._exp_avg_sq), self._arena.numel(), ptr(self._optimizer_hyper(grad_scale)),
+                 ptr(self._adam_state_block()), stream())
+        self._optimizer_step += 1
 
     def _enable_peer_optimizer(self):
         """Move the arena into this rank's NVLink peer block and switch the optimiser step to the fused
@@ -582,18 +609,13 @@ class InferenceNetwork(nn.Module):
         self._arena_store = peer.params
         self._arena = nn.Parameter(peer.params)
         self._peer = peer
-        self._peer_hyper = torch.zeros(6, dtype=torch.float32, device=peer.params.device)
-        self._peer_state = torch.zeros(4, dtype=torch.int32, device=peer.params.device)
-        self._peer_state.view(torch.int64)[0] = int(self._optimizer_step)
 
     def _peer_optimizer_step(self, loss, world):
         peer, n = self._peer, self._arena.numel()
         peer.grad[:n].copy_(self._arena.grad)
         peer.grad[n:n + 1].copy_(loss.reshape(1))
-        b1, b2 = self._adam_betas
-        self._peer_hyper.copy_(torch.tensor([float(self._learning_rate), b1, b2, self._adam_eps,
-                                             float(self._weight_decay or 0.0), 1.0 / world]))
-        peer.step(self._exp_avg, self._exp_avg_sq, self._peer_hyper, self._peer_state, stream())
+        hyper, state = self._optimizer_hyper(1.0 / world), self._adam_state_block()
+        peer.step(self._exp_avg, self._exp_avg_sq, hyper, state, stream())
         self._optimizer_step += 1
         loss_value = float(peer.grad[n]) / world
         if peer.timed_out():
@@ -823,7 +845,8 @@ class InferenceNetwork(nn.Module):
         ret._handle = None
         ret._tables_dirty = True
         for k, default in (('_peer', None), ('_seg', None), ('_skip_absent_gradients', False), ('_last_enc', None),
-                           ('_auto_skip_absent', True), ('_present_sig', None)):
+                           ('_auto_skip_absent', True), ('_present_sig', None), ('_hyper', None), ('_hyper_host', None),
+                           ('_adam_state', None), ('_adam_state_step', None)):
             ret.__dict__.setdefault(k, default)   # checkpoints written before these attributes existed
         if data['optimizer_state'] is not None:
             ret._create_optimizer(data['optimizer_state'])

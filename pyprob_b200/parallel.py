@@ -25,7 +25,7 @@ def allreduce_grad_and_loss(grad_flat, loss):
     """Sum the flat gradient arena over ranks in place (loss scalar piggy-backed).
 
     Returns (mean loss as float, grad_scale) — grad_scale = 1/world is folded into the optimiser kernel
-    (ppb_adam_step's grad_scale) instead of a separate divide pass."""
+    (the grad_scale slot of the optimiser's hyper vector) instead of a separate divide pass."""
     world, _ = world_info()
     if world == 1:
         return float(loss), 1.0
@@ -75,7 +75,7 @@ class _RawDeviceMemory:
 class PeerAdam:
     """Data-parallel Adam fused with its collective over NVLink peer memory (``ppb_dp_adam_step``).
 
-    Replaces ``allreduce_grad_and_loss`` + ``ppb_adam_step`` when all ranks sit on one NVLink node: the gradient
+    Replaces ``allreduce_grad_and_loss`` + ``ppb_adam_step_dev`` when all ranks sit on one NVLink node: the gradient
     is reduce-scattered by peer loads, Adam runs on the owning rank's slice only, and the updated parameters
     are all-gathered by peer stores — one kernel, two NVLink crossings per element, no NCCL on the step.
 
@@ -122,8 +122,8 @@ class PeerAdam:
             dist.barrier()   # every block is mapped (and zeroed) before anyone's first step
 
     def step(self, exp_avg, exp_avg_sq, hyper_dev, state_dev, stream):
-        """hyper_dev: float[6] = lr, beta1, beta2, eps, weight_decay, grad_scale (1/world);
-        state_dev: 16 bytes, int64 step counter + two bias corrections (see ppb_adam_step_dev)."""
+        """hyper_dev: the Adam slots of the hyper vector, grad_scale = 1/world; state_dev: the Adam state block
+        (both in include/pyprob_b200.h)."""
         from . import _lib
         _lib.call('ppb_dp_adam_step', self.world, self.rank, self._blocks, self.param_off, self.grad_off,
                   self.flag_off, _lib.ptr(exp_avg), _lib.ptr(exp_avg_sq), self.n, self.N_EXTRA, _lib.ptr(hyper_dev),

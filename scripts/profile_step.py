@@ -26,14 +26,14 @@ bs = BatchStruct(); call('ppb_batch_from_image', img.data_ptr(), dimg.data_ptr()
 need = net._ensure_workspace(enc)
 st = torch.cuda.current_stream().cuda_stream
 loss = torch.empty((), device=dev); status = torch.zeros(1, dtype=torch.int32, device=dev)
-n = [0]
+hyper = torch.tensor([1e-3, 0.9, 0.999, 1e-8, 0.0, 1.0], dtype=torch.float32, device=dev)
+adam_state = torch.zeros(2, dtype=torch.int64, device=dev)
 def step():
     st = torch.cuda.current_stream().cuda_stream
     grad.zero_()
     call('ppb_ic_loss_forward', net._handle, ptr(net._arena.data), C.byref(bs), ptr(net._workspace), need, prec, ptr(loss), ptr(status), None, 1, st)
     call('ppb_ic_loss_backward', net._handle, ptr(net._arena.data), ptr(grad), C.byref(bs), ptr(net._workspace), need, prec, 1.0, st)
-    n[0] += 1
-    call('ppb_adam_step', ptr(net._arena.data), ptr(grad), ptr(net._exp_avg), ptr(net._exp_avg_sq), net._arena.numel(), 1e-3, 0.9, 0.999, 1e-8, 0.0, n[0], 1.0, st)
+    call('ppb_adam_step_dev', ptr(net._arena.data), ptr(grad), ptr(net._exp_avg), ptr(net._exp_avg_sq), net._arena.numel(), ptr(hyper), ptr(adam_state), st)
 for _ in range(5): step()
 torch.cuda.synchronize()
 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)

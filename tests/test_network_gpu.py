@@ -1,4 +1,4 @@
-"""GPU parity of the proposal-network training path (C-ABI ppb_ic_loss_forward/backward, ppb_adam_step):
+"""GPU parity of the proposal-network training path (C-ABI ppb_ic_loss_forward/backward, ppb_adam_step_dev):
   (1) against the UNMODIFIED reference's loss and gradients on identical traces/weights (golden fixture),
   (2) against the oracle on seeded random networks/batches with ragged sub-batches and all four families,
   (3) size-independent properties at larger sizes (loss additivity over sub-batches, gradient linearity).
@@ -130,8 +130,8 @@ def test_adam_step_vs_torch(cuda):
         torch.testing.assert_close(net.view(name), ref[name].data, rtol=1e-5, atol=1e-6, msg=lambda m, name=name: name + ': ' + m)
 
 
-def test_flat_adam_kernel_vs_torch_on_the_whole_arena(cuda):
-    """The flat kernel itself (ppb_adam_step): every element updated, as torch.optim.Adam on one tensor."""
+def test_flat_adam_step_dev_vs_torch_on_the_whole_arena(cuda):
+    """The flat kernel itself (ppb_adam_step_dev): every element updated, as torch.optim.Adam on one tensor."""
     from pyprob_b200._lib import call, ptr, stream
     gen = torch.Generator().manual_seed(0)
     n = 100003
@@ -139,11 +139,14 @@ def test_flat_adam_kernel_vs_torch_on_the_whole_arena(cuda):
     ref_p = p.clone().requires_grad_(True)
     opt = torch.optim.Adam([ref_p], lr=1e-3, weight_decay=1e-2)
     m, v = torch.zeros(n, device=cuda), torch.zeros(n, device=cuda)
+    hyper = torch.tensor([1e-3, 0.9, 0.999, 1e-8, 1e-2, 1.0], device=cuda)
+    state = torch.zeros(2, dtype=torch.int64, device=cuda)
     for step in range(1, 4):
         g = torch.randn(n, generator=gen).to(cuda)
         ref_p.grad = g.clone()
         opt.step()
-        call('ppb_adam_step', ptr(p), ptr(g), ptr(m), ptr(v), n, 1e-3, 0.9, 0.999, 1e-8, 1e-2, step, 1.0, stream())
+        call('ppb_adam_step_dev', ptr(p), ptr(g), ptr(m), ptr(v), n, ptr(hyper), ptr(state), stream())
+    assert int(state[0]) == 3
     torch.testing.assert_close(p, ref_p.data, rtol=1e-5, atol=1e-6)
 
 
