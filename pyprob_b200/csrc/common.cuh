@@ -84,6 +84,14 @@ inline cudaError_t ppb_launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   return cudaLaunchKernelEx(&cfg, kernel, args...);
 }
 
+namespace gemm {
+// One launch of a grouped GEMM (SIMT: gemm_simt.cuh, tensor cores: tc_launch.cuh) over problems [first, first + count) of a
+// host-built list.  Problems are appended per phase; tile_start is local to the phase.
+struct Phase {
+  int first = 0, count = 0, tiles = 0;
+};
+}  // namespace gemm
+
 static inline int ppb_grid_for(int64_t n, int threads, int items_per_thread, int max_waves = 8) {
   int64_t blocks = (n + (int64_t)threads * items_per_thread - 1) / ((int64_t)threads * items_per_thread);
   if (blocks < 1) blocks = 1;

@@ -145,9 +145,4 @@ __global__ void __launch_bounds__(kThreads) k_grouped(const Problem* __restrict_
   }
 }
 
-// Host-side list builder.  Problems are appended per phase; tile_start is local to the phase.
-struct Phase {
-  int first = 0, count = 0, tiles = 0;
-};
-
 }  // namespace gemm

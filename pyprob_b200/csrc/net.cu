@@ -20,6 +20,7 @@
 #include "tc_lstm.cuh"
 #include "tc_cluster.cuh"
 #include "tc_persist.cuh"
+#include "tc_launch.cuh"
 #include "obs_mlp.cuh"
 
 using gemm::Problem;
@@ -309,40 +310,25 @@ struct Prof {
   int64_t launches = 0;
 } g_prof;
 
-// One profiled launch: prof_begin records the start event when profiling is on and the caller asks for it (`want`), else
-// leaves e0 null; prof_end records the end event after a non-null e0 and counts one launch of `flops` FLOPs.
-int prof_begin(bool want, cudaStream_t st, cudaEvent_t& e0) {
-  e0 = nullptr;
-  if (!want || !g_prof.on) return PPB_OK;
-  PPB_CUDA(cudaEventCreate(&e0));
-  PPB_CUDA(cudaEventRecord(e0, st));
-  return PPB_OK;
-}
-int prof_end(cudaEvent_t e0, cudaStream_t st, double flops) {
-  if (!e0) return PPB_OK;
-  cudaEvent_t e1;
-  PPB_CUDA(cudaEventCreate(&e1));
-  PPB_CUDA(cudaEventRecord(e1, st));
-  g_prof.spans.push_back({e0, e1});
-  g_prof.launches += 1;
-  g_prof.flops += flops;
-  return PPB_OK;
-}
-template <typename P>
-double phase_flops(const std::vector<P>& probs, const gemm::Phase& ph) {
+// The profiling argument of a phase runner for phase `i` of a problem list (Builder, TcBuilder): the phase's FLOPs, or 0 (not
+// profiled) while profiling is off
+template <typename B>
+double profile(const B& bl, int i) {
+  if (!g_prof.on) return 0.0;
+  const gemm::Phase& ph = bl.phases[i];
   double f = 0.0;
-  for (int i = 0; i < ph.count; ++i) { const P& p = probs[ph.first + i]; f += 2.0 * p.M * p.N * p.K; }
+  for (int j = 0; j < ph.count; ++j) { const auto& p = bl.probs[ph.first + j]; f += 2.0 * p.M * p.N * p.K; }
   return f;
 }
 
-int run_phase(const gemm::Phase& ph, const Problem* dev, cudaStream_t st, const Builder* bl_for_prof = nullptr) {
+int run_phase(const gemm::Phase& ph, const Problem* dev, cudaStream_t st, double prof_flops = 0.0) {
   if (ph.count == 0) return PPB_OK;
   int grid = ph.tiles < 8 * PPB_NUM_SMS ? ph.tiles : 8 * PPB_NUM_SMS;
-  cudaEvent_t e0;
-  int rc = prof_begin(bl_for_prof != nullptr, st, e0); if (rc) return rc;
-  gemm::k_grouped<<<grid, gemm::kThreads, 0, st>>>(dev + ph.first, ph.count, ph.tiles);
-  PPB_LAUNCH_CHECK();
-  return e0 ? prof_end(e0, st, phase_flops(bl_for_prof->probs, ph)) : PPB_OK;
+  return profiled(prof_flops, st, [&] {
+    gemm::k_grouped<<<grid, gemm::kThreads, 0, st>>>(dev + ph.first, ph.count, ph.tiles);
+    PPB_LAUNCH_CHECK();
+    return PPB_OK;
+  });
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -1425,10 +1411,10 @@ int simt_loss_forward(ppb_net* net, const float* arena, const ppb_batch* b, void
   PPB_CUDA(cudaMemsetAsync(w.loss_acc, 0, 256, st));
   for (int l = 0; l < ph_p; ++l) { rc = run_phase(bl.phases[l], w.problems, st); if (rc) return rc; }
   rc = launch_step_inputs_fwd(net, arena, b, w, st); if (rc) return rc;
-  rc = run_phase(bl.phases[ph_p], w.problems, st, &bl); if (rc) return rc;
+  rc = run_phase(bl.phases[ph_p], w.problems, st, profile(bl, ph_p)); if (rc) return rc;
   for (int t = 0; t < d.T; ++t) {
     int r0 = b->row_off_host[t], n = b->row_off_host[t + 1] - r0;
-    if (t > 0) { rc = run_phase(bl.phases[ph_rec0 + t - 1], w.problems, st, &bl); if (rc) return rc; }
+    if (t > 0) { rc = run_phase(bl.phases[ph_rec0 + t - 1], w.problems, st, profile(bl, ph_rec0 + t - 1)); if (rc) return rc; }
     k_cell_fwd<<<ew_grid((int64_t)n * H), 256, 0, st>>>(w.gates, w.p_obs, w.p_step, w.w_smp_t, w.smp_emb, b->row_step,
                                                        b->row_prev, b->row_trace, w.c, w.h, HImg(), r0, n, H, S, t);
     PPB_LAUNCH_CHECK();
@@ -1490,13 +1476,14 @@ int simt_loss_backward(ppb_net* net, const float* arena, float* grad, const ppb_
   for (int t = d.T - 1; t >= 0; --t) {
     int r0 = b->row_off_host[t], n = b->row_off_host[t + 1] - r0;
     int n_next = (t + 1 < d.T) ? b->row_off_host[t + 2] - b->row_off_host[t + 1] : 0;
-    if (n_next > 0) { rc = run_phase(bl.phases[ph_rec0 + (d.T - 2 - t)], dprobs, st, &bl); if (rc) return rc; }
+    const int ph = ph_rec0 + (d.T - 2 - t);
+    if (n_next > 0) { rc = run_phase(bl.phases[ph], dprobs, st, profile(bl, ph)); if (rc) return rc; }
     k_cell_bwd<false><<<ew_grid((int64_t)n * H), 256, 0, st>>>(w.gates, w.c, w.dh, w.dh_rec, w.dc, dgates, w.d_pobs, b->row_prev,
                                                        b->row_next, b->row_trace, HImg(), r0, n, H, t, HImg());
     PPB_LAUNCH_CHECK();
   }
   rc = launch_step_inputs_bwd(net, arena, grad, b, w, dgates, st); if (rc) return rc;
-  rc = run_phase(bl.phases[ph_lstm_w], dprobs, st, &bl); if (rc) return rc;
+  rc = run_phase(bl.phases[ph_lstm_w], dprobs, st, profile(bl, ph_lstm_w)); if (rc) return rc;
   return obs_fp32_bwd(bl, ph_obs, dprobs, D, grad, d.B, w, st);
 }
 
@@ -1857,6 +1844,24 @@ InferWs carve_infer(const ppb_net* net, int64_t n, void* base) {
 
 }  // namespace
 
+int prof_begin(double flops, cudaStream_t st, cudaEvent_t& e0) {
+  e0 = nullptr;
+  if (flops <= 0.0 || !g_prof.on) return PPB_OK;
+  PPB_CUDA(cudaEventCreate(&e0));
+  PPB_CUDA(cudaEventRecord(e0, st));
+  return PPB_OK;
+}
+int prof_end(cudaEvent_t e0, cudaStream_t st, double flops) {
+  if (!e0) return PPB_OK;
+  cudaEvent_t e1;
+  PPB_CUDA(cudaEventCreate(&e1));
+  PPB_CUDA(cudaEventRecord(e1, st));
+  g_prof.spans.push_back({e0, e1});
+  g_prof.launches += 1;
+  g_prof.flops += flops;
+  return PPB_OK;
+}
+
 extern "C" {
 
 int ppb_prof_enable(int on) {
@@ -2110,7 +2115,7 @@ int ppb_ic_infer_step(ppb_net* net, const float* arena, const float* obs_emb, in
     if (use_tc) {
       k_pack_rows<<<pack_grid, 256, 0, st>>>(h, (int)n, H, H, w.h_img);
       PPB_LAUNCH_CHECK();
-      rc = run_tc_phase(tb.phases[0], w.tprobs, precision, st, 0); if (rc) return rc;
+      rc = run_tc_phase<0>(tb.phases[0], w.tprobs, precision, st); if (rc) return rc;
     } else {
       rc = run_phase(bl.phases[2], w.problems, st); if (rc) return rc;
     }
@@ -2120,8 +2125,8 @@ int ppb_ic_infer_step(ppb_net* net, const float* arena, const float* obs_emb, in
   if (use_tc) {
     k_pack_rows<<<pack_grid, 256, 0, st>>>(h, (int)n, H, H, w.h_img);
     PPB_LAUNCH_CHECK();
-    rc = run_tc_phase(tb.phases[1], w.tprobs, precision, st, 2); if (rc) return rc;
-    rc = run_tc_phase(tb.phases[2], w.tprobs, precision, st, 0); if (rc) return rc;
+    rc = run_tc_phase<2>(tb.phases[1], w.tprobs, precision, st); if (rc) return rc;
+    rc = run_tc_phase<0>(tb.phases[2], w.tprobs, precision, st); if (rc) return rc;
   } else {
     rc = run_phase(bl.phases[3], w.problems, st); if (rc) return rc;
     rc = run_phase(bl.phases[4], w.problems, st); if (rc) return rc;

@@ -458,10 +458,4 @@ __global__ void __launch_bounds__(tcg::kThreads, 1) k_lstm_cluster(const tcl::St
   }
 }
 
-// host-side launch with a (CS, 1, 1) cluster (and the PDL attribute, common.cuh)
-template <typename Kernel, typename... Args>
-inline cudaError_t launch_cluster(Kernel kernel, int grid, int cluster, size_t smem, cudaStream_t st, Args... args) {
-  return ppb_launch(kernel, dim3((unsigned)grid, 1, 1), dim3(tcg::kThreads, 1, 1), smem, st, 1, cluster, args...);
-}
-
 }  // namespace tcc

@@ -5,9 +5,7 @@
 
 #include "common.cuh"
 #include "tc.cuh"
-#include "tc_grouped.cuh"
-#include "tc_cluster.cuh"
-#include "tc_persist.cuh"
+#include "tc_launch.cuh"
 
 namespace {
 
@@ -43,49 +41,22 @@ int g_trace_launch = 0;
 
 namespace {
 
-// one-problem launch of the production kernel (tc_grouped.cuh) — the standalone GEMM entry points below are thin
-// wrappers so that tests and micro-benchmarks exercise exactly the kernel the network uses
+// one-problem launch of the production kernels — the standalone GEMM entry points below are thin wrappers around the
+// network's phase runners (tc_launch.cuh), so that tests and micro-benchmarks exercise exactly the kernels and the launch code
+// the network uses
 tcg::Problem* g_dev_problem = nullptr;
 
-template <bool X3>
-int launch_single(const tcg::Problem& hp, cudaStream_t st) {
-  static bool attr = false;
-  if (!attr) {
-    PPB_CUDA(cudaFuncSetAttribute(tcg::k_grouped<X3, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tcg::smem_bytes()));
-    attr = true;
-  }
+// cs = 1: grouped or persistent form, launched without PDL (the benchmarks time these launches as such); else the cluster
+// split-K form over cs CTAs
+int run_single(tcg::Problem& hp, int precision, int cs, cudaStream_t st) {
+  hp.tiles_m = (hp.M + 127) / 128; hp.tiles_n = (hp.N + 127) / 128; hp.k_splits = 1;
   if (!g_dev_problem) PPB_CUDA(cudaMalloc((void**)&g_dev_problem, sizeof(tcg::Problem)));
   PPB_CUDA(cudaMemcpyAsync(g_dev_problem, &hp, sizeof(hp), cudaMemcpyHostToDevice, st));
-  const int tiles = hp.tiles_m * hp.tiles_n * (hp.k_splits > 1 ? hp.k_splits : 1);
-  if (ppb_persistent_enabled() && tiles > PPB_NUM_SMS) {   // persistent form (tc_persist.cuh)
-    static bool attr_p = false;
-    if (!attr_p) {
-      PPB_CUDA(cudaFuncSetAttribute(tcp::k_grouped_persistent<X3, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)tcp::smem_bytes()));
-      attr_p = true;
-    }
-    tcp::k_grouped_persistent<X3, 0><<<PPB_NUM_SMS, tcg::kThreads, tcp::smem_bytes(), st>>>(g_dev_problem, 1, tiles);
-    PPB_LAUNCH_CHECK();
-    return PPB_OK;
-  }
-  tcg::k_grouped<X3, 0><<<hp.tiles_m * hp.tiles_n, tcg::kThreads, tcg::smem_bytes(), st>>>(g_dev_problem, 1, nullptr);
-  PPB_LAUNCH_CHECK();
-  return PPB_OK;
-}
-
-template <bool X3, int CS>
-int launch_single_cluster(const tcg::Problem& hp, cudaStream_t st) {
-  static bool attr = false;
-  if (!attr) {
-    PPB_CUDA(cudaFuncSetAttribute(tcc::k_cluster<X3, CS, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tcc::smem_bytes()));
-    attr = true;
-  }
-  if (!g_dev_problem) PPB_CUDA(cudaMalloc((void**)&g_dev_problem, sizeof(tcg::Problem)));
-  PPB_CUDA(cudaMemcpyAsync(g_dev_problem, &hp, sizeof(hp), cudaMemcpyHostToDevice, st));
-  PPB_CUDA(tcc::launch_cluster(tcc::k_cluster<X3, CS, 0>, hp.tiles_m * hp.tiles_n * CS, CS, tcc::smem_bytes(), st,
-                               (const tcg::Problem*)g_dev_problem, 1, (unsigned long long*)nullptr, tcc::NoRowEpi{}));
-  PPB_LAUNCH_CHECK();
-  return PPB_OK;
+  gemm::Phase ph;
+  ph.count = 1;
+  ph.tiles = hp.tiles_m * hp.tiles_n;
+  if (cs == 1) return run_tc_phase<0>(ph, g_dev_problem, precision, st, 0.0, false);
+  return run_tc_phase_cluster<0>(cs, ph, g_dev_problem, precision, st);
 }
 
 }  // namespace
@@ -128,8 +99,7 @@ int ppb_gemm_packed(const float* A_hi, const float* A_lo, const float* B_hi, con
   p.b.hi = B_hi; p.b.lo = B_lo; p.b.kb = kb;
   p.M = (int)M; p.N = (int)N; p.K = (int)K;
   p.c = C; p.ldc = ldc; p.bias = bias; p.flags = relu ? tcg::kRelu : 0;
-  p.tiles_m = (int)((M + 127) / 128); p.tiles_n = (int)((N + 127) / 128); p.k_splits = 1;
-  return precision == PPB_PREC_TF32X3 ? launch_single<true>(p, (cudaStream_t)stream) : launch_single<false>(p, (cudaStream_t)stream);
+  return run_single(p, precision, 1, (cudaStream_t)stream);
 }
 
 // Same GEMM with the reduction split over a thread-block cluster of `cluster_size` CTAs per output tile (2, 4 or 8):
@@ -149,12 +119,7 @@ int ppb_gemm_packed_cluster(const float* A_hi, const float* A_lo, const float* B
   p.b.hi = B_hi; p.b.lo = B_lo; p.b.kb = kb;
   p.M = (int)M; p.N = (int)N; p.K = (int)K;
   p.c = C; p.ldc = ldc; p.bias = bias; p.flags = relu ? tcg::kRelu : 0;
-  p.tiles_m = (int)((M + 127) / 128); p.tiles_n = (int)((N + 127) / 128); p.k_splits = 1;
-  cudaStream_t st = (cudaStream_t)stream;
-  const bool x3 = precision == PPB_PREC_TF32X3;
-  if (cluster_size == 2) return x3 ? launch_single_cluster<true, 2>(p, st) : launch_single_cluster<false, 2>(p, st);
-  if (cluster_size == 4) return x3 ? launch_single_cluster<true, 4>(p, st) : launch_single_cluster<false, 4>(p, st);
-  return x3 ? launch_single_cluster<true, 8>(p, st) : launch_single_cluster<false, 8>(p, st);
+  return run_single(p, precision, cluster_size, (cudaStream_t)stream);
 }
 
 int ppb_gemm_packed_tn(const float* X_hi, const float* X_lo, const float* Y_hi, const float* Y_lo, float* C, int64_t M,
@@ -168,8 +133,7 @@ int ppb_gemm_packed_tn(const float* X_hi, const float* X_lo, const float* Y_hi, 
   p.b.hi = Y_hi; p.b.lo = Y_lo; p.b.kb = (int)((N + 31) / 32); p.b.mn = 1;
   p.M = (int)M; p.N = (int)N; p.K = (int)((R + 31) / 32 * 32);  // image rows beyond R are zero padding
   p.c = C; p.ldc = ldc;
-  p.tiles_m = (int)((M + 127) / 128); p.tiles_n = (int)((N + 127) / 128); p.k_splits = 1;
-  return precision == PPB_PREC_TF32X3 ? launch_single<true>(p, (cudaStream_t)stream) : launch_single<false>(p, (cudaStream_t)stream);
+  return run_single(p, precision, 1, (cudaStream_t)stream);
 }
 
 }  // extern "C"
