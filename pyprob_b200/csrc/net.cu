@@ -1829,7 +1829,7 @@ InferWs carve_infer(const ppb_net* net, int64_t n, void* base) {
   w.problems = (Problem*)take(w.max_problems * (int64_t)(sizeof(Problem) / 4));
   auto img_k = [&](int64_t rows, int64_t cols) {
     HImg im;
-    int64_t nfl = img_floats(rows, cols);
+    int64_t nfl = tc::img_floats(rows, cols);
     off = align_up(off, 1024);
     im.kb = (cols + 31) / 32;
     im.k_hi = take(nfl); im.k_lo = take(nfl);

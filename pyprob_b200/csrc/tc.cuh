@@ -6,31 +6,52 @@
 
 namespace tc {
 
-// ---- packed operand image: K-major, SWIZZLE_128B ------------------------------------------------
+// ---- packed operand image (tile image): K-major, SWIZZLE_128B ------------------------------------
 // A matrix X[rows, K] is stored as tiles of 128 rows x 32 fp32 (one 128-byte swizzle span along K):
-//   tile(rt, kb) at float offset (rt * KB + kb) * 4096, KB = ceil(K/32)
-//   inside a tile: 16 atoms of 8 rows x 128 B; row rr of an atom holds its eight 16-byte chunks at
-//   chunk position (c ^ rr)  -> exactly the shared-memory image wgmma expects, so a tile moves
-//   HBM -> SMEM with one linear cp.async.bulk (no tensor map needed).
+//   tile(rt, kb) at float offset (rt * KB + kb) * 4096, KB = ceil(K/32); row r of a tile is the 32-float span at r * 32
+//   inside a span the eight 16-byte chunks sit at chunk position (c16 ^ (r & 7))  -> exactly the shared-memory image
+//   wgmma expects, so a tile moves HBM -> SMEM with one linear cp.async.bulk (no tensor map needed).
+// MN-major flavour of the same tile (for tensors whose reduction runs along the image ROWS): same spans, but the four
+// 32-byte chunks of a span are permuted by (c32 ^ (r & 3)).  tf32 wgmma reads K-major operands only, so the GEMM kernels
+// rewrite an MN-major stage into the K-major image in shared memory before the MMAs (tcg::stage_to_kmajor).
+// Every writer of an image places its values through img_span + k_swz / mn_swz.
 constexpr int kTileRows = 128;
 constexpr int kTileK = 32;                       // fp32 elements per 128-byte swizzle span
 constexpr int kTileFloats = kTileRows * kTileK;  // 4096 floats = 16 KB
 constexpr int kTileBytes = kTileFloats * 4;
 
-__host__ __device__ __forceinline__ int64_t packed_offset(int64_t row, int64_t k, int64_t KB) {
-  int64_t rt = row >> 7, r = row & 127, kb = k >> 5, kk = k & 31;
-  int64_t atom = r >> 3, rr = r & 7, c = kk >> 2, j = kk & 3;
-  return (rt * KB + kb) * kTileFloats + atom * 256 + rr * 32 + ((c ^ rr) << 2) + j;
+// floats of one image (one part: hi or lo, one flavour) of a [rows, cols] matrix, padded to whole tiles
+__host__ __device__ __forceinline__ int64_t img_floats(int64_t rows, int64_t cols) {
+  return ((rows + 127) / 128) * ((cols + 31) / 32) * kTileFloats;
 }
 
-// MN-major flavour of the same tile (for tensors whose reduction runs along the image ROWS): same geometry (row r at
-// byte r*128 of the tile), but the four 32-byte chunks of a row are permuted by (c32 ^ (r & 3)) instead of the eight
-// 16-byte chunks by (c16 ^ (r & 7)).  tf32 wgmma reads K-major operands only, so the GEMM kernels rewrite an MN-major
-// stage into the K-major image in shared memory before the MMAs (tcg::stage_to_kmajor).
+// float offset of the 32-float span of row r (0..127) of row tile rt in column block cb
+template <class R>
+__host__ __device__ __forceinline__ int64_t img_span(int64_t rt, R r, int64_t cb, int64_t KB) {
+  return (rt * KB + cb) * kTileFloats + r * 32;
+}
+// the same for image row `row`
+__host__ __device__ __forceinline__ int64_t img_span(int64_t row, int64_t cb, int64_t KB) {
+  return img_span(row >> 7, row & 127, cb, KB);
+}
+
+// position of column c (0..31) of a block inside the span of image row `row`, K-major / MN-major, plus `span` (the span's
+// offset, when the caller passes it).  The chunk index is swizzled in the column's type and added to the span before the
+// column's low bits, so that callers keep their index widths.
+template <class R, class C, class S = C>
+__host__ __device__ __forceinline__ S k_swz(R row, C c, S span = 0) {
+  return span + (((c >> 2) ^ (C)(row & 7)) << 2) + (c & 3);
+}
+template <class R, class C, class S = C>
+__host__ __device__ __forceinline__ S mn_swz(R row, C c, S span = 0) {
+  return span + (((c >> 3) ^ (C)(row & 3)) << 3) + (c & 7);
+}
+
+__host__ __device__ __forceinline__ int64_t packed_offset(int64_t row, int64_t k, int64_t KB) {
+  return k_swz(row, k & 31, img_span(row, k >> 5, KB));
+}
 __host__ __device__ __forceinline__ int64_t packed_offset_mn(int64_t row, int64_t k, int64_t KB) {
-  int64_t rt = row >> 7, r = row & 127, kb = k >> 5, kk = k & 31;
-  int64_t c32 = kk >> 3, j = kk & 7;
-  return (rt * KB + kb) * kTileFloats + r * 32 + ((c32 ^ (r & 3)) << 3) + j;
+  return mn_swz(row, k & 31, img_span(row, k >> 5, KB));
 }
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -123,6 +144,34 @@ __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
   uint32_t l;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(l) : "f"(rest));
   lo = __uint_as_float(l);
+}
+
+// Which images pack_tile stores: the K-major pair, both flavours, or each flavour whose hi pointer is set (checked at run time)
+enum class Parts { k, both, present };
+
+// Packs row tile rt of an image with kb column blocks, one 16-byte chunk per thread and iteration; the CTAs along blockIdx.y
+// share the tile.  load(row, k0, x) fills x[0..3] with columns k0..k0+3 of image row `row` (zero outside the source).
+template <Parts P, class Load>
+__device__ __forceinline__ void pack_tile(int rt, int kb, float* k_hi, float* k_lo, float* mn_hi, float* mn_lo, Load load) {
+  for (int q = threadIdx.x + blockIdx.y * blockDim.x; q < 128 * kb * 8; q += blockDim.x * gridDim.y) {
+    const int c16 = q & 7, t = q >> 3;
+    const int cb = t % kb, r = t / kb;  // consecutive threads walk along a row: coalesced reads
+    float x[4], h[4], l[4];
+    load(rt * 128 + r, cb * 32 + c16 * 4, x);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) split_tf32(x[j], h[j], l[j]);
+    const int64_t span = img_span((int64_t)rt, r, cb, kb);
+    if (P != Parts::present || k_hi) {
+      const int64_t o = k_swz(r, c16 * 4, span);
+      *reinterpret_cast<float4*>(k_hi + o) = make_float4(h[0], h[1], h[2], h[3]);
+      *reinterpret_cast<float4*>(k_lo + o) = make_float4(l[0], l[1], l[2], l[3]);
+    }
+    if (P == Parts::both || (P == Parts::present && mn_hi)) {
+      const int64_t o = mn_swz(r, c16 * 4, span);
+      *reinterpret_cast<float4*>(mn_hi + o) = make_float4(h[0], h[1], h[2], h[3]);
+      *reinterpret_cast<float4*>(mn_lo + o) = make_float4(l[0], l[1], l[2], l[3]);
+    }
+  }
 }
 
 }  // namespace tc

@@ -265,8 +265,8 @@ __global__ void __launch_bounds__(tcg::kThreads, 1) k_cluster(const tcg::Problem
         x = do_relu ? fmaxf(x, 0.0f) : x;
         x = (n < pN && m < m_valid) ? x : 0.0f;
         if (EPI == 2) {
-          const int64_t span = ((orow >> 7) * o_kb + (ocb0 + g)) * kTileFloats + (orow & 127) * 32;
-          const int64_t pos_k = span + ((((lane >> 2) ^ (int)(orow & 7))) << 2) + (lane & 3);
+          const int64_t span = img_span(orow, ocb0 + g, o_kb);
+          const int64_t pos_k = k_swz(orow, lane, span);
           const float mk = (do_mask && live && g < n_blocks) ? __ldg(mask_p + pos_k) : 1.0f;
           x = (mk > 0.0f) ? x : 0.0f;
         }
@@ -288,13 +288,13 @@ __global__ void __launch_bounds__(tcg::kThreads, 1) k_cluster(const tcg::Problem
         const float x = r_x[rr][g];
         if (c_p && n < pN) tcg::st_global(c_p + (int64_t)m * ldc + n, x);
         if (EPI == 2) {
-          const int64_t span = ((orow >> 7) * o_kb + (ocb0 + g)) * kTileFloats + (orow & 127) * 32;
-          const int64_t pos_k = span + ((((lane >> 2) ^ (int)(orow & 7))) << 2) + (lane & 3);
+          const int64_t span = img_span(orow, ocb0 + g, o_kb);
+          const int64_t pos_k = k_swz(orow, lane, span);
           float h, l;
           split_tf32(x, h, l);
           if (ok_hi) { tcg::st_global(ok_hi + pos_k, h); tcg::st_global(ok_lo + pos_k, l); }
           if (omn_hi) {
-            const int64_t pos_mn = span + ((((lane >> 3) ^ (int)(orow & 3))) << 3) + (lane & 7);
+            const int64_t pos_mn = mn_swz(orow, lane, span);
             tcg::st_global(omn_hi + pos_mn, h);
             tcg::st_global(omn_lo + pos_mn, l);
           }
@@ -435,13 +435,13 @@ __global__ void __launch_bounds__(tcg::kThreads, 1) k_lstm_cluster(const tcl::St
         for (int g = 0; g < 4; ++g) tcg::st_global(g_gates + row * H4 + g * H + u, r_act[rr][g]);
         tcg::st_global(g_c + row * H + u, r_c[rr]);
         tcg::st_global(g_h + row * H + u, r_h[rr]);
-        const int64_t span = ((row >> 7) * hkb + nt) * kTileFloats + (row & 127) * 32;
+        const int64_t span = img_span(row, nt, hkb);
         float hh, hl;
         split_tf32(r_h[rr], hh, hl);
-        const int64_t pos_k = span + ((((lane >> 2) ^ (int)(row & 7))) << 2) + (lane & 3);
+        const int64_t pos_k = k_swz(row, lane, span);
         tcg::st_global(g_hk_hi + pos_k, hh);
         tcg::st_global(g_hk_lo + pos_k, hl);
-        const int64_t pos_mn = span + ((((lane >> 3) ^ (int)(row & 3))) << 3) + (lane & 7);
+        const int64_t pos_mn = mn_swz(row, lane, span);
         tcg::st_global(g_hmn_hi + pos_mn, hh);
         tcg::st_global(g_hmn_lo + pos_mn, hl);
       }

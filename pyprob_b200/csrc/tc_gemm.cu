@@ -66,10 +66,7 @@ extern "C" {
 // Phase-trace buffer (64 launches x 16 slots of globaltimer stamps) for the tensor-core grouped GEMM; NULL disables.
 int ppb_debug_trace(void* buf_dev) { g_trace = (unsigned long long*)buf_dev; g_trace_launch = 0; return PPB_OK; }
 
-int64_t ppb_packed_floats(int64_t rows, int64_t K) {
-  int64_t RT = (rows + tc::kTileRows - 1) / tc::kTileRows, KB = (K + tc::kTileK - 1) / tc::kTileK;
-  return RT * KB * tc::kTileFloats;
-}
+int64_t ppb_packed_floats(int64_t rows, int64_t K) { return img_floats(rows, K); }
 
 int ppb_pack_tf32(const float* X, int64_t rows, int64_t K, int64_t ldx, float* hi_out, float* lo_out, void* stream) {
   PPB_CHECK_ARG(X && hi_out && rows > 0 && K > 0 && ldx >= K, "bad arguments");

@@ -313,7 +313,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_grouped(const Problem* __restri
       const float bias = (bias_p && col_ok) ? __ldg(bias_p + n) : 0.0f;
       // the warp's 32 rows sit inside one 128-row image tile (m_base % 32 == 0, o_row0 % 128 == 0): row r of the block is
       // image row (orow0 + r), so (orow & 7) == (r & 7) and the span offset advances by 32 floats per row
-      const int64_t span0 = ((orow0 >> 7) * o_kb + (ocb0 + cb)) * kTileFloats + (orow0 & 127) * 32;
+      const int64_t span0 = img_span(orow0, ocb0 + cb, o_kb);
       float* cp = c_p ? c_p + (int64_t)m_base * ldc + n : nullptr;
       const bool c_ok = cp != nullptr && col_ok;
       // rows in batches of eight: the ReLU-mask loads of a batch are issued together (one L2 round trip per batch instead of
@@ -325,7 +325,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_grouped(const Problem* __restri
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
             const int r = rb + j;
-            const int64_t pos_k = span0 + r * 32 + ((((lane >> 2) ^ (r & 7))) << 2) + (lane & 3);
+            const int64_t pos_k = k_swz(r, lane, span0 + r * 32);
             // explicit loads into distinct registers, issued back to back (the compiler folded the predicated __ldg's into
             // one register and serialised them)
             mk[j] = 1.0f;
@@ -344,14 +344,14 @@ __global__ void __launch_bounds__(kThreads, 1) k_grouped(const Problem* __restri
           } else if (EPI == 1) {
             if (live && c_ok && x != 0.0f) red_add_global(cp + (int64_t)r * ldc, x);
           } else {
-            const int64_t pos_k = span0 + r * 32 + ((((lane >> 2) ^ (r & 7))) << 2) + (lane & 3);
+            const int64_t pos_k = k_swz(r, lane, span0 + r * 32);
             if (do_mask && live) x = (mk[j] > 0.0f) ? x : 0.0f;
             if (live && c_ok) st_global(cp + (int64_t)r * ldc, x);
             float h, l;
             split_tf32(x, h, l);
             if (live && ok_hi) { st_global(ok_hi + pos_k, h); st_global(ok_lo + pos_k, l); }
             if (live && omn_hi) {
-              const int64_t pos_mn = span0 + r * 32 + ((((lane >> 3) ^ (r & 3))) << 3) + (lane & 7);
+              const int64_t pos_mn = mn_swz(r, lane, span0 + r * 32);
               st_global(omn_hi + pos_mn, h);
               st_global(omn_lo + pos_mn, l);
             }

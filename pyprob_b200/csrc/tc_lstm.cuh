@@ -122,14 +122,14 @@ __device__ __forceinline__ void cell_epilogue(float* staging, const float* ctile
     }
     tcg::st_global(io.c + row * H + u, cn);
     tcg::st_global(io.h + row * H + u, hn);
-    // image position of (row, u): tile (row / 128, nt), row span of 32 floats, swizzled chunk
-    const int64_t span = ((row >> 7) * hkb + nt) * kTileFloats + (row & 127) * 32;
+    // image position of (row, u): column lane of block nt
+    const int64_t span = img_span(row, nt, hkb);
     float hh, hl;
     split_tf32(hn, hh, hl);
-    const int64_t pos_k = span + ((((lane >> 2) ^ (int)(row & 7))) << 2) + (lane & 3);
+    const int64_t pos_k = k_swz(row, lane, span);
     tcg::st_global(io.hk_hi + pos_k, hh);
     tcg::st_global(io.hk_lo + pos_k, hl);
-    const int64_t pos_mn = span + ((((lane >> 3) ^ (int)(row & 3))) << 3) + (lane & 7);
+    const int64_t pos_mn = mn_swz(row, lane, span);
     tcg::st_global(io.hmn_hi + pos_mn, hh);
     tcg::st_global(io.hmn_lo + pos_mn, hl);
   }
@@ -180,20 +180,13 @@ inline size_t smem_bytes() { return sizeof(Smem) + 1024; }
 // W_hh [4H, H] (row-major, gate-major rows) -> K-format hi / lo tile image with gate-interleaved rows
 static __global__ void __launch_bounds__(256) k_pack_whh_interleaved(const float* __restrict__ w_hh, int H,
                                                                float* __restrict__ img_hi, float* __restrict__ img_lo) {
-  const int kb = H / 32;
   const int rt = blockIdx.x;             // packed row tile = block of 32 hidden units
-  for (int qi = threadIdx.x + blockIdx.y * blockDim.x; qi < 128 * kb * 8; qi += blockDim.x * gridDim.y) {
-    const int c16 = qi & 7, t = qi >> 3;
-    const int cb = t % kb, r = t / kb;   // r = packed row inside the tile = gate * 32 + j
+  pack_tile<Parts::k>(rt, H / 32, img_hi, img_lo, nullptr, nullptr, [&](int row, int k0, float (&x)[4]) {
+    const int r = row - rt * 128;        // packed row inside the tile = gate * 32 + j
     const int src_row = (r >> 5) * H + rt * 32 + (r & 31);
-    const int k0 = cb * 32 + c16 * 4;
-    float h[4], l[4];
 #pragma unroll
-    for (int j = 0; j < 4; ++j) split_tf32(__ldg(w_hh + (int64_t)src_row * H + k0 + j), h[j], l[j]);
-    const int64_t o = ((int64_t)rt * kb + cb) * kTileFloats + r * 32 + ((c16 ^ (r & 7)) << 2);
-    *reinterpret_cast<float4*>(img_hi + o) = make_float4(h[0], h[1], h[2], h[3]);
-    *reinterpret_cast<float4*>(img_lo + o) = make_float4(l[0], l[1], l[2], l[3]);
-  }
+    for (int j = 0; j < 4; ++j) x[j] = __ldg(w_hh + (int64_t)src_row * H + k0 + j);
+  });
 }
 
 }  // namespace tcl

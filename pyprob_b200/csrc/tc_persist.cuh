@@ -109,7 +109,7 @@ __global__ void __launch_bounds__(tcg::kThreads, 1) k_grouped_persistent(const t
       const int n = n0 + lane;
       const bool col_ok = n < pN;
       const float bias = (bias_p && col_ok) ? __ldg(bias_p + n) : 0.0f;
-      const int64_t span0 = ((orow0 >> 7) * o_kb + (ocb0 + cb)) * kTileFloats + (orow0 & 127) * 32;
+      const int64_t span0 = img_span(orow0, ocb0 + cb, o_kb);
       float* cp = c_p ? c_p + (int64_t)m_base * ldc + n : nullptr;
       const bool c_ok = cp != nullptr && col_ok;
 #pragma unroll
@@ -119,7 +119,7 @@ __global__ void __launch_bounds__(tcg::kThreads, 1) k_grouped_persistent(const t
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
             const int r = rb + j;
-            const int64_t pos_k = span0 + r * 32 + ((((lane >> 2) ^ (r & 7))) << 2) + (lane & 3);
+            const int64_t pos_k = k_swz(r, lane, span0 + r * 32);
             mk[j] = 1.0f;
             if (do_mask && r < rows) asm volatile("ld.global.nc.f32 %0, [%1];" : "=f"(mk[j]) : "l"(mask_p + pos_k));
           }
@@ -136,14 +136,14 @@ __global__ void __launch_bounds__(tcg::kThreads, 1) k_grouped_persistent(const t
           } else if (EPI == 1) {
             if (live && c_ok && x != 0.0f) tcg::red_add_global(cp + (int64_t)r * ldc, x);
           } else {
-            const int64_t pos_k = span0 + r * 32 + ((((lane >> 2) ^ (r & 7))) << 2) + (lane & 3);
+            const int64_t pos_k = k_swz(r, lane, span0 + r * 32);
             if (do_mask && live) x = (mk[j] > 0.0f) ? x : 0.0f;
             if (live && c_ok) tcg::st_global(cp + (int64_t)r * ldc, x);
             float h, l;
             split_tf32(x, h, l);
             if (live && ok_hi) { tcg::st_global(ok_hi + pos_k, h); tcg::st_global(ok_lo + pos_k, l); }
             if (live && omn_hi) {
-              const int64_t pos_mn = span0 + r * 32 + ((((lane >> 3) ^ (r & 3))) << 3) + (lane & 7);
+              const int64_t pos_mn = mn_swz(r, lane, span0 + r * 32);
               tcg::st_global(omn_hi + pos_mn, h);
               tcg::st_global(omn_lo + pos_mn, l);
             }
