@@ -328,7 +328,7 @@ typedef struct {
 int ppb_batch_from_image(const void* image_host, const void* image_dev, int64_t image_bytes,
                          ppb_batch* out);
 /* sizeof() of the ABI structs, for binding self-checks: 0 = ppb_net_desc, 1 = ppb_addr_desc,
- * 2 = ppb_batch, 3 = ppb_ff_desc, 4 = ppb_linear_desc */
+ * 2 = ppb_batch, 3 = ppb_ff_desc, 4 = ppb_linear_desc, 5 = tcg::Problem (ppb_tc_run_problems) */
 int64_t ppb_sizeof(int which);
 
 /* precision of the tensor-core GEMMs: 0 = 3xTF32 split (fp32-faithful, parity mode, default),
@@ -512,6 +512,15 @@ int ppb_debug_trace(void* buf16_dev);
 int ppb_gemm_packed_tn(const float* X_hi, const float* X_lo, const float* Y_hi, const float* Y_lo,
                        float* C, int64_t M, int64_t N, int64_t R, int64_t ldc, int precision,
                        void* stream);
+/* Runs n tensor-core GEMM descriptors (host array of tcg::Problem, csrc/tc_grouped.cuh; ppb_sizeof(5) bytes each) as one
+ * launch of the kernel the network would use: cluster_size 1 = the grouped kernel, or its persistent form when the problems
+ * have more tiles than SMs (PPB_PERSISTENT=0 keeps the grouped one); 2, 4, 8 = cluster split-K; chunk_table != 0 = the
+ * grouped kernel that reads the K-major A through its chunk table.  epi: 0 = fp32 store, 1 = fp32 red.add, 2 = tile images
+ * (+ fp32).  The tile bookkeeping (tiles_m, tiles_n, tile_start, k_splits >= 1) is filled in here.  Combinations the kernels
+ * do not implement are refused before anything is uploaded or launched.  The K padding of the last 32-element reduction
+ * chunk must be zero in both operands. */
+int ppb_tc_run_problems(const void* problems_host, int n, int epi, int cluster_size, int chunk_table, int precision,
+                        void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * 7. Metropolis-Hastings chains (LMH / RMH), csrc/mcmc.cu.  C chains run as the C lanes of one lock-step execution.

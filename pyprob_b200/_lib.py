@@ -78,6 +78,7 @@ _SIGNATURES = {
     'ppb_gemm_packed_tn': [c_f, c_f, c_f, c_f, c_f, c_i64, c_i64, c_i64, c_i64, c_int, c_f],
     'ppb_gemm_packed': [c_f, c_f, c_f, c_f, c_f, c_i64, c_i64, c_i64, c_i64, c_f, c_int, c_int, c_f],
     'ppb_gemm_packed_cluster': [c_f, c_f, c_f, c_f, c_f, c_i64, c_i64, c_i64, c_i64, c_f, c_int, c_int, c_int, c_f],
+    'ppb_tc_run_problems': [C.c_void_p, c_int, c_int, c_int, c_int, c_int, c_f],
     'ppb_mh_select': [c_f, c_f, c_f, c_i64, c_i64, c_int, c_f, c_f, c_f, c_f, c_f, c_int, c_u64, c_u64, c_f],
     'ppb_mh_fetch': [c_f, c_f, c_f, c_f, c_f, c_i64, c_i64, c_int, c_f, c_i64, c_i64, c_f, c_f, c_f, c_f],
     'ppb_mh_site': [c_int, c_int, c_f, c_i64, c_i64, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_int, c_f, c_int, c_f, c_f,

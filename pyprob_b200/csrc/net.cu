@@ -1894,6 +1894,7 @@ int64_t ppb_sizeof(int which) {
     case 2: return sizeof(ppb_batch);
     case 3: return sizeof(ppb_ff_desc);
     case 4: return sizeof(ppb_linear_desc);
+    case 5: return sizeof(tcg::Problem);
     default: return -1;
   }
 }

@@ -26,12 +26,12 @@ __device__ __forceinline__ float ld_global(const float* p) { float v; asm volati
 
 enum : int {
   kRelu = 1,        // max(x, 0)
-  kAccumulate = 2,  // fp32 output: C += result (exclusive owner)
   kMaskImg = 4,     // result = mask_img(m, n) > 0 ? result : 0   (mask image: K-format hi part, output geometry)
   kZeroInvalid = 8, // rows m >= m_valid produce zeros (padding rows of a segment)
 };
-// Split-K: when k_splits > 1 the reduction is divided over k_splits CTAs per output tile and the fp32 result
-// is combined with atomicAdd (the caller zero-initialises / accumulates into C; no images, bias or mask).
+// Epilogue 1 always adds into C (red.add), so the caller zero-initialises C or accumulates into it.
+// Split-K: when k_splits > 1 the reduction is divided over k_splits CTAs per output tile and the fp32 result is combined
+// that way (epilogue 1 only; no images, bias, ReLU, mask or zero-invalid rows).
 
 struct Operand {
   const float* hi;

@@ -71,6 +71,19 @@ int profiled(double prof_flops, cudaStream_t st, F&& launch) {
   return prof_end(e0, st, prof_flops);
 }
 
+// Appends problem p to phase ph: fills its tile bookkeeping (tiles_m, tiles_n, tile_start inside the phase, k_splits >= 1) and
+// counts its tiles.  A problem with an empty dimension computes nothing and is not appended (false).
+inline bool phase_add(gemm::Phase& ph, tcg::Problem& p) {
+  if (p.M <= 0 || p.N <= 0 || p.K <= 0) return false;
+  p.tiles_m = (p.M + 127) / 128;
+  p.tiles_n = (p.N + 127) / 128;
+  p.tile_start = ph.tiles;
+  if (p.k_splits < 1) p.k_splits = 1;
+  ph.tiles += p.tiles_m * p.tiles_n * p.k_splits;
+  ph.count += 1;
+  return true;
+}
+
 // A phase of tcg::k_grouped with epilogue EPI: 0 = fp32 store, 1 = fp32 reduction (weight gradients / split-K), 2 = tile images
 // (+ fp32).  With more tiles than SMs it runs the persistent form (tc_persist.cuh), which overlaps every tile's epilogue with
 // the next tile's mainloop, unless the launch is traced.
@@ -86,6 +99,15 @@ int run_tc_phase(const gemm::Phase& ph, const tcg::Problem* dev, int precision, 
                                                              ph.count, ph.tiles);
       return tc_launch<tcg::k_grouped<x3, EPI>>(ph.tiles, tcg::smem_bytes(), 1, pdl, st, dev + ph.first, ph.count, tr);
     });
+  });
+}
+
+// A phase of tcg::k_grouped whose A operands are read through their chunk tables (the KTAB instantiation, epilogue 0)
+inline int run_tc_phase_ktab(const gemm::Phase& ph, const tcg::Problem* dev, int precision, cudaStream_t st, bool pdl = true) {
+  if (ph.count == 0) return PPB_OK;
+  return with_x3(precision, [&](auto x3) {
+    return tc_launch<tcg::k_grouped<x3, 0, true>>(ph.tiles, tcg::smem_bytes(), 1, pdl, st, dev + ph.first, ph.count,
+                                                  (unsigned long long*)nullptr);
   });
 }
 
