@@ -71,10 +71,12 @@ def _head_log_q(params, address, family, num_categories, K, h, values, prior0, p
     return out.index_copy(0, keep, lq(keep)) if keep.numel() else out
 
 
-def loss_and_grads(params, sub_batches, observe_names, observe_in_dims, K, dtype=torch.float64, addr_dim=64, type_dim=8):
+def loss_and_grads(params, sub_batches, observe_names, observe_in_dims, K, dtype=torch.float64, addr_dim=64, type_dim=8,
+                   embed=onet.embed_observe):
     """params: reference state_dict names -> tensors; sub_batches: dicts as synthetic.random_sub_batch makes (numpy or
     torch).  Returns {'loss', 'lps': per sub-batch [T, B] log q, 'grads': keyed like params, 'steps': per sub-batch a list
-    over t of {'x', 'pre', 'act', 'c', 'h', 'dgates'}}, all detached, at `dtype`."""
+    over t of {'x', 'pre', 'act', 'c', 'h', 'dgates'}}, all detached, at `dtype`.  `embed` computes each sub-batch's
+    observation embedding (signature of onet.embed_observe; tests/obs_fp64.py passes one that keeps every layer)."""
     p = {k: torch.as_tensor(v).detach().to(dtype).clone().requires_grad_(True) for k, v in params.items()}
     W_ih, W_hh = p['_layers_lstm.weight_ih_l0'], p['_layers_lstm.weight_hh_l0']
     b_ih, b_hh = p['_layers_lstm.bias_ih_l0'], p['_layers_lstm.bias_hh_l0']
@@ -85,7 +87,7 @@ def loss_and_grads(params, sub_batches, observe_names, observe_in_dims, K, dtype
     for sb in sub_batches:
         values, prior0, prior1 = (torch.as_tensor(sb[k]).to(dtype) for k in ('values', 'prior0', 'prior1'))
         T, B = values.shape
-        obs_emb = onet.embed_observe(p, torch.as_tensor(sb['obs']).to(dtype), observe_names, observe_in_dims)
+        obs_emb = embed(p, torch.as_tensor(sb['obs']).to(dtype), observe_names, observe_in_dims)
         h = torch.zeros(B, H, dtype=dtype)
         c = torch.zeros(B, H, dtype=dtype)
         sub_lp, sub_steps = [], []

@@ -184,6 +184,12 @@ def _truncated_head(name):
     return any(name.startswith('_layers_proposal.{}.'.format(a)) for a, fam, _ in TABLE if fam in ('Uniform', 'Poisson'))
 
 
+def _abs_err(got, want):
+    """|got - want| with NaN as +inf: a NaN that reaches a result (an unwritten or poisoned row) fails every tolerance,
+    where torch's max and norm would turn it into a NaN that Python's max() then drops."""
+    return torch.nan_to_num((torch.as_tensor(got, dtype=torch.float64) - want).abs(), nan=math.inf)
+
+
 def errors(net, subs, enc, loss, lp, grad, ref, M):
     """Worst error of each observable in units of its tolerance scale:
       lq        log q of every (t, row) and the loss, against 1 + |want|
@@ -195,7 +201,7 @@ def errors(net, subs, enc, loss, lp, grad, ref, M):
       norm_trunc  the same for the truncated-normal head tensors"""
     a = enc.arrays
     out = dict.fromkeys(('lq', 'lstm', 'lstm_row', 'trunc', 'other', 'norm', 'norm_trunc'), 0.0)
-    out['lq'] = abs(loss - float(ref['loss'])) / (1 + abs(float(ref['loss'])))
+    out['lq'] = float(_abs_err(loss, ref['loss'])) / (1 + abs(float(ref['loss'])))
     for pos, s in enumerate(enc.sub_order):
         want = ref['lps'][s]
         T, B = want.shape
@@ -204,10 +210,10 @@ def errors(net, subs, enc, loss, lp, grad, ref, M):
             assert a['step_nrows'][st] == B
             r0 = int(a['step_row0'][st])
             got = lp[r0:r0 + B]
-            out['lq'] = max(out['lq'], float(((got - want[t]).abs() / (1 + want[t].abs())).max()))
+            out['lq'] = max(out['lq'], float((_abs_err(got, want[t]) / (1 + want[t].abs())).max()))
     for k, want in ref['grads'].items():
         got = net.grad_view(k, grad).cpu().double()
-        err = (got - want).abs()
+        err = _abs_err(got, want)
         nk = 'norm_trunc' if _truncated_head(k) else 'norm'
         out[nk] = max(out[nk], float(err.norm()) / max(float(want.norm()), 1e-12))
         if k in M:
@@ -334,7 +340,7 @@ def test_infer_step_vs_fp64(cuda, H):
     steps = [{'address': a, 'family': f, 'num_categories': C, 'prev_value': sb['values'][t - 1] if t else None}
              for t, (a, f, C) in enumerate(seq)]
     want = lstm_fp64.infer_steps(params, torch.cat([obs['o0'], obs['o1']]), list(OBS), IN_DIMS, steps, n=n)
-    worst = max(float(((g - w).abs() / (1 + w.abs())).max()) for gw, ww in zip(got, want) for g, w in zip(gw, ww))
+    worst = max(float((_abs_err(g, w) / (1 + w.abs())).max()) for gw, ww in zip(got, want) for g, w in zip(gw, ww))
     check({'infer': worst}, 0, keys=('infer',))
 
 
