@@ -49,10 +49,27 @@ struct Plan {
   // embedding and the P_obs GEMM on the critical path (only when B % 128 == 0 and E % 32 == 0: no padding to zero-fill)
   float* emb_k_hi; float* emb_k_lo; float* emb_mn_hi; float* emb_mn_lo;
   long long emb_kb;
+  // optional (G > 0, LSTM network): k_bwd forms d obs_emb = d_pobs W_ih[:, :E] itself (form_d_emb) instead of reading it.
+  // Rank r of a cluster reduces over gates [r G / kCluster, (r + 1) G / kCluster) in chunks of kg gates.
+  int G, kg;
+  int64_t wih_off, ld_wih; int wih_vec;   // W_ih row g at arena + wih_off + g * ld_wih; wih_vec: rows copied 16 bytes at a time
+  const float* dp; int64_t ld_dp;         // d_pobs rows
+  // non-null: dp holds batch rows (the T = 1 dgates), and trace tr's row is its sub-batch's first t = 0 row plus its place
+  // in the sub-batch (whose first trace is row_trace of that row); null: dp holds one row per trace
+  const int* trace_sub; const int* step_row0; const int* row_trace;
 };
 
 inline size_t smem_fwd(const Plan& p) { return (size_t)(p.w_floats + kMT * p.A) * sizeof(float); }
 inline size_t smem_bwd(const Plan& p) { return (size_t)(p.w_floats + p.part_floats + kMT * (p.A + p.Dz)) * sizeof(float); }
+// form_d_emb's buffers, from the end of the staged weights (over act / dz / part, which it runs before): a chunk of the
+// W_ih[:, :E] slice (kg x emb_wp), the d_pobs chunk of the cluster's kCluster * kMT traces of a round (pitch kg + 4) and
+// their partial sums (x emb_wp).  Overlaid rather than appended: the kernel is slower with the larger allocation.
+constexpr int kRoundTraces = kCluster * kMT;
+__host__ __device__ inline int emb_wp(int E) { return (E + 3) & ~3; }
+inline size_t smem_emb(const Plan& p, int kg) {
+  const int wp = emb_wp(p.E);
+  return (size_t)(p.w_floats + kg * wp + kRoundTraces * (kg + 4) + kRoundTraces * wp) * sizeof(float);
+}
 
 __device__ __forceinline__ void cp_async16(float* smem_dst, const float* gmem_src) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gmem_src)
@@ -217,34 +234,169 @@ __device__ __forceinline__ void layer_dx(const Plan& P, const Layer& L, const fl
   }
 }
 
-// this chunk's share of dW[n][k] = sum_t dz[t][n] x[t][k] and db[n] = sum_t dz[t][n], added to part
+// this chunk's share of dW[n][k] = sum_t dz[t][n] x[t][k] and db[n] = sum_t dz[t][n], added to part.  A thread takes four
+// of its entries at a time and loads all their operands before the first read-modify-write of part: one entry after the
+// other, every sum was a chain of dependent shared-memory loads, and eight warps per SM could not hide it.  Traces t >= nt
+// enter as zeros (selected, not branched around), which keeps the sums those of the nt traces in the same order.
 __device__ __forceinline__ void layer_partial(const Plan& P, const Layer& L, const float* act, const float* dz, float* part,
                                               int nt) {
+  constexpr int kBatch = 4;
   const int in_dim = L.in_dim, out_dim = L.out_dim, A = P.A, Dz = P.Dz;
   const int nw = out_dim * in_dim;
   const float* dr = dz + L.dzoff;
   const float* xr = act + L.xoff;
   float* pr = part + L.part;
-  for (int e = threadIdx.x; e < nw + out_dim; e += kThreads) {
-    float v = 0.f;
-    if (e < nw) {
-      const int n = e / in_dim, k = e - n * in_dim;
+  const int dn = kThreads / in_dim, dk = kThreads - dn * in_dim;   // (n, k) of entry e + kThreads from those of e
+  int n = threadIdx.x / in_dim, k = threadIdx.x - n * in_dim;
+  for (int e = threadIdx.x; e < nw; e += kBatch * kThreads) {
+    float v[kBatch];
 #pragma unroll
-      for (int t = 0; t < kMT; ++t)
-        if (t < nt) v = fmaf(dr[t * Dz + n], xr[t * A + k], v);
-    } else {
+    for (int j = 0; j < kBatch; ++j) {
+      v[j] = 0.f;
+      const bool in = e + j * kThreads < nw;
 #pragma unroll
-      for (int t = 0; t < kMT; ++t)
-        if (t < nt) v += dr[t * Dz + e - nw];
+      for (int t = 0; t < kMT; ++t) {
+        const bool on = in && t < nt;
+        const float d = on ? dr[t * Dz + n] : 0.f, x = on ? xr[t * A + k] : 0.f;
+        v[j] = fmaf(d, x, v[j]);
+      }
+      n += dn; k += dk;
+      if (k >= in_dim) { k -= in_dim; ++n; }
     }
-    pr[e] += v;
+#pragma unroll
+    for (int j = 0; j < kBatch; ++j)
+      if (e + j * kThreads < nw) pr[e + j * kThreads] += v[j];
+  }
+  for (int o = threadIdx.x; o < out_dim; o += kThreads) {
+    float v = 0.f;
+#pragma unroll
+    for (int t = 0; t < kMT; ++t) v += t < nt ? dr[t * Dz + o] : 0.f;
+    pr[nw + o] += v;
   }
 }
 
-// d_emb holds d(loss)/d(obs_emb).  grad += dW, db of every layer.  grid = a multiple of kCluster CTAs (some may own no
-// trace: they still take part in the cluster reduction).
+// rows [g0, g0 + kg) of W_ih[:, :E] -> wsl[g * emb_wp + e]
+__device__ __forceinline__ void stage_wih(const Plan& P, const float* __restrict__ arena, float* wsl, int g0, int kg) {
+  const int E = P.E, wp = emb_wp(E);
+  const int64_t ld = P.ld_wih;
+  const float* src = arena + P.wih_off + (int64_t)g0 * ld;
+  if (P.wih_vec) {
+    const int q = E >> 2;
+    for (int c = threadIdx.x; c < kg * q; c += kThreads) {
+      const int g = c / q, k4 = c - g * q;
+      cp_async16(wsl + g * wp + 4 * k4, src + g * ld + 4 * k4);
+    }
+  } else {
+    for (int c = threadIdx.x; c < kg * E; c += kThreads) {
+      const int g = c / E, e = c - g * E;
+      cp_async4(wsl + g * wp + e, src + g * ld + e);
+    }
+  }
+}
+
+// d_emb[tr] = d_pobs[tr] W_ih[:, :E] for the traces of this CTA, exact fp32.  Round c takes the c-th chunk of kMT traces of
+// every rank of the cluster (kRoundTraces in all): each rank forms their partial sums over its gate slice, and the partials
+// meet in distributed shared memory, where rank r adds those of its own kMT traces in rank order (deterministic, no
+// atomics) and stores them to d_emb.  The first W_ih chunk is staged by the caller before the PDL wait.
+__device__ __forceinline__ void form_d_emb(const Plan& P, const float* __restrict__ arena, float* buf, float* d_emb, int B,
+                                           int traces_per_cta) {
+  const int E = P.E, wp = emb_wp(E), KG = P.kg, dpp = KG + 4, gs = P.G / kCluster;
+  float* wsl = buf;
+  float* dps = wsl + KG * wp;
+  float* pb = dps + kRoundTraces * dpp;
+  const uint32_t rank = tcc::cluster_ctarank();
+  const int cbase = (int)(blockIdx.x - rank) * traces_per_cta;   // first trace of the cluster
+  const int g_first = (int)rank * gs;
+  const int nch = (gs + KG - 1) / KG, rounds = (traces_per_cta + kMT - 1) / kMT;
+  const int np = (E + 1) >> 1;                                   // (trace quad, column pair) work items: 8 * np <= 2 * kThreads
+  const float* dp = P.dp;
+  const int64_t ld_dp = P.ld_dp;
+  const int* trace_sub = P.trace_sub; const int* step_row0 = P.step_row0; const int* row_trace = P.row_trace;
+  const uint32_t pb_addr = (uint32_t)__cvta_generic_to_shared(pb);
+  for (int c = 0; c < rounds; ++c) {
+    float acc[2][kMT][2];
+#pragma unroll
+    for (int k = 0; k < 2; ++k)
+#pragma unroll
+      for (int t = 0; t < kMT; ++t) acc[k][t][0] = acc[k][t][1] = 0.f;
+    for (int ch = 0; ch < nch; ++ch) {
+      const int g0 = ch * KG, kg = min(KG, gs - g0);
+      if (c > 0 || ch > 0) {
+        __syncthreads();   // every thread is through the previous chunk
+        if (nch > 1) stage_wih(P, arena, wsl, g_first + g0, kg);
+      }
+      const int q4 = kg >> 2;
+      for (int idx = threadIdx.x; idx < kRoundTraces * q4; idx += kThreads) {
+        const int j = idx / q4, k4 = idx - j * q4;
+        const int i = c * kMT + (j % kMT);
+        const int tr = cbase + (j / kMT) * traces_per_cta + i;
+        if (i >= traces_per_cta || tr >= B) continue;   // a slot without a trace: its sums are never stored
+        int row = tr;
+        if (trace_sub) {
+          const int r0 = __ldg(step_row0 + __ldg(trace_sub + tr));
+          row = r0 + tr - __ldg(row_trace + r0);
+        }
+        cp_async16(dps + j * dpp + 4 * k4, dp + (int64_t)row * ld_dp + g_first + g0 + 4 * k4);
+      }
+      cp_async_wait_all();
+      __syncthreads();
+#pragma unroll
+      for (int k = 0; k < 2; ++k) {
+        const int it = threadIdx.x + k * kThreads;
+        if (it >= kRoundTraces / kMT * np) continue;
+        const int q = it / np, p = it - q * np;
+        const float* dr = dps + q * kMT * dpp;
+        const float* wr = wsl + 2 * p;
+#pragma unroll 2
+        for (int g = 0; g < kg; g += 4) {
+          float d[kMT][4];
+#pragma unroll
+          for (int t = 0; t < kMT; ++t) {
+            const float4 v = *reinterpret_cast<const float4*>(dr + t * dpp + g);
+            d[t][0] = v.x; d[t][1] = v.y; d[t][2] = v.z; d[t][3] = v.w;
+          }
+#pragma unroll
+          for (int u = 0; u < 4; ++u) {
+            const float2 w = *reinterpret_cast<const float2*>(wr + (g + u) * wp);
+#pragma unroll
+            for (int t = 0; t < kMT; ++t) {
+              acc[k][t][0] = fmaf(d[t][u], w.x, acc[k][t][0]);
+              acc[k][t][1] = fmaf(d[t][u], w.y, acc[k][t][1]);
+            }
+          }
+        }
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+      const int it = threadIdx.x + k * kThreads;
+      if (it >= kRoundTraces / kMT * np) continue;
+      const int q = it / np, p = it - q * np;
+#pragma unroll
+      for (int t = 0; t < kMT; ++t) {
+        pb[(q * kMT + t) * wp + 2 * p] = acc[k][t][0];
+        pb[(q * kMT + t) * wp + 2 * p + 1] = acc[k][t][1];
+      }
+    }
+    tcc::cluster_sync_all();
+    for (int idx = threadIdx.x; idx < kMT * E; idx += kThreads) {
+      const int t = idx / E, e = idx - t * E;
+      const int i = c * kMT + t, tr = cbase + (int)rank * traces_per_cta + i;
+      if (i >= traces_per_cta || tr >= B) continue;
+      const uint32_t a = pb_addr + 4u * (uint32_t)(((int)rank * kMT + t) * wp + e);
+      float v = 0.f;
+#pragma unroll
+      for (int r = 0; r < kCluster; ++r) v += tcc::ld_cluster(tcc::map_to_rank(a, (uint32_t)r));
+      d_emb[(int64_t)tr * E + e] = v;
+    }
+    tcc::cluster_sync_all();   // the partial sums stay readable until every rank is through
+  }
+}
+
+// d_emb holds d(loss)/d(obs_emb), or (P.G > 0) is written with it by form_d_emb.  grad += dW, db of every layer.  grid = a
+// multiple of kCluster CTAs (some may own no trace: they still take part in the cluster reductions).
 __global__ void __launch_bounds__(kThreads) k_bwd(const __grid_constant__ Plan P, const float* __restrict__ arena,
-                                                  const float* __restrict__ d_emb, float* __restrict__ grad, int B,
+                                                  float* __restrict__ d_emb, float* __restrict__ grad, int B,
                                                   int traces_per_cta) {
   ppb_pdl_trigger();
   extern __shared__ __align__(16) float smem[];
@@ -252,15 +404,23 @@ __global__ void __launch_bounds__(kThreads) k_bwd(const __grid_constant__ Plan P
   float* act = smem + P.w_floats;
   float* dz = act + kMT * A;
   float* part = dz + kMT * Dz;
-  // Staged before the wait: the weights (arena).  Only the optimiser writes them, and no kernel of a training step can
-  // start before the previous step's optimiser has finished: k_fwd waits before it lets its dependents launch.  The
-  // first layer of a chain never propagates further down: it is not staged.
+  // Staged before the wait: the weights (arena), the first chunk of W_ih[:, :E] included.  Only the optimiser writes them,
+  // and no kernel of a training step can start before the previous step's optimiser has finished: k_fwd waits before it
+  // lets its dependents launch.  The first layer of a chain never propagates further down: it is not staged.
   for (int i = 0; i < n_layers; ++i)
     if (P.L[i].dxoff >= 0) stage_layer(smem, arena, P.L[i]);
-  for (int i = threadIdx.x; i < part_floats; i += kThreads) part[i] = 0.f;
+  const bool form = P.G > 0;
+  if (form) stage_wih(P, arena, act, (int)tcc::cluster_ctarank() * (P.G / kCluster), min(P.kg, P.G / kCluster));
+  else for (int i = threadIdx.x; i < part_floats; i += kThreads) part[i] = 0.f;
   // Everything else after it: the forward activations and the embedding are written by k_fwd of this same step, which a
-  // chain of programmatic edges does not order before this point (each kernel of the chain triggers before its own wait)
+  // chain of programmatic edges does not order before this point (each kernel of the chain triggers before its own wait);
+  // d_pobs by the kernel right before this one
   ppb_pdl_wait();
+  if (form) {
+    form_d_emb(P, arena, act, d_emb, B, traces_per_cta);   // its buffers overlay act, dz and part
+    for (int i = threadIdx.x; i < part_floats; i += kThreads) part[i] = 0.f;
+    __syncthreads();
+  }
   const int t_begin = blockIdx.x * traces_per_cta;
   const int t_end = min(B, t_begin + traces_per_cta);
   const int zoff = P.L[n_layers - 1].dzoff, eoff = P.L[n_layers - 1].yoff;
