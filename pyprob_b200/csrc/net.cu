@@ -45,6 +45,17 @@ struct PackEntry {  // one matrix of the weight-packing table
 // how the tensor-core pipeline runs the observe embedding (obs_embed.inc)
 enum class ObsForm { fused, tensor_core, simt };
 
+// The device regions whose last upload ppb_net remembers (upload_cached): the problem lists of a loss call (SIMT and tensor
+// core, forward in the first half of a region and backward in the second, and the tensor-core backward's reduction chunks),
+// those of an inference call, and the fused LSTM step list, which lives in memory the net owns.  forget_on_new_layout
+// forgets the lists of one kind of call: a contiguous range.
+enum UploadSlot {
+  kSlotSimtFwd, kSlotSimtBwd, kSlotTcFwd, kSlotTcBwd, kSlotChunks,  // loss calls (ws_layout)
+  kSlotInferSimt, kSlotInferTc,                                       // observe embedding and infer step (infer_layout)
+  kSlotLstmSteps,
+  kNumUploadSlots
+};
+
 struct ppb_net {
   // tensor-core path: packed tf32 images of every GEMM weight, refreshed from the arena each forward
   float* wimg = nullptr;
@@ -60,8 +71,8 @@ struct ppb_net {
   WImg w_fin[PPB_MAX_FF_LAYERS];
   // content hashes of the problem lists last uploaded to each device region: identical lists are not re-sent,
   // which also makes a repeated step capturable in a CUDA graph (no host->device copy inside the capture)
-  uint64_t slot_hash[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-  const void* slot_dev[10] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  uint64_t slot_hash[kNumUploadSlots] = {};
+  const void* slot_dev[kNumUploadSlots] = {};
   uint64_t ws_layout = 0;      // workspace address, batch dims and precision of the last loss call (forget_on_new_layout)
   uint64_t infer_layout = 0;   // workspace address, particle count and entry of the last inference call
   void* h_blob[2] = {nullptr, nullptr};
@@ -253,7 +264,7 @@ inline uint64_t fnv1a(const void* data, size_t n, uint64_t h = 14695981039346656
 }
 
 // Send `bytes` of host data to `dev` through the pinned staging ring unless the same content already lives there.
-int upload_cached(ppb_net* net, int slot, const void* src, size_t bytes, void* dev, cudaStream_t st) {
+int upload_cached(ppb_net* net, UploadSlot slot, const void* src, size_t bytes, void* dev, cudaStream_t st) {
   if (bytes == 0) return PPB_OK;
   uint64_t h = fnv1a(src, bytes, 1469598103934665603ULL ^ (uint64_t)bytes);
   if (net->slot_hash[slot] == h && net->slot_dev[slot] == dev) return PPB_OK;
@@ -282,9 +293,8 @@ int upload_cached(ppb_net* net, int slot, const void* src, size_t bytes, void* d
   return PPB_OK;
 }
 
-// slots: 0/1 SIMT forward/backward lists, 2/3 tensor-core forward/backward lists, 4 reduction-chunk lists,
-// 5 inference-time lists.  Forward and backward lists live in separate halves of the device region.
-int upload_and_get(ppb_net* net, const Builder& b, Problem* dev, int64_t cap, cudaStream_t st, int slot = 0) {
+// Send a SIMT problem list of at most `cap` problems to `dev`, tracked as `slot` (UploadSlot)
+int upload_and_get(ppb_net* net, const Builder& b, Problem* dev, int64_t cap, cudaStream_t st, UploadSlot slot) {
   size_t n = b.probs.size();
   if ((int64_t)n > cap) { ppb_set_error("problem list overflow (%zu > %lld)", n, (long long)cap); return PPB_ENOMEM; }
   return upload_cached(net, slot, b.probs.data(), n * sizeof(Problem), dev, st);
@@ -401,7 +411,18 @@ __global__ void k_smp_embed(const float* __restrict__ arena, const ppb_addr_desc
   }
 }
 
-// LSTM cell, one time step, all active rows (torch.nn.LSTM gate order i,f,g,o; h0 = c0 = 0, :186-187)
+// LSTM cell forward of one (row, unit) from its gate pre-activations (torch.nn.LSTM gate order i, f, g, o): the activations,
+// c_t and h_t.  c_prev() returns c_{t-1}; it is called after the activations, where both cell kernels issue that load.
+struct CellFwd { float i, f, g, o, c, h; };
+template <typename CPrev>
+__device__ __forceinline__ CellFwd cell_fwd_unit(const float (&pre)[4], CPrev c_prev) {
+  const float i = ppb_cell_sigmoid(pre[0]), f = ppb_cell_sigmoid(pre[1]);
+  const float g = ppb_cell_tanh(pre[2]), o = ppb_cell_sigmoid(pre[3]);
+  const float c = f * c_prev() + i * g;
+  return {i, f, g, o, c, o * ppb_cell_tanh(c)};
+}
+
+// LSTM cell, one time step, all active rows (h0 = c0 = 0, :186-187)
 __global__ void __launch_bounds__(256) k_cell_fwd(float* __restrict__ gates, const float* __restrict__ p_obs,
                                                    const float* __restrict__ p_step, const float* __restrict__ w_smp_t,
                                                    const float* __restrict__ smp_emb, const int* __restrict__ row_step,
@@ -434,20 +455,14 @@ __global__ void __launch_bounds__(256) k_cell_fwd(float* __restrict__ gates, con
       }
       pre[g] = v;
     }
-    float ig = ppb_cell_sigmoid(pre[0]);
-    float fg = ppb_cell_sigmoid(pre[1]);
-    float gg = ppb_cell_tanh(pre[2]);
-    float og = ppb_cell_sigmoid(pre[3]);
-    float cp = (t > 0) ? c[(int64_t)row_prev[row] * H + j] : 0.0f;
-    float cn = fg * cp + ig * gg;
-    float hn = og * ppb_cell_tanh(cn);
-    gates[(int64_t)row * 4 * H + j] = ig;
-    gates[(int64_t)row * 4 * H + H + j] = fg;
-    gates[(int64_t)row * 4 * H + 2 * H + j] = gg;
-    gates[(int64_t)row * 4 * H + 3 * H + j] = og;
-    c[(int64_t)row * H + j] = cn;
-    h[(int64_t)row * H + j] = hn;
-    if (himg.k_hi) tcg::img_store(himg.k_hi, himg.k_lo, himg.mn_hi, himg.mn_lo, row, j, himg.kb, hn);
+    const CellFwd u = cell_fwd_unit(pre, [&] { return (t > 0) ? c[(int64_t)row_prev[row] * H + j] : 0.0f; });
+    gates[(int64_t)row * 4 * H + j] = u.i;
+    gates[(int64_t)row * 4 * H + H + j] = u.f;
+    gates[(int64_t)row * 4 * H + 2 * H + j] = u.g;
+    gates[(int64_t)row * 4 * H + 3 * H + j] = u.o;
+    c[(int64_t)row * H + j] = u.c;
+    h[(int64_t)row * H + j] = u.h;
+    if (himg.k_hi) tcg::img_store(himg.k_hi, himg.k_lo, himg.mn_hi, himg.mn_lo, row, j, himg.kb, u.h);
   }
 }
 
@@ -1404,7 +1419,7 @@ int simt_loss_forward(ppb_net* net, const float* arena, const ppb_batch* b, void
   }
   int ph_h1, ph_h2;
   simt_head_fwd(bl, net, arena, b, w, H, ph_h1, ph_h2);
-  int rc = upload_and_get(net, bl, w.problems, w.max_problems / 2, st, 0);
+  int rc = upload_and_get(net, bl, w.problems, w.max_problems / 2, st, kSlotSimtFwd);
   if (rc) return rc;
 
   // ---- launches -----------------------------------------------------------------------------------
@@ -1465,7 +1480,7 @@ int simt_loss_backward(ppb_net* net, const float* arena, float* grad, const ppb_
   }
   const int ph_obs = obs_fp32_plan_bwd(bl, D, arena, grad, b->obs, d.B, w);
   Problem* dprobs = w.problems + w.max_problems / 2;
-  int rc = upload_and_get(net, bl, dprobs, w.max_problems / 2, st, 1);
+  int rc = upload_and_get(net, bl, dprobs, w.max_problems / 2, st, kSlotSimtBwd);
   if (rc) return rc;
 
   // ---- launches -----------------------------------------------------------------------------------
@@ -1586,9 +1601,9 @@ int64_t ppb_ic_workspace_bytes(const ppb_net* net, int32_t n_traces, int32_t n_r
 // The workspace regions move with the batch dims (carve, carve_tc; carve_infer with n), so a call with another layout may
 // write its buffers over a list an earlier call uploaded (a no-grad forward of a larger batch over the last step's backward
 // lists, _infer_init's embedding over the infer step's list): when the workspace address or the layout key changes, the
-// lists of slots [first, last] are sent again.  Slot 7 (the fused LSTM step list) lives in memory the net owns.
+// lists of slots [first, last] are sent again.  kSlotLstmSteps (the fused LSTM step list) lives in memory the net owns.
 static void forget_on_new_layout(ppb_net* net, uint64_t& last_key, const void* key, size_t key_bytes, const void* workspace,
-                                 int first, int last) {
+                                 UploadSlot first, UploadSlot last) {
   const uint64_t h = fnv1a(&workspace, sizeof(workspace), fnv1a(key, key_bytes));
   if (h == last_key) return;
   for (int i = first; i <= last; ++i) net->slot_hash[i] = 0;
@@ -1607,7 +1622,7 @@ int ppb_ic_loss_forward(ppb_net* net, const float* arena, const ppb_batch* b, vo
   PPB_CHECK_ARG(workspace_bytes >= ppb_ic_workspace_bytes(net, d.B, d.R, d.T, d.NS, d.G), "workspace too small");
   {
     const int key[6] = {d.B, d.R, d.T, d.NS, d.G, precision};
-    forget_on_new_layout(net, net->ws_layout, key, sizeof(key), workspace, 0, 4);
+    forget_on_new_layout(net, net->ws_layout, key, sizeof(key), workspace, kSlotSimtFwd, kSlotChunks);
   }
   cudaStream_t st = (cudaStream_t)stream;
   if (net->desc.network_type == PPB_NET_FEEDFORWARD)
@@ -1626,7 +1641,7 @@ int ppb_ic_loss_backward(ppb_net* net, const float* arena, float* grad, const pp
   PPB_CHECK_ARG(workspace_bytes >= ppb_ic_workspace_bytes(net, d.B, d.R, d.T, d.NS, d.G), "workspace too small");
   {
     const int key[6] = {d.B, d.R, d.T, d.NS, d.G, precision};
-    forget_on_new_layout(net, net->ws_layout, key, sizeof(key), workspace, 0, 4);
+    forget_on_new_layout(net, net->ws_layout, key, sizeof(key), workspace, kSlotSimtFwd, kSlotChunks);
   }
   cudaStream_t st = (cudaStream_t)stream;
   if (net->desc.network_type == PPB_NET_FEEDFORWARD)
@@ -1735,14 +1750,9 @@ __global__ void __launch_bounds__(256) k_cell_infer(const float* __restrict__ re
       }
       pre[g] = v;
     }
-    float ig = ppb_cell_sigmoid(pre[0]);
-    float fg = ppb_cell_sigmoid(pre[1]);
-    float gg = ppb_cell_tanh(pre[2]);
-    float og = ppb_cell_sigmoid(pre[3]);
-    float cp = first ? 0.0f : c[i * H + j];
-    float cn = fg * cp + ig * gg;
-    c[i * H + j] = cn;
-    h[i * H + j] = og * ppb_cell_tanh(cn);
+    const CellFwd u = cell_fwd_unit(pre, [&] { return first ? 0.0f : c[i * H + j]; });
+    c[i * H + j] = u.c;
+    h[i * H + j] = u.h;
   }
 }
 
@@ -1962,7 +1972,7 @@ int ppb_adam_step_dev(float* arena, const float* grad, float* exp_avg, float* ex
 
 int ppb_net_forget_uploads(ppb_net* net) {
   PPB_CHECK_ARG(net, "bad arguments");
-  for (int i = 0; i < (int)(sizeof(net->slot_hash) / sizeof(net->slot_hash[0])); ++i) net->slot_hash[i] = 0;
+  for (int i = 0; i < kNumUploadSlots; ++i) net->slot_hash[i] = 0;
   return PPB_OK;
 }
 
@@ -1984,7 +1994,7 @@ int ppb_ic_embed_observe(ppb_net* net, const float* arena, const float* obs, flo
   PPB_CHECK_ARG(workspace_bytes >= ppb_ic_infer_workspace_bytes(net, n), "workspace too small");
   {
     const int64_t key[2] = {n, 0};
-    forget_on_new_layout(net, net->infer_layout, key, sizeof(key), workspace, 5, 6);
+    forget_on_new_layout(net, net->infer_layout, key, sizeof(key), workspace, kSlotInferSimt, kSlotInferTc);
   }
   cudaStream_t st = (cudaStream_t)stream;
   InferWs w = carve_infer(net, n, workspace);
@@ -1994,7 +2004,7 @@ int ppb_ic_embed_observe(ppb_net* net, const float* arena, const float* obs, flo
   }
   Builder bl;
   obs_fp32_plan_fwd(bl, net->desc, arena, obs, (int)n, w, obs_emb_out);
-  int rc = upload_and_get(net, bl, w.problems, w.max_problems, st, 5);
+  int rc = upload_and_get(net, bl, w.problems, w.max_problems, st, kSlotInferSimt);
   if (rc) return rc;
   for (auto& ph : bl.phases) { rc = run_phase(ph, w.problems, st); if (rc) return rc; }
   return PPB_OK;
@@ -2004,76 +2014,61 @@ int ppb_ic_infer_step(ppb_net* net, const float* arena, const float* obs_emb, in
                       const float* prev_value, int32_t cur_addr, const float* prior0, int prior0_stride,
                       const float* prior1, int prior1_stride, float* h, float* c, float* params_out, int64_t n,
                       void* workspace, int64_t workspace_bytes, int precision, void* stream) {
-  const bool ff = net && net->desc.network_type == PPB_NET_FEEDFORWARD;
-  PPB_CHECK_ARG(net && arena && obs_emb && (ff || (h && c)) && params_out && workspace && n > 0, "bad arguments");
+  PPB_CHECK_ARG(net && arena && obs_emb && params_out && workspace && n > 0, "bad arguments");
   PPB_CHECK_ARG(cur_addr >= 0 && cur_addr < (int)net->addrs.size(), "unknown current address");
   PPB_CHECK_ARG(workspace_bytes >= ppb_ic_infer_workspace_bytes(net, n), "workspace too small");
-  {
-    const int64_t key[2] = {n, 1};
-    forget_on_new_layout(net, net->infer_layout, key, sizeof(key), workspace, 5, 6);
-  }
-  if (ff) {
-    if (obs_emb_row_stride != 0) {
-      ppb_set_error("ppb_ic_infer_step: per-particle observation embeddings are not supported yet (stride must be 0)");
-      return PPB_ENOTSUP;
-    }
-    // inference_network_feedforward.py:53-66: the head of the current address on the observation embedding.  With one
-    // shared observation every particle's head output is the same: ONE row, expanded over the particles by k_head_params
-    // (row stride 0), which applies each particle's prior.
-    const ppb_net_desc& D = net->desc;
-    cudaStream_t st = (cudaStream_t)stream;
-    InferWs w = carve_infer(net, n, workspace);
-    const ppb_addr_desc cur = net->addrs[cur_addr];
-    const int E = D.obs_dim;
-    Builder bl;
-    bl.begin();
-    bl.add(linear_fwd(obs_emb, E, arena + cur.w1_off, E, arena + cur.b1_off, w.hid, net->dh_pad, 1, cur.head_hidden, E, gemm::kRelu));
-    bl.begin();
-    bl.add(linear_fwd(w.hid, net->dh_pad, arena + cur.w2_off, cur.head_hidden, arena + cur.b2_off, w.out_raw, net->out_pad, 1,
-                      cur.head_out, cur.head_hidden, 0));
-    int rc = upload_and_get(net, bl, w.problems, w.max_problems, st, 5);
-    if (rc) return rc;
-    rc = run_phase(bl.phases[0], w.problems, st); if (rc) return rc;
-    rc = run_phase(bl.phases[1], w.problems, st); if (rc) return rc;
-    k_head_params<<<ew_grid(n, 128), 128, 0, st>>>(w.out_raw, 0, cur, D.mixture_k, prior0, prior0_stride, prior1, prior1_stride,
-                                                   params_out, n);
-    PPB_LAUNCH_CHECK();
-    return PPB_OK;
-  }
-  PPB_CHECK_ARG(prev_addr < (int)net->addrs.size(), "unknown previous address");
-  PPB_CHECK_ARG(prev_addr < 0 || prev_value, "previous value missing");
   if (obs_emb_row_stride != 0) {
     ppb_set_error("ppb_ic_infer_step: per-particle observation embeddings are not supported yet (stride must be 0)");
     return PPB_ENOTSUP;
   }
-  (void)precision;
+  const bool lstm = net->desc.network_type != PPB_NET_FEEDFORWARD;
+  if (lstm) {
+    PPB_CHECK_ARG(h && c, "bad arguments");
+    PPB_CHECK_ARG(prev_addr < (int)net->addrs.size(), "unknown previous address");
+    PPB_CHECK_ARG(prev_addr < 0 || prev_value, "previous value missing");
+  }
+  {
+    const int64_t key[2] = {n, 1};
+    forget_on_new_layout(net, net->infer_layout, key, sizeof(key), workspace, kSlotInferSimt, kSlotInferTc);
+  }
   const ppb_net_desc& D = net->desc;
   cudaStream_t st = (cudaStream_t)stream;
   InferWs w = carve_infer(net, n, workspace);
   const int H = D.lstm_dim, H4 = 4 * H, E = D.obs_dim, S = D.sample_dim, I = net->I, C2 = 2 * (D.type_dim + D.addr_dim);
   const ppb_addr_desc cur = net->addrs[cur_addr];
   const bool first = prev_addr < 0;
-  const ppb_addr_desc prev = first ? cur : net->addrs[prev_addr];
+  // The head reads the LSTM output h after the cell update, n rows.  The feed-forward head reads the observation embedding
+  // (inference_network_feedforward.py:53-66); with one shared observation every particle's head output is the same, so it
+  // runs on ONE row and k_head_params expands it over the particles (row stride 0), applying each particle's prior.
+  const float* x = lstm ? h : obs_emb;
+  const int x_dim = lstm ? H : E, head_rows = lstm ? (int)n : 1, out_stride = lstm ? net->out_pad : 0;
+  // large LSTM GEMMs on the tensor cores (weight images must be current: ppb_net_refresh_weights / ppb_ic_embed_observe)
+  const bool use_tc = lstm && precision != PPB_PREC_FP32_SIMT && (H % 32 == 0) && net->wimg != nullptr;
 
+  // One phase per GEMM, at the same index in both problem lists.  The p_row GEMMs run on the CUDA cores; the recurrent and
+  // head GEMMs go to the tensor-core list when use_tc, else to the SIMT list.
+  enum { kPRowStep, kPRowObs, kRecurrent, kHeadHidden, kHeadOut };
   Builder bl;
-  bl.begin();  // 0: p_row = step_emb W_ih[:, E+S:]^T + b_ih
-  bl.add(linear_fwd(w.emb_row, C2, arena + D.w_ih_off + E + S, I, arena + D.b_ih_off, w.p_row, H4, 1, H4, C2, 0));
-  bl.begin();  // 1: p_row += obs_emb W_ih[:, :E]^T + b_hh   (one shared observation row)
-  bl.add(linear_fwd(obs_emb, E, arena + D.w_ih_off, I, arena + D.b_hh_off, w.p_row, H4, 1, H4, E, gemm::kAccumulate));
-  bl.begin();  // 2: recurrent part
-  if (!first) bl.add(linear_fwd(h, H, arena + D.w_hh_off, H, nullptr, w.gates, H4, (int)n, H4, H, 0));
-  bl.begin();  // 3, 4: head (after the cell update)
-  bl.add(linear_fwd(h, H, arena + cur.w1_off, H, arena + cur.b1_off, w.hid, net->dh_pad, (int)n, cur.head_hidden, H, gemm::kRelu));
-  bl.begin();
-  bl.add(linear_fwd(w.hid, net->dh_pad, arena + cur.w2_off, cur.head_hidden, arena + cur.b2_off, w.out_raw, net->out_pad,
-                    (int)n, cur.head_out, cur.head_hidden, 0));
-  int rc = upload_and_get(net, bl, w.problems, w.max_problems, st, 5);
+  bl.begin();  // kPRowStep: p_row = step_emb W_ih[:, E+S:]^T + b_ih
+  if (lstm) bl.add(linear_fwd(w.emb_row, C2, arena + D.w_ih_off + E + S, I, arena + D.b_ih_off, w.p_row, H4, 1, H4, C2, 0));
+  bl.begin();  // kPRowObs: p_row += obs_emb W_ih[:, :E]^T + b_hh   (one shared observation row)
+  if (lstm) bl.add(linear_fwd(obs_emb, E, arena + D.w_ih_off, I, arena + D.b_hh_off, w.p_row, H4, 1, H4, E, gemm::kAccumulate));
+  bl.begin();  // kRecurrent
+  if (lstm && !first && !use_tc) bl.add(linear_fwd(h, H, arena + D.w_hh_off, H, nullptr, w.gates, H4, (int)n, H4, H, 0));
+  bl.begin();  // kHeadHidden
+  if (!use_tc)
+    bl.add(linear_fwd(x, x_dim, arena + cur.w1_off, x_dim, arena + cur.b1_off, w.hid, net->dh_pad, head_rows, cur.head_hidden,
+                      x_dim, gemm::kRelu));
+  bl.begin();  // kHeadOut
+  if (!use_tc)
+    bl.add(linear_fwd(w.hid, net->dh_pad, arena + cur.w2_off, cur.head_hidden, arena + cur.b2_off, w.out_raw, net->out_pad,
+                      head_rows, cur.head_out, cur.head_hidden, 0));
+  int rc = upload_and_get(net, bl, w.problems, w.max_problems, st, kSlotInferSimt);
   if (rc) return rc;
-  // large GEMMs on the tensor cores (weight images must be current: ppb_net_refresh_weights / ppb_ic_embed_observe)
-  const bool use_tc = precision != PPB_PREC_FP32_SIMT && (H % 32 == 0) && net->wimg != nullptr;
   TcBuilder tb;
   if (use_tc) {
-    tb.begin();  // 0: recurrent
+    tb.begin(); tb.begin();  // kPRowStep, kPRowObs: SIMT list only
+    tb.begin();  // kRecurrent
     if (!first) {
       tcg::Problem p = TP0();
       p.a = op_k(w.h_img.k_hi, w.h_img.k_lo, (int)w.h_img.kb, 0, 0);
@@ -2081,7 +2076,7 @@ int ppb_ic_infer_step(ppb_net* net, const float* arena, const float* obs_emb, in
       p.M = (int)n; p.N = H4; p.K = H; p.c = w.gates; p.ldc = H4;
       tb.add(p);
     }
-    tb.begin();  // 1: head trunk -> hid image
+    tb.begin();  // kHeadHidden: head trunk -> hid image
     {
       tcg::Problem p = TP0();
       p.a = op_k(w.h_img.k_hi, w.h_img.k_lo, (int)w.h_img.kb, 0, 0);
@@ -2091,7 +2086,7 @@ int ppb_ic_infer_step(ppb_net* net, const float* arena, const float* obs_emb, in
       p.o_k_hi = w.hid_img.k_hi; p.o_k_lo = w.hid_img.k_lo; p.o_kb = (int)w.hid_img.kb;
       tb.add(p);
     }
-    tb.begin();  // 2: head output
+    tb.begin();  // kHeadOut
     {
       tcg::Problem p = TP0();
       p.a = op_k(w.hid_img.k_hi, w.hid_img.k_lo, (int)w.hid_img.kb, 0, 0);
@@ -2100,39 +2095,42 @@ int ppb_ic_infer_step(ppb_net* net, const float* arena, const float* obs_emb, in
       p.bias = arena + cur.b2_off; p.c = w.out_raw; p.ldc = net->out_pad;
       tb.add(p);
     }
-    rc = upload_cached(net, 6, tb.probs.data(), tb.probs.size() * sizeof(tcg::Problem), w.tprobs, st);
+    rc = upload_cached(net, kSlotInferTc, tb.probs.data(), tb.probs.size() * sizeof(tcg::Problem), w.tprobs, st);
     if (rc) return rc;
   }
   const dim3 pack_grid((unsigned)((n + 127) / 128), 4);
-  k_step_row_infer<<<1, 128, 0, st>>>(arena, prev, first ? 0 : 1, cur, net->d_type_off, D.type_dim, D.addr_dim, w.emb_row);
-  PPB_LAUNCH_CHECK();
-  rc = run_phase(bl.phases[0], w.problems, st); if (rc) return rc;
-  rc = run_phase(bl.phases[1], w.problems, st); if (rc) return rc;
-  if (!first) {
-    k_wsmp_transpose<<<ew_grid(S * H4), 256, 0, st>>>(arena + D.w_ih_off, I, E, S, H4, w.w_smp_t);
+  if (lstm) {
+    const ppb_addr_desc prev = first ? cur : net->addrs[prev_addr];
+    k_step_row_infer<<<1, 128, 0, st>>>(arena, prev, first ? 0 : 1, cur, net->d_type_off, D.type_dim, D.addr_dim, w.emb_row);
     PPB_LAUNCH_CHECK();
-    k_smp_embed_infer<<<ew_grid(n * S), 256, 0, st>>>(arena, prev, prev_value, n, S, w.smp_emb);
-    PPB_LAUNCH_CHECK();
-    if (use_tc) {
-      k_pack_rows<<<pack_grid, 256, 0, st>>>(h, (int)n, H, H, w.h_img);
+    rc = run_phase(bl.phases[kPRowStep], w.problems, st); if (rc) return rc;
+    rc = run_phase(bl.phases[kPRowObs], w.problems, st); if (rc) return rc;
+    if (!first) {
+      k_wsmp_transpose<<<ew_grid(S * H4), 256, 0, st>>>(arena + D.w_ih_off, I, E, S, H4, w.w_smp_t);
       PPB_LAUNCH_CHECK();
-      rc = run_tc_phase<0>(tb.phases[0], w.tprobs, precision, st); if (rc) return rc;
-    } else {
-      rc = run_phase(bl.phases[2], w.problems, st); if (rc) return rc;
+      k_smp_embed_infer<<<ew_grid(n * S), 256, 0, st>>>(arena, prev, prev_value, n, S, w.smp_emb);
+      PPB_LAUNCH_CHECK();
+      if (use_tc) {
+        k_pack_rows<<<pack_grid, 256, 0, st>>>(h, (int)n, H, H, w.h_img);
+        PPB_LAUNCH_CHECK();
+        rc = run_tc_phase<0>(tb.phases[kRecurrent], w.tprobs, precision, st); if (rc) return rc;
+      } else {
+        rc = run_phase(bl.phases[kRecurrent], w.problems, st); if (rc) return rc;
+      }
     }
+    k_cell_infer<<<ew_grid(n * H), 256, 0, st>>>(w.gates, w.p_row, w.w_smp_t, w.smp_emb, c, h, n, H, S, first ? 1 : 0);
+    PPB_LAUNCH_CHECK();
   }
-  k_cell_infer<<<ew_grid(n * H), 256, 0, st>>>(w.gates, w.p_row, w.w_smp_t, w.smp_emb, c, h, n, H, S, first ? 1 : 0);
-  PPB_LAUNCH_CHECK();
   if (use_tc) {
     k_pack_rows<<<pack_grid, 256, 0, st>>>(h, (int)n, H, H, w.h_img);
     PPB_LAUNCH_CHECK();
-    rc = run_tc_phase<2>(tb.phases[1], w.tprobs, precision, st); if (rc) return rc;
-    rc = run_tc_phase<0>(tb.phases[2], w.tprobs, precision, st); if (rc) return rc;
+    rc = run_tc_phase<2>(tb.phases[kHeadHidden], w.tprobs, precision, st); if (rc) return rc;
+    rc = run_tc_phase<0>(tb.phases[kHeadOut], w.tprobs, precision, st); if (rc) return rc;
   } else {
-    rc = run_phase(bl.phases[3], w.problems, st); if (rc) return rc;
-    rc = run_phase(bl.phases[4], w.problems, st); if (rc) return rc;
+    rc = run_phase(bl.phases[kHeadHidden], w.problems, st); if (rc) return rc;
+    rc = run_phase(bl.phases[kHeadOut], w.problems, st); if (rc) return rc;
   }
-  k_head_params<<<ew_grid(n, 128), 128, 0, st>>>(w.out_raw, net->out_pad, cur, D.mixture_k, prior0, prior0_stride, prior1,
+  k_head_params<<<ew_grid(n, 128), 128, 0, st>>>(w.out_raw, out_stride, cur, D.mixture_k, prior0, prior0_stride, prior1,
                                                  prior1_stride, params_out, n);
   PPB_LAUNCH_CHECK();
   return PPB_OK;
